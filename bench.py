@@ -26,6 +26,7 @@ import sys
 import threading
 import time
 
+import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
@@ -82,34 +83,12 @@ def bind_to_gpu_numa_node(local_rank: int):
     return info
 
 
-def ncu_traffic(dtype_name: str):
-    """DRAM traffic (dram__bytes_read.sum + dram__bytes_write.sum) of one op forward / backward, parsed from the committed
-    ncu summary of tools/run_op.py (BASELINE config 2, fp32 or bf16).  Returns None when no capture matches."""
-    fname = "r02_tc_ncu_summary.txt" if dtype_name == "f32" else "r02_tc_ncu_summary_bf16.txt"
-    path = os.path.join(ROOT, "profiles", fname)
-    if not os.path.exists(path):
-        return None
-    units = {"byte": 1.0, "kbyte": 1e3, "mbyte": 1e6, "gbyte": 1e9}
-    tot = {"fwd": 0.0, "bwd": 0.0}
-    cur = None
-    for line in open(path):
-        if line.startswith("Kernel Name"):
-            name = line.split(None, 2)[2]
-            cur = "fwd" if ("stats_kernel" in name or "fwd_kernel" in name) else ("bwd" if "bwd" in name else None)
-        elif cur and (line.startswith("dram__bytes_read.sum") or line.startswith("dram__bytes_write.sum")):
-            f = line.split()
-            tot[cur] += float(f[1].replace(",", "")) * units.get(f[2].lower(), 1.0)
-    if tot["fwd"] == 0.0 or tot["bwd"] == 0.0:
-        return None
-    return {"fwd": tot["fwd"], "bwd": tot["bwd"], "source": "profiles/" + fname}
-
-
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not a measured peak"
 
 
 class ClockSampler:
@@ -243,6 +222,25 @@ def time_events(fn, steps, warmup, barrier=None, finish=None):
     return e0.elapsed_time(e1) / steps          # ms per step
 
 
+DUMP_SAMPLE = 1 << 21          # elements kept of an output too large to store whole (fixed, seeded positions)
+DUMP_WHOLE = 6 << 20           # outputs up to this many elements are stored whole (the total stays under 64 MB)
+
+
+def dump_outputs(path, arrays):
+    """Write what the timed op path returned in its last step (out, lse, dq, dk, dv) as float32 .npy files.  An output of
+    more than DUMP_WHOLE elements is stored as <name>_sample.npy: the flat (memory-order) elements at the sorted first
+    DUMP_SAMPLE positions of torch.randperm(numel, generator=torch.Generator().manual_seed(0))."""
+    os.makedirs(path, exist_ok=True)
+    for name, t in arrays.items():
+        flat = t.detach().float().contiguous().view(-1)
+        if flat.numel() > DUMP_WHOLE:
+            gen = torch.Generator().manual_seed(0)
+            idx = torch.randperm(flat.numel(), generator=gen)[:DUMP_SAMPLE].sort().values
+            flat = flat[idx.to(flat.device)]
+            name = f"{name}_sample"
+        np.save(os.path.join(path, f"{name}.npy"), flat.cpu().numpy().astype(np.float32))
+
+
 def run_ours(args):
     import torch.distributed as dist
     rank, local_rank, world = dist_env()
@@ -255,7 +253,7 @@ def run_ours(args):
         dist.init_process_group("nccl", device_id=dev)
     from ccnet_b200 import RCCA, capi, cca_backward, cca_forward
     lib = capi.load()
-    assert lib.cca_b200_device_ok() == 1, "not an sm_100 device"
+    assert lib.cca_b200_device_ok() == 1, "not an sm_90 device"
 
     B, C, H, W, R = CFG["B"], CFG["C"], CFG["H"], CFG["W"], CFG["R"]
     Cq = C // 8
@@ -367,10 +365,13 @@ def run_ours(args):
         q, k, v, do = (t.contiguous(memory_format=torch.channels_last) for t in (q, k, v, do))
     op_layout = "channels_last" if not q.is_contiguous() else "nchw"
 
+    last = {}
+
     def step_op():                                  # R sequential op applications, forward + backward
         for _ in range(R):
             out, lse = cca_forward(q, k, v, impl=args.kernels)
-            cca_backward(do, q, k, v, out, lse, impl=args.kernels)
+            dq, dk, dv = cca_backward(do, q, k, v, out, lse, impl=args.kernels)
+        last.update(out=out, lse=lse, dq=dq, dk=dk, dv=dv)
 
     # ---- main timed region: op level, resident ------------------------------------------------------
     n0 = capi.launch_count()
@@ -378,6 +379,8 @@ def run_ours(args):
         ms = time_events(step_op, args.steps, args.warmup, barrier)
     launches = (capi.launch_count() - n0) * args.steps // (args.steps + args.warmup)
     ms = max_over_ranks(ms)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     px = B * H * W * world
     value = px / (ms * 1e-3)
 
@@ -385,7 +388,7 @@ def run_ours(args):
     ms_mod = max_over_ranks(time_events(step_resident, max(3, args.steps // 2), 3, barrier))
     module = {"value": px / (ms_mod * 1e-3), "unit": UNIT, "ms_per_step": ms_mod,
               "note": "CrissCrossAttention nn.Module x R fwd+bwd, x resident (NCHW in, converted once per call); projections, "
-                      "attention and their backward all on this repository's tcgen05 kernels (one autograd node per step)"}
+                      "attention and their backward all on this repository's wgmma kernels (one autograd node per step)"}
     ms_e2e_serial = max_over_ranks(time_events(step_e2e, max(3, args.steps // 2), 3, barrier))
     ms_e2e = max_over_ranks(time_events(step_e2e_pipelined, max(6, args.steps // 2), 4, barrier, finish=join_streams))
     e2e = {"value": px / (ms_e2e * 1e-3), "unit": UNIT, "ms_per_step": ms_e2e,
@@ -400,7 +403,7 @@ def run_ours(args):
 
     # ---- per-op timings of the kernels of this repo -> roofline ----------------------------------------
     out, lse = cca_forward(q, k, v, impl=args.kernels)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)      # > L2 (126 MB)
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)      # > L2 (50 MB on an H100)
 
     def op_time(fn, iters=10):
         ts = []
@@ -430,16 +433,9 @@ def run_ours(args):
     dom_is_bwd = b_avg >= f_avg
     dom_bytes, dom_ms = (bytes_b, b_avg) if dom_is_bwd else (bytes_f, f_avg)
     ach = dom_bytes / (dom_ms * 1e-3) / 1e9
-    # DRAM traffic of one op call: parsed from the committed ncu --set full summary of tools/run_op.py (same shape / dtype)
-    traffic = None
-    if (B, C, H, W) == (8, 512, 97, 97) and op_layout == "channels_last":
-        traffic = ncu_traffic("f32" if dtype == torch.float32 else "bf16")
     roofline = {"bound": "hbm", "kernel": "cca backward op (prep + one persistent item kernel)" if dom_is_bwd
                 else "cca forward op (statistics pre-pass + values kernel)",
                 "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                "traffic": (traffic["bwd" if dom_is_bwd else "fwd"] if traffic else None),
-                "traffic_fwd": traffic["fwd"] if traffic else None, "traffic_bwd": traffic["bwd"] if traffic else None,
-                "traffic_source": (traffic["source"] + " (ncu --set full; sum over the launches of one op call)") if traffic else None,
                 "peak_source": peak_src, "launches_per_op": nb if dom_is_bwd else nf,
                 "op_fwd": {"ms": f_avg, "ms_min": f_min, "alg_bytes": bytes_f, "gbs": bytes_f / f_avg / 1e6,
                            "frac": bytes_f / f_avg / 1e6 / peak, "launches": nf},
@@ -498,7 +494,7 @@ def run_ours(args):
                 "vs_baseline": None, "dtype": "f32" if dtype == torch.float32 else "bf16", "data": "synthetic",
                 "config": {"workload": workload_name(), "global_batch": B * world, "kernels": args.kernels,
                            "op_layout": op_layout,
-                           "l2": "inputs larger than L2: one op fwd+bwd touches q,k,v,dout,out,dq,dk,dv = 1.04 GB vs 126 MB "
+                           "l2": "inputs larger than L2: one op fwd+bwd touches q,k,v,dout,out,dq,dk,dv = 1.04 GB vs 50 MB "
                                  "L2 (no explicit flush in the timed loop); the per-op roofline timings flush 256 MB explicitly",
                            "parallelism": f"dp{world} (image-sharded, DDP grad all-reduce only)",
                            "host_binding": numa},
@@ -519,6 +515,8 @@ def main():
     ap.add_argument("--kernels", default="auto", choices=["auto", "simt", "tc"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-train", action="store_true", help="skip the ResNet101+RCCA train-step leg (BASELINE configs[2], [3])")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the op outputs of the last timed step (out, lse, dq, dk, dv; large ones as a seeded sample) as .npy")
     args = ap.parse_args()
     args.warmup = max(3, args.warmup)
     if args.impl == "reference":

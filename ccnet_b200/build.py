@@ -1,6 +1,6 @@
-"""Build the C-ABI shared library ``ccnet_b200/lib/libcca_b200.so`` with nvcc for sm_100a.
+"""Build the C-ABI shared library ``ccnet_b200/lib/libcca_b200.so`` with nvcc for sm_90a.
 
-In-tree build (the .so is git-ignored but travels to the GPU box with the gpurun snapshot).
+In-tree build (the .so is git-ignored; build() recompiles it).
 ``python -m ccnet_b200.build [--force]``
 """
 from __future__ import annotations
@@ -12,12 +12,12 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-LIBDIR = os.environ.get("CCA_B200_LIBDIR") or os.path.join(HERE, "lib")      # (override: a second, profiling flavour)
+LIBDIR = os.environ.get("CCA_B200_LIBDIR") or os.path.join(HERE, "lib")      # (override: a second build flavour)
 LIB = os.path.join(LIBDIR, "libcca_b200.so")
 SOURCES = ["cca_capi.cu", "cca_simt.cu", "cca_tc_host.cu", "cca_tc_stats.cu", "cca_tc_fwd.cu", "cca_tc_bwd.cu", "cca_gemm.cu"]
-HEADERS = ["cca_common.cuh", "cca_sm100.cuh", "cca_tc_common.cuh", "cca_items.cuh", "../../include/cca_b200.h"]
+HEADERS = ["cca_common.cuh", "cca_sm90.cuh", "cca_tc_common.cuh", "cca_items.cuh", "../../include/cca_b200.h"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo", "--use_fast_math",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
 ]
@@ -41,13 +41,12 @@ DEBUG_FLAGS = ["-DCCA_SPIN_TRAP=1", "-DCCA_DEBUG_HOOKS"]   # bounded spins that 
 
 
 def build(force: bool = False, verbose: bool = False, debug: bool | None = None) -> str:
-    """Release build by default; ``debug=True`` / ``--debug`` / CCA_B200_DEBUG_BUILD=1 adds DEBUG_FLAGS
-    (and ``--timeline`` / CCA_B200_TIMELINE=1 the in-kernel clock stamps).  The flavour is recorded in lib/flavour.txt;
-    changing it rebuilds everything."""
+    """Release build by default; ``debug=True`` / ``--debug`` / CCA_B200_DEBUG_BUILD=1 adds DEBUG_FLAGS.  The flavour is
+    recorded in lib/flavour.txt; changing it rebuilds everything."""
     os.makedirs(LIBDIR, exist_ok=True)
     if debug is None:
         debug = bool(os.environ.get("CCA_B200_DEBUG_BUILD"))
-    flavour_flags = (DEBUG_FLAGS if debug else []) + (["-DCCA_TIMELINE"] if os.environ.get("CCA_B200_TIMELINE") else [])
+    flavour_flags = DEBUG_FLAGS if debug else []
     stamp = os.path.join(LIBDIR, "flavour.txt")
     flavour = " ".join(flavour_flags) or "release"
     if not os.path.exists(stamp) or open(stamp).read() != flavour:
@@ -82,6 +81,4 @@ def build(force: bool = False, verbose: bool = False, debug: bool | None = None)
 
 
 if __name__ == "__main__":
-    if "--timeline" in sys.argv:
-        os.environ["CCA_B200_TIMELINE"] = "1"
     print(build(force="--force" in sys.argv, verbose="-v" in sys.argv, debug=True if "--debug" in sys.argv else None))

@@ -77,10 +77,7 @@ extern "C" {
 
 int cca_b200_version(void) { return CCA_B200_VERSION; }
 #ifdef CCA_DEBUG_HOOKS
-// A/B and profiling aids of debug builds (`python -m ccnet_b200.build --debug`); not part of the ABI, absent from release builds
-CCA_API void cca_b200__set_debug_buffer(void *p) { set_tc_debug_buffer(p); }
-CCA_API void cca_b200__set_bwd_debug_buffer(void *p) { set_tc_bwd_debug_buffer(p); }
-CCA_API void cca_b200__set_stats_debug_buffer(void *p) { set_tc_stats_debug_buffer(p); }
+// A/B aids of debug builds (`python -m ccnet_b200.build --debug`); not part of the ABI, absent from release builds
 CCA_API void cca_b200__set_pdl(int on) { set_tc_pdl(on); }
 CCA_API void cca_b200__set_zero_ahead(int n) { set_tc_zero_ahead(n); }
 CCA_API void cca_b200__set_delta_mode(int m) { set_tc_delta_mode(m); }
@@ -96,7 +93,7 @@ const char *cca_b200_strerror(int s)
         case CCA_ERR_UNSUPPORTED: return "unsupported shape";
         case CCA_ERR_WORKSPACE: return "workspace too small";
         case CCA_ERR_CUDA: return "CUDA error";
-        case CCA_ERR_DEVICE: return "device is not sm_100";
+        case CCA_ERR_DEVICE: return "device is not sm_90";
         default: return "unknown status";
     }
 }
@@ -123,7 +120,7 @@ int check_device()
 {
     const int major = device_major();
     if (major == 0) return fail(CCA_ERR_CUDA, "cannot query the current CUDA device%s%s");
-    if (major != 10) return fail(CCA_ERR_DEVICE, "the current device is not sm_100 (B200); this library has no other code path%s%s");
+    if (major != 9) return fail(CCA_ERR_DEVICE, "the current device is not sm_90 (H100); this library has no other code path%s%s");
     return CCA_OK;
 }
 }  // namespace
@@ -135,14 +132,14 @@ int cca_b200_device_ok(void)
     if (e != cudaSuccess) return cuda_fail(e, "cudaGetDevice");
     e = cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
     if (e != cudaSuccess) return cuda_fail(e, "cudaDeviceGetAttribute");
-    return major == 10 ? 1 : 0;
+    return major == 9 ? 1 : 0;
 }
 
 int cca_b200_tc_supported(int which, int B, int Cq, int C, int H, int W, int dtype)
 {
     if (check_dims(B, Cq, C, H, W, dtype)) return 0;
     int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && device_major() != 10) return 0;   // (no device at all: shape answer only)
+    if (cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && device_major() != 9) return 0;   // (no device at all: shape answer only)
     const Dims d{B, Cq, C, H, W};
     return (which == CCA_WS_BACKWARD ? tc_backward_supported(d, dtype) : tc_forward_supported(d, dtype)) ? 1 : 0;
 }
@@ -254,7 +251,7 @@ int cca_b200_qkv_supported(int C, int Cq)
 {
     if (C <= 0 || Cq <= 0) return 0;
     int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && device_major() != 10) return 0;
+    if (cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && device_major() != 9) return 0;
     return qkv_gemm_supported(C, Cq) ? 1 : 0;
 }
 size_t cca_b200_qkv_workspace_bytes(int C, int Cq) { return C > 0 && Cq > 0 ? qkv_gemm_workspace(C, Cq) : 0; }
@@ -318,7 +315,7 @@ int cca_b200_qkv_wgrad_supported(int C, int Cq)
 {
     if (C <= 0 || Cq <= 0) return 0;
     int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && device_major() != 10) return 0;
+    if (cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && device_major() != 9) return 0;
     return qkv_wgrad_supported(C, Cq) ? 1 : 0;
 }
 

@@ -1,4 +1,4 @@
-// Shared declarations for the criss-cross attention kernels (sm_100a).
+// Shared declarations for the criss-cross attention kernels (sm_90a).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -52,7 +52,7 @@ size_t tc_backward_workspace(Dims d);
 cudaError_t tc_backward(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
                         void *dq, void *dk, void *dv, void *ws, Dims d, int dtype, cudaStream_t st, const char **why);
 
-// tcgen05 GEMMs of the 1x1 Q/K/V projections (cca_gemm.cu), fp32 channels-last tensors as [pixels, channels] matrices
+// wgmma GEMMs of the 1x1 Q/K/V projections (cca_gemm.cu), fp32 channels-last tensors as [pixels, channels] matrices
 bool qkv_gemm_supported(int C, int Cq);
 size_t qkv_gemm_workspace(int C, int Cq);
 cudaError_t qkv_project(const float *x, const float *wq, const float *bq, const float *wk, const float *bk, const float *wv, const float *bv,
@@ -82,9 +82,6 @@ void set_tc_zero_ahead(int n);
 void set_tc_delta_mode(int m);
 void set_tc_lag(int v);
 void set_tc_l2_hints(int v);
-void set_tc_debug_buffer(void *p);
-void set_tc_bwd_debug_buffer(void *p);
-void set_tc_stats_debug_buffer(void *p);
 #endif
 
 }  // namespace cca

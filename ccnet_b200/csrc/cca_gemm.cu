@@ -1,260 +1,134 @@
-// tcgen05 / TMA GEMMs for the 1x1 Q/K/V projections around the operator (cc_attention/functions.py:29,32,35 and their
-// input gradient), channels-last fp32 tensors seen as row-major [pixels, channels] matrices:
+// wgmma GEMMs for the 1x1 Q/K/V projections around the operator (cc_attention/functions.py:29,32,35 and their gradients),
+// channels-last fp32 tensors seen as row-major [pixels, channels] matrices:
 //   forward :  [q | k | v](P x (2Cq+C))  =  x(P x C) . [Wq; Wk; Wv]^T + [bq | bk | bv]
 //   dgrad   :  dx(P x C)                 =  [dq | dk | dv](P x (2Cq+C)) . [Wq; Wk; Wv]
+//   wgrad   :  dW[n][k] = scale * sum_p G[p][n] x[p][k],  db[n] = scale * sum_p G[p][n]      (G = [dq | dk | dv])
 // fp32 accuracy on the bf16 tensor pipe with the same split the attention kernels use: every operand is hi + lo in bf16
-// (x = hi + lo to ~2^-17), every product three MMAs (hi*hi + hi*lo + lo*hi), fp32 accumulation in TMEM.
+// (x = hi + lo to ~2^-17), every product three MMAs (hi*hi + hi*lo + lo*hi), fp32 accumulation in registers.
 //
-// One generic kernel: D[128-pixel tile, N tile] = sum over 32-channel stages of A_stage . B_stage^T
-//   A (activations) : TMA 2-D boxes [128 px][32 ch] fp32 (SWIZZLE_128B) from up to three source tensors, split in place by the
-//                     converter warps into UMMA canonical K-major planes [8-channel chunk][pixel][16 B] (hi planes, lo planes)
-//   B (weights)     : split ONCE per call by a small pack kernel into exactly those planes, one contiguous block per
-//                     (N tile, stage); a stage is one cp.async.bulk
-//   D               : TMEM, two accumulator buffers of up to 256 columns; epilogue adds the bias, stages [128 px][64 ch]
-//                     tiles and TMA-stores them into up to three destination tensors (q, k, v are separate tensors)
-// Persistent grid, tiles (pixel block, N tile) round-robin; N tiles of one pixel block run on neighbouring CTAs at the same
-// time, so the activation tile is fetched from DRAM once and from L2 otherwise.
-// Warp roles (512 threads): 0-3 epilogue (TMEM lane == pixel), 4-11 converters, 12 TMA producer, 13 MMA issuer, 14 store.
+// forward / dgrad: one work unit = (128-pixel block, 64-column chunk), persistent grid; per 32-channel stage the 256 threads load
+// the activation tile, split it into K-major planes [8-channel chunk][pixel][16 B] in shared memory, copy the chunk's packed
+// weight planes (split ONCE per call by the pack kernel), and two warpgroups (64 pixels each) issue m64n64k16 wgmmas.
 #include "cca_tc_common.cuh"
 
 namespace cca {
 namespace {
 using namespace tc;
 
-constexpr int kGThreads = 512;
-constexpr int kGM = 128;               // pixels per tile (UMMA M)
-constexpr int kGK = 32;                // channels per stage: one SWIZZLE_128B fp32 TMA tile
-constexpr int kGNMax = 256;            // widest N tile (UMMA N)
-constexpr int kATile = kGM * 128;      // 16 KB
+constexpr int kGThreads = 256;
+constexpr int kGM = 128;               // pixels per unit (two warpgroups of 64)
+constexpr int kGK = 32;                // channels per stage
 constexpr int kAPlane = kGM * 16;      // 2 KB: 8 channels x 128 pixels (bf16)
-constexpr int kNA = 4, kNB = 3, kNStg = 2;
-constexpr int kBSlot = 128 * kGNMax;   // 32 KB: [hi | lo][4 planes][N rows][16 B]
-constexpr int kStg = 2 * kATile;       // staging tile [128 px][64 ch] fp32 = two swizzled 32-channel tiles
-constexpr int kGWConv0 = 4, kGWProducer = 12, kGWMma = 13, kGWStore = 14;
+constexpr int kBPlane = 64 * 16;       // 1 KB: 8 channels x 64 weight rows
 constexpr int kMaxStages = 32, kMaxTiles = 4, kMaxChunks = 16;
 
 struct GemmParams {
     int P;                          // rows (pixels)
     int n_stages;                   // K / 32
-    int stage_seg[kMaxStages];      // source map of the stage (0..2)
+    int stage_seg[kMaxStages];      // source tensor of the stage (0..2)
     int stage_c0[kMaxStages];       // channel offset inside that tensor
-    int n_tiles;                    // N tiles per pixel block
+    int n_tiles;                    // N tiles of the packed weights
     int tile_n[kMaxTiles];          // width (multiple of 64, <= 256)
     int tile_chunk0[kMaxTiles];     // first 64-column chunk of the tile
     long tile_woff[kMaxTiles];      // byte offset of the tile's first weight block in wblocks
-    int chunk_seg[kMaxChunks];      // destination map of each 64-column chunk (0..2)
+    int n_chunks;
+    int chunk_seg[kMaxChunks];      // destination tensor of each 64-column chunk (0..2)
     int chunk_c0[kMaxChunks];       // channel offset inside that tensor
+    const float *a[3];
+    int ach[3];
+    float *o[3];
+    int och[3];
     const uint8_t *wblocks;         // packed weights
     const float *bias;              // packed bias (nullptr: none)
-    int accumulate;                 // 1: add onto the destination (TMA reduce-add) instead of storing
+    int accumulate;                 // 1: add onto the destination instead of storing
 };
 
-struct GemmSmem {
-    static constexpr int off_a = 0;
-    static constexpr int off_b = off_a + kNA * kATile;
-    static constexpr int off_stg = off_b + kNB * kBSlot;
-    static constexpr int off_bar = off_stg + kNStg * kStg;
-    static constexpr int kBytes = off_bar + 8 * 32 + 16;
-    static_assert(kBytes <= 232448, "shared memory budget");
-};
-enum { G_A_FULL = 0, G_A_OP = 4, G_A_EMPTY = 8, G_B_FULL = 12, G_B_EMPTY = 15, G_ACC_FULL = 18, G_ACC_EMPTY = 20,
-       G_STG_FREE = 22, G_STAGED = 24, G_COUNT = 26 };
-
-// fp32 tile [128 px][32 ch] (SWIZZLE_128B) -> bf16 hi / lo planes [4 hi | 4 lo][128 px][16 B], in place.  256 threads:
-// two per pixel row, 16 channels each; all read, meet on named barrier 1, then overwrite.
-__device__ __forceinline__ void convert_tile32_inplace(uint8_t *tile, int t)
+// smem: A planes [hi 4 | lo 4] x 2 KB, B planes [hi 4 | lo 4] x 1 KB
+__global__ void __launch_bounds__(kGThreads, 1) cca_gemm_kernel(const __grid_constant__ GemmParams p)
 {
-    const int r = t & 127, half = t >> 7, sw = r & 7;
-    float4 raw[4];
+    __shared__ __align__(1024) uint8_t sa[8 * kAPlane];
+    __shared__ __align__(1024) uint8_t sb[8 * kBPlane];
+    const int t = threadIdx.x, wg = t >> 7, wq = (t >> 5) & 3, lane = t & 31;
+    const int rbase = 64 * wg + 16 * wq + (lane >> 2), cq = 2 * (lane & 3);
+    pdl_wait();                                                     // the pack kernel's weights
+    const int nblk = (p.P + kGM - 1) / kGM, units = nblk * p.n_chunks;
+    for (int u = blockIdx.x; u < units; u += gridDim.x) {
+        const int blk = u / p.n_chunks, chunk = u - blk * p.n_chunks;
+        int tile = 0;
+        while (tile + 1 < p.n_tiles && p.tile_chunk0[tile + 1] <= chunk) ++tile;
+        const int N = p.tile_n[tile], cin = chunk - p.tile_chunk0[tile];
+        const long row0 = (long)blk * kGM;
+        float acc[32];
+        for (int s = 0; s < p.n_stages; ++s) {
+            // A: thread = (pixel row t & 127, 16-channel half t >> 7)
+            {
+                const int r = t & 127, hq = t >> 7;
+                const long row = row0 + r;
+                const int seg = p.stage_seg[s];
+                float v[16];
+                if (row < p.P) {
+                    const float4 *src = reinterpret_cast<const float4 *>(p.a[seg] + row * p.ach[seg] + p.stage_c0[s] + 16 * hq);
 #pragma unroll
-    for (int j = 0; j < 4; ++j) raw[j] = *reinterpret_cast<const float4 *>(tile + r * 128 + (((half * 4 + j) ^ sw) * 16));
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    uint8_t *dh = tile + r * 16 + half * 2 * kAPlane, *dl = dh + 4 * kAPlane;
+                    for (int j = 0; j < 4; ++j) { const float4 x = __ldg(src + j); v[4 * j] = x.x; v[4 * j + 1] = x.y; v[4 * j + 2] = x.z; v[4 * j + 3] = x.w; }
+                } else {
 #pragma unroll
-    for (int j = 0; j < 2; ++j) {
-        const float4 a = raw[2 * j], b = raw[2 * j + 1];
-        const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-        uint4 hi, lo;
-        split8(v, hi, lo);
-        *reinterpret_cast<uint4 *>(dh + j * kAPlane) = hi;
-        *reinterpret_cast<uint4 *>(dl + j * kAPlane) = lo;
+                    for (int j = 0; j < 16; ++j) v[j] = 0.f;
+                }
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    uint4 hi, lo;
+                    split8(v + 8 * j, hi, lo);
+                    *reinterpret_cast<uint4 *>(sa + (2 * hq + j) * kAPlane + r * 16) = hi;
+                    *reinterpret_cast<uint4 *>(sa + (4 + 2 * hq + j) * kAPlane + r * 16) = lo;
+                }
+            }
+            // B: the chunk's 64 rows of the packed block [hi | lo][4 planes][N rows][16 B]
+            {
+                const uint8_t *blkp = p.wblocks + p.tile_woff[tile] + (long)s * 128 * N;
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int e = t + 256 * i;                     // 512 x 16 B
+                    const int pl = e >> 6, rw = e & 63;
+                    *reinterpret_cast<uint4 *>(sb + pl * kBPlane + rw * 16) =
+                        __ldg(reinterpret_cast<const uint4 *>(blkp + (long)pl * N * 16 + (cin * 64 + rw) * 16));
+                }
+            }
+            fence_proxy_async();
+            __syncthreads();
+            const uint32_t ab = smem_u32(sa) + 64 * wg * 16, bb = smem_u32(sb);
+            wg_fence();
+#pragma unroll
+            for (int ks = 0; ks < 2; ++ks) {
+                const uint64_t ah = smem_desc(ab + ks * 2 * kAPlane, kAPlane, 128), al = smem_desc(ab + (4 + 2 * ks) * kAPlane, kAPlane, 128);
+                const uint64_t bh = smem_desc(bb + ks * 2 * kBPlane, kBPlane, 128), bl = smem_desc(bb + (4 + 2 * ks) * kBPlane, kBPlane, 128);
+                wgmma_ss_n64(acc, ah, bh, s > 0 || ks > 0, 0, 0);
+                wgmma_ss_n64(acc, ah, bl, 1, 0, 0);
+                wgmma_ss_n64(acc, al, bh, 1, 0, 0);
+            }
+            wg_commit();
+            wg_wait<0>();
+            wg_acc_fence<32>(acc);
+            __syncthreads();                                        // the planes are rewritten by the next stage
+        }
+        const int seg = p.chunk_seg[chunk];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const long row = row0 + rbase + 8 * h;
+            if (row >= p.P) continue;
+            float *dst = p.o[seg] + row * p.och[seg] + p.chunk_c0[chunk] + cq;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+                if (p.bias) { x0 += __ldg(p.bias + chunk * 64 + 8 * j + cq); x1 += __ldg(p.bias + chunk * 64 + 8 * j + cq + 1); }
+                float2 *d2 = reinterpret_cast<float2 *>(dst + 8 * j);
+                if (p.accumulate) { const float2 old = *d2; x0 += old.x; x1 += old.y; }
+                *d2 = make_float2(x0, x1);
+            }
+        }
     }
 }
 
-__global__ void __launch_bounds__(kGThreads, 1)
-cca_gemm_kernel(const __grid_constant__ CUtensorMap ma0, const __grid_constant__ CUtensorMap ma1, const __grid_constant__ CUtensorMap ma2,
-                const __grid_constant__ CUtensorMap mo0, const __grid_constant__ CUtensorMap mo1, const __grid_constant__ CUtensorMap mo2,
-                const __grid_constant__ GemmParams p)
-{
-    using S = GemmSmem;
-    extern __shared__ __align__(1024) uint8_t smem[];
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + S::off_bar);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + S::off_bar + 8 * G_COUNT);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int mblocks = (p.P + kGM - 1) / kGM;
-    const int total = mblocks * p.n_tiles;
-    const int nt_cta = total > (int)blockIdx.x ? (total - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
-    auto tile_of = [&](int i, int &mb, int &nt) {
-        const int t = (int)blockIdx.x + i * (int)gridDim.x;
-        mb = t / p.n_tiles; nt = t - mb * p.n_tiles;
-    };
-
-    if (tid == 0) {
-        for (int i = 0; i < kNA; ++i) {
-            mbar_init(&bars[G_A_FULL + i], 1); mbar_init(&bars[G_A_OP + i], 256); mbar_init(&bars[G_A_EMPTY + i], 1);
-        }
-        for (int i = 0; i < kNB; ++i) { mbar_init(&bars[G_B_FULL + i], 1); mbar_init(&bars[G_B_EMPTY + i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&bars[G_ACC_FULL + i], 1); mbar_init(&bars[G_ACC_EMPTY + i], 128); }
-        for (int i = 0; i < kNStg; ++i) { mbar_init(&bars[G_STG_FREE + i], 1); mbar_init(&bars[G_STAGED + i], 128); }
-        fence_mbar_init();
-        prefetch_tmap(&ma0); prefetch_tmap(&ma1); prefetch_tmap(&ma2); prefetch_tmap(&mo0); prefetch_tmap(&mo1); prefetch_tmap(&mo2);
-    }
-    if (warp == 0) tmem_alloc<512>(tmem_slot);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    pdl_wait();                                   // the weight blocks come from the pack kernel launched right before
-
-    if (warp == kGWProducer) {
-        if (lane == 0) {
-            uint32_t ga = 0, gb = 0;
-            for (int i = 0; i < nt_cta; ++i) {
-                int mb, nt;
-                tile_of(i, mb, nt);
-                const uint32_t bbytes = 128u * (uint32_t)p.tile_n[nt];
-                const uint8_t *wsrc = p.wblocks + p.tile_woff[nt];
-                for (int s = 0; s < p.n_stages; ++s, ++ga, ++gb) {
-                    const int a = ga % kNA, b = gb % kNB;
-                    mbar_wait(&bars[G_B_EMPTY + b], ((gb / kNB) & 1) ^ 1);
-                    mbar_expect_tx(&bars[G_B_FULL + b], bbytes);
-                    bulk_load(smem + S::off_b + b * kBSlot, wsrc + (size_t)s * bbytes, bbytes, &bars[G_B_FULL + b]);
-                    mbar_wait(&bars[G_A_EMPTY + a], ((ga / kNA) & 1) ^ 1);
-                    mbar_expect_tx(&bars[G_A_FULL + a], kATile);
-                    const int seg = p.stage_seg[s];
-                    const CUtensorMap *m = seg == 0 ? &ma0 : (seg == 1 ? &ma1 : &ma2);
-                    tma_load_2d(smem + S::off_a + a * kATile, m, &bars[G_A_FULL + a], p.stage_c0[s], mb * kGM);
-                }
-            }
-        }
-    } else if (warp == kGWMma) {
-        uint32_t ga = 0, gb = 0;
-        const uint32_t a_base = smem_u32(smem + S::off_a), b_base = smem_u32(smem + S::off_b);
-        for (int i = 0; i < nt_cta; ++i) {
-            int mb, nt;
-            tile_of(i, mb, nt);
-            const int N = p.tile_n[nt];
-            const uint32_t idesc = instr_desc(kFmtBF16, kFmtBF16, kGM, N, false, false);
-            const uint32_t acc = tmem + (i & 1) * kGNMax;
-            mbar_wait(&bars[G_ACC_EMPTY + (i & 1)], ((i >> 1) & 1) ^ 1);
-            for (int s = 0; s < p.n_stages; ++s, ++ga, ++gb) {
-                const int a = ga % kNA, b = gb % kNB;
-                mbar_wait(&bars[G_A_OP + a], (ga / kNA) & 1);
-                mbar_wait(&bars[G_B_FULL + b], (gb / kNB) & 1);
-                tc_fence_after();
-                const uint32_t ah = a_base + a * kATile, al = ah + 4 * kAPlane;
-                const uint32_t bh = b_base + b * kBSlot, bl = bh + 4 * N * 16;
-                if (elect_one()) {
-#pragma unroll
-                    for (int ks = 0; ks < kGK / 16; ++ks) {
-                        const uint64_t dah = smem_desc(ah + ks * 2 * kAPlane, kAPlane, 128), dal = smem_desc(al + ks * 2 * kAPlane, kAPlane, 128);
-                        const uint64_t dbh = smem_desc(bh + ks * 2 * N * 16, N * 16, 128), dbl = smem_desc(bl + ks * 2 * N * 16, N * 16, 128);
-                        mma_f16(acc, dah, dbh, idesc, s > 0 || ks > 0);
-                        mma_f16(acc, dah, dbl, idesc, true);
-                        mma_f16(acc, dal, dbh, idesc, true);
-                    }
-                }
-                __syncwarp();
-                commit_to(&bars[G_A_EMPTY + a]);
-                commit_to(&bars[G_B_EMPTY + b]);
-            }
-            commit_to(&bars[G_ACC_FULL + (i & 1)]);
-        }
-    } else if (warp == kGWStore) {
-        if (lane == 0) {
-            uint32_t c = 0;
-            for (int i = 0; i < nt_cta; ++i) {
-                int mb, nt;
-                tile_of(i, mb, nt);
-                const int nch = p.tile_n[nt] / 64;
-                for (int j = 0; j < nch; ++j, ++c) {
-                    const int ss = c % kNStg;
-                    const int gc = p.tile_chunk0[nt] + j;
-                    const int seg = p.chunk_seg[gc], c0 = p.chunk_c0[gc];
-                    const CUtensorMap *m = seg == 0 ? &mo0 : (seg == 1 ? &mo1 : &mo2);
-                    mbar_wait(&bars[G_STAGED + ss], (c / kNStg) & 1);
-                    const uint8_t *src = smem + S::off_stg + ss * kStg;
-                    if (p.accumulate) {
-                        tma_reduce_add_2d(m, src, c0, mb * kGM);
-                        tma_reduce_add_2d(m, src + kATile, c0 + 32, mb * kGM);
-                    } else {
-                        tma_store_2d(m, src, c0, mb * kGM);
-                        tma_store_2d(m, src + kATile, c0 + 32, mb * kGM);
-                    }
-                    tma_store_commit();
-                    tma_store_wait_read<0>();
-                    mbar_arrive(&bars[G_STG_FREE + ss]);
-                }
-            }
-            tma_store_wait_all<0>();
-        }
-    } else if (warp >= kGWConv0 && warp < kGWProducer) {
-        const int t = tid - kGWConv0 * 32;
-        uint32_t ga = 0;
-        for (int i = 0; i < nt_cta; ++i)
-            for (int s = 0; s < p.n_stages; ++s, ++ga) {
-                const int a = ga % kNA;
-                mbar_wait(&bars[G_A_FULL + a], (ga / kNA) & 1);
-                convert_tile32_inplace(smem + S::off_a + a * kATile, t);
-                fence_proxy_async();
-                mbar_arrive(&bars[G_A_OP + a]);
-            }
-    } else if (warp < 4) {
-        // =============================== epilogue (128 threads, TMEM lane == pixel row) ===============================
-        const int r = tid;
-        const uint32_t tl = tmem + ((uint32_t)(warp * 32) << 16);
-        uint32_t c = 0;
-        for (int i = 0; i < nt_cta; ++i) {
-            int mb, nt;
-            tile_of(i, mb, nt);
-            const int nch = p.tile_n[nt] / 64;
-            mbar_wait(&bars[G_ACC_FULL + (i & 1)], (i >> 1) & 1);
-            tc_fence_after();
-            for (int j = 0; j < nch; ++j, ++c) {
-                const int ss = c % kNStg;
-                uint8_t *row = smem + S::off_stg + ss * kStg + r * 128;
-                const int sw = r & 7;
-                const float *bias = p.bias ? p.bias + (p.tile_chunk0[nt] + j) * 64 : nullptr;
-                mbar_wait(&bars[G_STG_FREE + ss], ((c / kNStg) & 1) ^ 1);
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {                      // two 32-channel halves = the two swizzled tiles of the slot
-                    float o[32];
-                    tmem_ld16(tl + (i & 1) * kGNMax + j * 64 + h * 32, reinterpret_cast<uint32_t *>(o));
-                    tmem_ld16(tl + (i & 1) * kGNMax + j * 64 + h * 32 + 16, reinterpret_cast<uint32_t *>(o + 16));
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int q4 = 0; q4 < 8; ++q4) {
-                        float4 v = make_float4(o[4 * q4], o[4 * q4 + 1], o[4 * q4 + 2], o[4 * q4 + 3]);
-                        if (bias) {
-                            const float4 bb = __ldg(reinterpret_cast<const float4 *>(bias + h * 32) + q4);
-                            v.x += bb.x; v.y += bb.y; v.z += bb.z; v.w += bb.w;
-                        }
-                        *reinterpret_cast<float4 *>(row + h * kATile + ((q4 ^ sw) * 16)) = v;
-                    }
-                }
-                fence_proxy_async();
-                mbar_arrive(&bars[G_STAGED + ss]);
-            }
-            tc_fence_before();
-            mbar_arrive(&bars[G_ACC_EMPTY + (i & 1)]);
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc<512>(tmem);
-}
-
-// ---- weight packing: fp32 conv weights -> bf16 hi/lo UMMA planes, one block per (N tile, stage) -------------------------
+// ---- weight packing: fp32 conv weights -> bf16 hi/lo UMMA planes, one block per (N tile, stage) ------------------------
 struct PackParams {
     const float *wq, *wk, *wv;       // [Cq][C], [Cq][C], [C][C] row-major (the 1x1 conv weights)
     const float *bq, *bk, *bv;
@@ -302,18 +176,6 @@ __global__ void __launch_bounds__(256) cca_gemm_pack_kernel(const __grid_constan
         for (long i = gid; i < C + 2 * Cq; i += nth) p.bias[i] = i < C ? p.bv[i] : (i < C + Cq ? p.bq[i - C] : p.bk[i - C - Cq]);
 }
 
-bool make_map_2d(CUtensorMap *m, const void *base, long rows, int ch)
-{
-    EncodeFn enc = get_encode();
-    if (!enc) return false;
-    cuuint64_t dims[2] = {(cuuint64_t)ch, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)ch * 4};
-    cuuint32_t box[2] = {32u, (cuuint32_t)kGM};
-    cuuint32_t es[2] = {1, 1};
-    return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void *>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 // N tiles of up to 256 columns over n_chunks 64-column chunks
 void plan_tiles(int n_chunks, int n_stages, int *n_tiles, int *tile_n, int *tile_chunk0, long *tile_woff, long *total)
 {
@@ -328,282 +190,147 @@ void plan_tiles(int n_chunks, int n_stages, int *n_tiles, int *tile_n, int *tile
     *n_tiles = t; *total = off;
 }
 
-cudaError_t launch_gemm(const GemmParams &gp, const PackParams &pp, const void *a[3], const int ach[3], void *o[3], const int och[3],
-                        cudaStream_t st, const char **why)
+cudaError_t launch_gemm(GemmParams &gp, const PackParams &pp, const void *a[3], const int ach[3], void *o[3], const int och[3],
+                        cudaStream_t st, const char **)
 {
-    CUtensorMap m[6];
     for (int i = 0; i < 3; ++i) {
-        const void *ab = a[i] ? a[i] : a[0];
-        void *ob = o[i] ? o[i] : o[0];
-        if (!make_map_2d(&m[i], ab, gp.P, a[i] ? ach[i] : ach[0]) || !make_map_2d(&m[3 + i], ob, gp.P, o[i] ? och[i] : och[0])) {
-            if (why) *why = "cuTensorMapEncodeTiled failed";
-            return cudaErrorInvalidValue;
-        }
+        gp.a[i] = reinterpret_cast<const float *>(a[i] ? a[i] : a[0]); gp.ach[i] = a[i] ? ach[i] : ach[0];
+        gp.o[i] = reinterpret_cast<float *>(o[i] ? o[i] : o[0]); gp.och[i] = o[i] ? och[i] : och[0];
     }
     cca_gemm_pack_kernel<<<64, 256, 0, st>>>(pp);
     count_launch();
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(cca_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmSmem::kBytes);
-    if (e != cudaSuccess) return e;
-    const int total = ((gp.P + kGM - 1) / kGM) * gp.n_tiles;
+    const int total = ((gp.P + kGM - 1) / kGM) * gp.n_chunks;
     const int sms = sm_count();
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(total < sms ? total : sms); cfg.blockDim = dim3(kGThreads); cfg.dynamicSmemBytes = GemmSmem::kBytes; cfg.stream = st;
+    cfg.gridDim = dim3(total < 2 * sms ? total : 2 * sms); cfg.blockDim = dim3(kGThreads); cfg.dynamicSmemBytes = 0; cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = tc_pdl() ? 1 : 0;
-    e = cudaLaunchKernelEx(&cfg, cca_gemm_kernel, m[0], m[1], m[2], m[3], m[4], m[5], gp);
+    e = cudaLaunchKernelEx(&cfg, cca_gemm_kernel, gp);
     count_launch();
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 
-
 // =====================================================================================================================
 // Weight gradients of the three projections:  dW[n][k] = scale * sum_p G[p][n] X[p][k],   db[n] = scale * sum_p G[p][n]
 // with G = [dq | dk | dv] (n packed in that order) and X = x.  The contraction runs over the PIXELS, so both operands are
-// used MN-major: the same [8-channel chunk][pixel][16 B] planes the other kernels produce, addressed with the transposed
-// descriptor (the attention backward does the same for dV = P^T dO).  One CTA owns one output tile (128 rows n x 256 columns
-// k) over a range of pixels (split-K); its fp32 accumulator lives in TMEM for the whole kernel and is added onto the
-// zero-initialised dW with TMA reduce-adds at the end.  Stages of 64 pixels: 4 + 8 TMA tiles [64 px][32 ch], converted in
-// place by the 256 converter threads (hi and lo planes interleaved so that the 8-channel planes of neighbouring tiles keep
-// one uniform stride), 12 MMAs (4 k-steps x 3 split terms) of M=128, N=256.
+// MN-major planes [8-channel chunk][pixel][16 B].  One CTA owns one output tile (128 rows n x 64 columns k) over a range of
+// pixels (split-K), accumulates in registers (two warpgroups of 64 rows n) and adds onto the zero-initialised dW at the end.
 // =====================================================================================================================
 constexpr int kWPix = 64;                   // pixels per stage
-constexpr int kWTile = kWPix * 128;         // 8 KB: [64 px][32 ch] fp32
 constexpr int kWPlane = kWPix * 16;         // 1 KB
-constexpr int kWATiles = 4, kWBTiles = 8;   // 128 rows n, 256 columns k
-constexpr int kWStageBytes = (kWATiles + kWBTiles) * kWTile;   // 96 KB
-constexpr int kWNS = 2;
 
 struct WgradParams {
     int P, C, Cq;
-    int n_row_tiles, n_col_tiles, splits;   // 128-row tiles of n, 256-column tiles of k, pixel ranges
-    int stages_per_split;
-    const float *scale;                     // optional device scalar (gamma)
-    float *db;                              // [2Cq + C] packed bias gradient (q | k | v), zero-initialised; may be nullptr
+    int n_row_tiles, n_col_tiles, splits, stages_per_split;
+    const float *x, *dq, *dk, *dv;
+    const float *scale;
+    float *dwq, *dwk, *dwv, *db;
 };
-struct WgradSmem {
-    static constexpr int off_st = 0;
-    static constexpr int off_stg = off_st + kWNS * kWStageBytes;
-    static constexpr int off_bar = off_stg + kStg;
-    static constexpr int kBytes = off_bar + 8 * 16 + 16;
-    static_assert(kBytes <= 232448, "shared memory budget");
-};
-enum { W_FULL = 0, W_OP = 2, W_EMPTY = 4, W_ACC_FULL = 6, W_STG_FREE = 7, W_STAGED = 8, W_COUNT = 9 };
 
-// two fp32 tiles [64 px][32 ch] (SWIZZLE_128B) at once -> per tile [hi0 lo0 hi1 lo1 hi2 lo2 hi3 lo3] planes of [64 px][16 B],
-// in place; 256 threads: tile = t >> 7, pixel = t & 63, channel half = (t >> 6) & 1.  Returns the thread's 16 raw values
-// through `raw` (the bias gradient sums them).
-__device__ __forceinline__ void convert_tile_pair(uint8_t *tiles, int t, float4 (&raw)[4])
+__global__ void __launch_bounds__(kGThreads, 1) cca_wgrad_kernel(const __grid_constant__ WgradParams p)
 {
-    uint8_t *tile = tiles + (t >> 7) * kWTile;
-    const int r = t & 63, half = (t >> 6) & 1, sw = r & 7;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) raw[j] = *reinterpret_cast<const float4 *>(tile + r * 128 + (((half * 4 + j) ^ sw) * 16));
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-        const float4 a = raw[2 * j], b = raw[2 * j + 1];
-        const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-        uint4 hi, lo;
-        split8(v, hi, lo);
-        uint8_t *d = tile + (half * 2 + j) * 2 * kWPlane + r * 16;
-        *reinterpret_cast<uint4 *>(d) = hi;
-        *reinterpret_cast<uint4 *>(d + kWPlane) = lo;
-    }
-}
-
-__global__ void __launch_bounds__(kGThreads, 1)
-cca_wgrad_kernel(const __grid_constant__ CUtensorMap mg0, const __grid_constant__ CUtensorMap mg1, const __grid_constant__ CUtensorMap mg2,
-                 const __grid_constant__ CUtensorMap mx, const __grid_constant__ CUtensorMap mw0, const __grid_constant__ CUtensorMap mw1,
-                 const __grid_constant__ CUtensorMap mw2, const __grid_constant__ WgradParams p)
-{
-    using S = WgradSmem;
-    extern __shared__ __align__(1024) uint8_t smem[];
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + S::off_bar);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + S::off_bar + 8 * W_COUNT);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    // work unit of this CTA: (row tile, column tile, pixel split)
-    const int unit = blockIdx.x;
+    __shared__ __align__(1024) uint8_t sg[2 * 16 * kWPlane];   // G^T planes: [hi | lo][16 n-chunks][64 px][16 B]
+    __shared__ __align__(1024) uint8_t sx[2 * 8 * kWPlane];    // X planes:   [hi | lo][8 k-chunks][64 px][16 B]
+    const int t = threadIdx.x, wg = t >> 7, wq = (t >> 5) & 3, lane = t & 31;
+    const int rbase = 64 * wg + 16 * wq + (lane >> 2), cq = 2 * (lane & 3);
     const int tiles = p.n_row_tiles * p.n_col_tiles;
-    const int split = unit / tiles, tile = unit - split * tiles;
-    const int rt = tile / p.n_col_tiles, ct = tile - rt * p.n_col_tiles;
-    const int total_stages = (p.P + kWPix - 1) / kWPix;
-    const int s0 = split * p.stages_per_split;
-    const int ns = s0 >= total_stages ? 0 : (total_stages - s0 < p.stages_per_split ? total_stages - s0 : p.stages_per_split);
-    // 32-channel group g of packed n (q | k | v) -> source map and channel offset
-    auto gsrc = [&](int g, const CUtensorMap *&m, int &c0) {
-        const int n0 = g * 32;
-        if (n0 < p.Cq) { m = &mg0; c0 = n0; }
-        else if (n0 < 2 * p.Cq) { m = &mg1; c0 = n0 - p.Cq; }
-        else { m = &mg2; c0 = n0 - 2 * p.Cq; }
-    };
-
-    if (tid == 0) {
-        for (int i = 0; i < kWNS; ++i) { mbar_init(&bars[W_FULL + i], 1); mbar_init(&bars[W_OP + i], 256); mbar_init(&bars[W_EMPTY + i], 1); }
-        mbar_init(&bars[W_ACC_FULL], 1); mbar_init(&bars[W_STG_FREE], 1); mbar_init(&bars[W_STAGED], 128);
-        fence_mbar_init();
-        prefetch_tmap(&mg0); prefetch_tmap(&mg1); prefetch_tmap(&mg2); prefetch_tmap(&mx);
-        prefetch_tmap(&mw0); prefetch_tmap(&mw1); prefetch_tmap(&mw2);
+    const int tile = blockIdx.x % tiles, split = blockIdx.x / tiles;
+    const int nt = tile / p.n_col_tiles, kt = tile - nt * p.n_col_tiles;
+    const int n0 = nt * 128, k0 = kt * 64;
+    const int C = p.C, Cq = p.Cq;
+    const float sc = p.scale ? __ldg(p.scale) : 1.f;
+    const long s_lo = (long)split * p.stages_per_split;
+    const long n_st = (p.P + kWPix - 1) / kWPix;
+    const long s_hi = s_lo + p.stages_per_split < n_st ? s_lo + p.stages_per_split : n_st;
+    // loader roles: G: thread = (8 n values (t & 15), pixels (t >> 4) + 16 i);  X: thread = (8 k values (t & 7), pixels (t >> 3) + 32 i)
+    const int gn = n0 + 8 * (t & 15);
+    const float *gsrc; int gld;
+    if (gn < Cq) { gsrc = p.dq + gn; gld = Cq; } else if (gn < 2 * Cq) { gsrc = p.dk + (gn - Cq); gld = Cq; } else { gsrc = p.dv + (gn - 2 * Cq); gld = C; }
+    float colsum[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    float acc[32];
+    bool first = true;
+    for (long s = s_lo; s < s_hi; ++s) {
+        const long p0 = s * kWPix;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int px = (t >> 4) + 16 * i;
+            float v[8];
+            if (p0 + px < p.P) {
+                const float4 *src = reinterpret_cast<const float4 *>(gsrc + (p0 + px) * gld);
+                const float4 a = __ldg(src), b = __ldg(src + 1);
+                v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+            } else {
+#pragma unroll
+                for (int e = 0; e < 8; ++e) v[e] = 0.f;
+            }
+#pragma unroll
+            for (int e = 0; e < 8; ++e) colsum[e] += v[e];
+            uint4 hi, lo;
+            split8(v, hi, lo);
+            *reinterpret_cast<uint4 *>(sg + (t & 15) * kWPlane + px * 16) = hi;
+            *reinterpret_cast<uint4 *>(sg + (16 + (t & 15)) * kWPlane + px * 16) = lo;
+        }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int px = (t >> 3) + 32 * i;
+            float v[8];
+            if (p0 + px < p.P) {
+                const float4 *src = reinterpret_cast<const float4 *>(p.x + (p0 + px) * C + k0 + 8 * (t & 7));
+                const float4 a = __ldg(src), b = __ldg(src + 1);
+                v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+            } else {
+#pragma unroll
+                for (int e = 0; e < 8; ++e) v[e] = 0.f;
+            }
+            uint4 hi, lo;
+            split8(v, hi, lo);
+            *reinterpret_cast<uint4 *>(sx + (t & 7) * kWPlane + px * 16) = hi;
+            *reinterpret_cast<uint4 *>(sx + (8 + (t & 7)) * kWPlane + px * 16) = lo;
+        }
+        fence_proxy_async();
+        __syncthreads();
+        const uint32_t ga = smem_u32(sg) + 8 * wg * kWPlane, xb = smem_u32(sx);
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < kWPix / 16; ++ks) {
+            const uint64_t ah = smem_desc(ga + ks * 256, 128, kWPlane), al = smem_desc(ga + 16 * kWPlane + ks * 256, 128, kWPlane);
+            const uint64_t bh = smem_desc(xb + ks * 256, 128, kWPlane), bl = smem_desc(xb + 8 * kWPlane + ks * 256, 128, kWPlane);
+            wgmma_ss_n64(acc, ah, bh, first ? (ks > 0) : 1, 1, 1);
+            wgmma_ss_n64(acc, ah, bl, 1, 1, 1);
+            wgmma_ss_n64(acc, al, bh, 1, 1, 1);
+        }
+        wg_commit();
+        wg_wait<0>();
+        wg_acc_fence<32>(acc);
+        first = false;
+        __syncthreads();
     }
-    if (warp == 0) tmem_alloc<256>(tmem_slot);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-
-    if (warp == kGWProducer) {
-        if (lane == 0) {
-            for (int i = 0; i < ns; ++i) {
-                const int st = i % kWNS, px = (s0 + i) * kWPix;
-                mbar_wait(&bars[W_EMPTY + st], ((i / kWNS) & 1) ^ 1);
-                uint8_t *dst = smem + S::off_st + st * kWStageBytes;
-                mbar_expect_tx(&bars[W_FULL + st], kWStageBytes);
-                for (int a = 0; a < kWATiles; ++a) {
-                    const CUtensorMap *m; int c0;
-                    gsrc(rt * kWATiles + a, m, c0);
-                    tma_load_2d(dst + a * kWTile, m, &bars[W_FULL + st], c0, px);
-                }
-                for (int b = 0; b < kWBTiles; ++b)
-                    tma_load_2d(dst + (kWATiles + b) * kWTile, &mx, &bars[W_FULL + st], ct * 256 + b * 32, px);
-            }
-        }
-    } else if (warp == kGWMma) {
-        const uint32_t idesc = instr_desc(kFmtBF16, kFmtBF16, 128, 256, true, true);
-        for (int i = 0; i < ns; ++i) {
-            const int st = i % kWNS;
-            mbar_wait(&bars[W_OP + st], (i / kWNS) & 1);
-            tc_fence_after();
-            const uint32_t ab = smem_u32(smem + S::off_st + st * kWStageBytes), bb = ab + kWATiles * kWTile;
-            if (elect_one()) {
+    if (first) return;                                              // (no pixels in this split)
 #pragma unroll
-                for (int ks = 0; ks < kWPix / 16; ++ks) {
-                    // MN-major planes: next 8 pixels (K) at +128 B, next 8 channels (M / N) at +2 planes (hi, lo interleaved)
-                    const uint64_t ah = smem_desc(ab + ks * 256, 128, 2 * kWPlane), al = smem_desc(ab + kWPlane + ks * 256, 128, 2 * kWPlane);
-                    const uint64_t bh = smem_desc(bb + ks * 256, 128, 2 * kWPlane), bl = smem_desc(bb + kWPlane + ks * 256, 128, 2 * kWPlane);
-                    mma_f16(tmem, ah, bh, idesc, i > 0 || ks > 0);
-                    mma_f16(tmem, ah, bl, idesc, true);
-                    mma_f16(tmem, al, bh, idesc, true);
-                }
-            }
-            __syncwarp();
-            commit_to(&bars[W_EMPTY + st]);
-        }
-        commit_to(&bars[W_ACC_FULL]);
-    } else if (warp == kGWStore) {
-        if (lane == 0 && ns > 0) {
-            // rows of this tile in packed n order -> (dWq | dWk | dWv, first row); 64-row halves never straddle two tensors
-            for (int j = 0; j < 4; ++j) {
-                mbar_wait(&bars[W_STAGED], j & 1);
-                const uint8_t *src = smem + S::off_stg;
-                for (int hrow = 0; hrow < 2; ++hrow) {
-                    const int n0 = rt * 128 + hrow * 64;
-                    const CUtensorMap *m = n0 < p.Cq ? &mw0 : (n0 < 2 * p.Cq ? &mw1 : &mw2);
-                    const int row0 = n0 < p.Cq ? n0 : (n0 < 2 * p.Cq ? n0 - p.Cq : n0 - 2 * p.Cq);
-                    const int col0 = ct * 256 + j * 64;
-                    tma_reduce_add_2d(m, src + hrow * 64 * 128, col0, row0);
-                    tma_reduce_add_2d(m, src + kATile + hrow * 64 * 128, col0 + 32, row0);
-                }
-                tma_store_commit();
-                tma_store_wait_read<0>();
-                mbar_arrive(&bars[W_STG_FREE]);
-            }
-            tma_store_wait_all<0>();
-        }
-    } else if (warp >= kGWConv0 && warp < kGWProducer) {
-        const int t = tid - kGWConv0 * 32;
-        // bias gradient: only the CTAs of column tile 0 add it (every pixel of G passes through them exactly once per row tile)
-        float bsum[2][16];
+    for (int h = 0; h < 2; ++h) {
+        const int n = n0 + rbase + 8 * h;
+        float *row = n < Cq ? p.dwq + (long)n * C : (n < 2 * Cq ? p.dwk + (long)(n - Cq) * C : p.dwv + (long)(n - 2 * Cq) * C);
 #pragma unroll
-        for (int a = 0; a < 2; ++a)
-#pragma unroll
-            for (int e = 0; e < 16; ++e) bsum[a][e] = 0.f;
-        for (int i = 0; i < ns; ++i) {
-            const int st = i % kWNS;
-            mbar_wait(&bars[W_FULL + st], (i / kWNS) & 1);
-            uint8_t *base = smem + S::off_st + st * kWStageBytes;
-#pragma unroll
-            for (int pr = 0; pr < (kWATiles + kWBTiles) / 2; ++pr) {
-                float4 raw[4];
-                convert_tile_pair(base + pr * 2 * kWTile, t, raw);
-                if (pr < kWATiles / 2) {
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        bsum[pr][4 * j] += raw[j].x; bsum[pr][4 * j + 1] += raw[j].y; bsum[pr][4 * j + 2] += raw[j].z; bsum[pr][4 * j + 3] += raw[j].w;
-                    }
-                }
-            }
-            fence_proxy_async();
-            mbar_arrive(&bars[W_OP + st]);
-        }
-        if (p.db && ct == 0 && ns > 0) {
-            const float sc = p.scale ? __ldg(p.scale) : 1.f;
-            // thread (tile pair pr, tile-in-pair t>>7, half (t>>6)&1) holds channels n = rt*128 + (2 pr + (t>>7))*32 + half*16 + e
-            // summed over its pixel; reduce over the 64 pixels of the thread group with warp shuffles (a warp = 32 pixels of one
-            // (tile, half)), then one atomicAdd per channel and warp
-#pragma unroll
-            for (int a = 0; a < 2; ++a)
-#pragma unroll
-                for (int e = 0; e < 16; ++e) {
-                    float v = bsum[a][e];
-#pragma unroll
-                    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-                    if (lane == 0) atomicAdd(p.db + rt * 128 + (2 * a + (t >> 7)) * 32 + ((t >> 6) & 1) * 16 + e, v * sc);
-                }
-        }
-    } else if (warp < 4) {
-        if (ns > 0) {
-            const int r = tid;
-            const uint32_t tl = tmem + ((uint32_t)(warp * 32) << 16);
-            const float sc = p.scale ? __ldg(p.scale) : 1.f;
-            mbar_wait(&bars[W_ACC_FULL], 0);
-            tc_fence_after();
-            for (int j = 0; j < 4; ++j) {
-                uint8_t *row = smem + S::off_stg + r * 128;
-                const int sw = r & 7;
-                mbar_wait(&bars[W_STG_FREE], (j & 1) ^ 1);
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    float o[32];
-                    tmem_ld16(tl + j * 64 + h * 32, reinterpret_cast<uint32_t *>(o));
-                    tmem_ld16(tl + j * 64 + h * 32 + 16, reinterpret_cast<uint32_t *>(o + 16));
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int q4 = 0; q4 < 8; ++q4)
-                        *reinterpret_cast<float4 *>(row + h * kATile + ((q4 ^ sw) * 16)) =
-                            make_float4(o[4 * q4] * sc, o[4 * q4 + 1] * sc, o[4 * q4 + 2] * sc, o[4 * q4 + 3] * sc);
-                }
-                fence_proxy_async();
-                mbar_arrive(&bars[W_STAGED]);
-            }
+        for (int j = 0; j < 8; ++j) {
+            const int k = k0 + 8 * j + cq;
+            atomicAdd(reinterpret_cast<float2 *>(row + k), make_float2(sc * acc[4 * j + 2 * h], sc * acc[4 * j + 2 * h + 1]));
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc<256>(tmem);
-}
-
-bool make_map_2d_box(CUtensorMap *m, const void *base, long rows, int ch, int box_rows)
-{
-    EncodeFn enc = get_encode();
-    if (!enc) return false;
-    cuuint64_t dims[2] = {(cuuint64_t)ch, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)ch * 4};
-    cuuint32_t box[2] = {32u, (cuuint32_t)box_rows};
-    cuuint32_t es[2] = {1, 1};
-    return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void *>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    if (p.db && kt == 0)
+#pragma unroll
+        for (int e = 0; e < 8; ++e) atomicAdd(p.db + gn + e, sc * colsum[e]);
 }
 
 }  // namespace
 
 bool qkv_gemm_supported(int C, int Cq)
 {
-    return C % 64 == 0 && Cq % 64 == 0 && C >= 64 && Cq >= 64 && C + 2 * Cq <= 64 * kMaxChunks && (C + 2 * Cq) / kGK <= kMaxStages &&
-           get_encode() != nullptr;
+    return C % 64 == 0 && Cq % 64 == 0 && C >= 64 && Cq >= 64 && C + 2 * Cq <= 64 * kMaxChunks && (C + 2 * Cq) / kGK <= kMaxStages;
 }
 // packed weight blocks + packed bias
 size_t qkv_gemm_workspace(int C, int Cq)
@@ -624,6 +351,7 @@ cudaError_t qkv_project(const float *x, const float *wq, const float *bq, const 
     const int n_chunks = (C + 2 * Cq) / 64;
     long wbytes = 0;
     plan_tiles(n_chunks, gp.n_stages, &gp.n_tiles, gp.tile_n, gp.tile_chunk0, gp.tile_woff, &wbytes);
+    gp.n_chunks = n_chunks;
     for (int c = 0; c < n_chunks; ++c) {          // packed column order: v | q | k
         const int col = c * 64;
         if (col < C) { gp.chunk_seg[c] = 2; gp.chunk_c0[c] = col; }
@@ -662,6 +390,7 @@ cudaError_t qkv_project_dgrad(const float *dq, const float *dk, const float *dv,
     const int n_chunks = C / 64;
     long wbytes = 0;
     plan_tiles(n_chunks, gp.n_stages, &gp.n_tiles, gp.tile_n, gp.tile_chunk0, gp.tile_woff, &wbytes);
+    gp.n_chunks = n_chunks;
     for (int c = 0; c < n_chunks; ++c) { gp.chunk_seg[c] = 0; gp.chunk_c0[c] = c * 64; }
     uint8_t *wblocks = reinterpret_cast<uint8_t *>(ws);
     gp.wblocks = wblocks; gp.bias = nullptr; gp.accumulate = accumulate;
@@ -679,16 +408,8 @@ cudaError_t qkv_project_dgrad(const float *dq, const float *dk, const float *dv,
 // dWq [Cq,C], dWk [Cq,C], dWv [C,C] = scale * G^T x ; db (packed q | k | v, 2Cq + C floats) = scale * column sums of G.
 // The outputs are cleared here (cudaMemsetAsync) and accumulated by the split-K CTAs.
 cudaError_t qkv_project_wgrad(const float *x, const float *dq, const float *dk, const float *dv, const float *scale, float *dwq,
-                              float *dwk, float *dwv, float *db, long P, int C, int Cq, cudaStream_t st, const char **why)
+                              float *dwk, float *dwv, float *db, long P, int C, int Cq, cudaStream_t st, const char **)
 {
-    CUtensorMap m[7];
-    const bool ok = make_map_2d_box(&m[0], dq, P, Cq, kWPix) && make_map_2d_box(&m[1], dk, P, Cq, kWPix) && make_map_2d_box(&m[2], dv, P, C, kWPix) &&
-                    make_map_2d_box(&m[3], x, P, C, kWPix) && make_map_2d_box(&m[4], dwq, Cq, C, 64) && make_map_2d_box(&m[5], dwk, Cq, C, 64) &&
-                    make_map_2d_box(&m[6], dwv, C, C, 64);
-    if (!ok) {
-        if (why) *why = "cuTensorMapEncodeTiled failed";
-        return cudaErrorInvalidValue;
-    }
     cudaError_t e;
     if ((e = cudaMemsetAsync(dwq, 0, sizeof(float) * Cq * C, st)) != cudaSuccess || (e = cudaMemsetAsync(dwk, 0, sizeof(float) * Cq * C, st)) != cudaSuccess ||
         (e = cudaMemsetAsync(dwv, 0, sizeof(float) * C * C, st)) != cudaSuccess)
@@ -696,16 +417,15 @@ cudaError_t qkv_project_wgrad(const float *x, const float *dq, const float *dk, 
     if (db && (e = cudaMemsetAsync(db, 0, sizeof(float) * (2 * Cq + C), st)) != cudaSuccess) return e;
     WgradParams p = {};
     p.P = (int)P; p.C = C; p.Cq = Cq;
-    p.n_row_tiles = (2 * Cq + C) / 128; p.n_col_tiles = C / 256;
+    p.n_row_tiles = (2 * Cq + C) / 128; p.n_col_tiles = C / 64;
     const int tiles = p.n_row_tiles * p.n_col_tiles;
     const int sms = sm_count();
-    p.splits = sms / tiles > 0 ? sms / tiles : 1;
+    p.splits = 2 * sms / tiles > 0 ? 2 * sms / tiles : 1;
     const int total_stages = (int)((P + kWPix - 1) / kWPix);
     p.stages_per_split = (total_stages + p.splits - 1) / p.splits;
-    p.scale = scale; p.db = db;
-    e = cudaFuncSetAttribute(cca_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WgradSmem::kBytes);
-    if (e != cudaSuccess) return e;
-    cca_wgrad_kernel<<<tiles * p.splits, kGThreads, WgradSmem::kBytes, st>>>(m[0], m[1], m[2], m[3], m[4], m[5], m[6], p);
+    p.x = x; p.dq = dq; p.dk = dk; p.dv = dv;
+    p.scale = scale; p.dwq = dwq; p.dwk = dwk; p.dwv = dwv; p.db = db;
+    cca_wgrad_kernel<<<tiles * p.splits, kGThreads, 0, st>>>(p);
     count_launch();
     return cudaGetLastError();
 }

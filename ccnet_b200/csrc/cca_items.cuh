@@ -1,4 +1,4 @@
-// Work decomposition shared by the tcgen05 kernels (statistics pre-pass, forward values, backward).
+// Work decomposition shared by the tensor-core kernels (statistics pre-pass, forward values, backward).
 //
 // One ITEM = (direction, sample b, line, query tile iq, key block ik):
 //   direction : column line (pixels (h, w=line), h = 0..H-1; self entry masked, cc_attention/functions.py:38)

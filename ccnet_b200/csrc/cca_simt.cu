@@ -1,5 +1,5 @@
-// Generic CUDA-core (FFMA) criss-cross attention kernels for sm_100a: any dtype/shape within
-// the shared-memory limits.  They are the shape-general companion of the tcgen05 kernels
+// Generic CUDA-core (FFMA) criss-cross attention kernels for sm_90a: any dtype/shape within
+// the shared-memory limits.  They are the shape-general companion of the wgmma kernels
 // (cca_tc_fwd.cu) and the first correct CUDA path of the operator.
 //
 // Decomposition (replaces cc_attention/functions.py:30-47 without materialising any

@@ -1,32 +1,31 @@
-// tcgen05 / TMA backward kernel of criss-cross attention for sm_100a (channels-last tensors).
+// wgmma / TMA backward kernel of criss-cross attention for sm_90a (channels-last tensors).
 //
 // Closed form of SURVEY.md 8(a) row a11 (autograd of cc_attention/functions.py:38-47), flash-style: the attention matrix is
 // recomputed per item from (q, k, lse), never stored.  Items are those of cca_items.cuh (direction, sample, line, query
 // tile, key block); because P = exp(S - lse) uses the FINAL lse, every item is independent and ADDS its contributions:
-//   S  = Q K^T                     (K-dim Cq)        P  = exp(S - lse[jq])            [TMEM -> planes in smem]
-//   dP = dO V^T                    (K-dim C, chunked, accumulated in TMEM over the V/dO chunks)
+//   S  = Q K^T                     (K-dim Cq)        P  = exp(S - lse[jq])            [registers -> bf16 planes in smem]
+//   dP = dO V^T                    (K-dim C, accumulated in registers over the V/dO chunks)
 //   dV[jk,c] += sum_jq P[jq,jk] dO[jq,c]   per chunk  (A = P planes read MN-major = P^T, B = dO chunk)
 //   dS = P * (dP - delta[jq])      [planes overwrite P]
 //   dQ[jq,c] += sum_jk dS[jq,jk] K[jk,c]   (A = dS planes K-major)     dK[jk,c] += sum_jq dS[jq,jk] Q[jq,c]  (A = dS^T)
 // ONE persistent launch walks the items sample by sample (column items, then row items of the same sample): the second
-// direction finds q,k,v,dO in L2 and its TMA reduce-adds land on dq/dk/dv lines that are still L2-resident.
+// direction finds q,k,v,dO in L2 and its adds land on dq/dk/dv lines that are still L2-resident.
 //
 // delta[jq] = sum_c dO[jq,c] O[jq,c] is folded into the items (no separate pass over dO and O): the O chunk of the query
-// pixels rides the same ring as V and dO, and the converter warps -- which touch every dO element anyway -- accumulate the
+// pixels rides the same ring as V and dO, and the conversion of dO -- which reads every dO element anyway -- accumulates the
 // dot products.  Two modes: every item computes delta for itself (no dependency), or only the column items of the first key
 // block do, publish it through global memory and a per-sample counter, and the other items of the sample wait for that counter
 // right before their dS phase (such items always have a higher index than the producers: no cyclic waits).
 //
-// Output path (dq, dk, dv need no initialisation by the caller).  One tile per line (H, W <= 112): as in the forward
-// (cca_tc_fwd.cu) the column items STORE their tiles, the row items ADD onto them (TMA reduce-add) once the per-sample counter
-// cdone[b] says every column item of the sample has completed its stores.  Tiled lines: several items contribute to the same
-// dk / dv rows, so everything is added: the items of sample b first clear 1/per_sample of sample b+ahead's slices (zero-ahead,
-// bulk copies of a zero tile, counter zdone), a prep kernel clears the first `ahead` samples and the counters.
+// Output path (dq, dk, dv need no initialisation by the caller).  One tile per line (H, W <= 112): as in the forward the
+// column items STORE their rows, the row items ADD onto them once the per-sample counter cdone[b] says every column item of the
+// sample has completed its stores.  Tiled lines: several items contribute to the same dk / dv rows, so a prologue clears the
+// outputs and every item adds.
 //
-// All GEMMs run as bf16x3 split MMAs (hi*hi + hi*lo + lo*hi) with fp32 accumulation in TMEM (single bf16 MMAs for bf16 I/O).
-// The same operand planes serve several GEMMs: planes over channels are a K-major operand when the contraction runs over
-// channels (S, dP) and an MN-major B operand when channels are the output (dV, dQ, dK); planes over key pixels are K-major A
-// for dQ and MN-major A (= transpose) for dV / dK.
+// All GEMMs run as bf16x3 split MMAs (hi*hi + hi*lo + lo*hi) with fp32 accumulation in registers (single bf16 MMAs for bf16
+// I/O), two consumer warpgroups of 64 rows each (cca_tc_common.cuh).
+#include <type_traits>
+
 #include "cca_items.cuh"
 #include "cca_tc_common.cuh"
 
@@ -34,670 +33,329 @@ namespace cca {
 namespace {
 using namespace tc;
 
-constexpr int kTmemCols = 512;      // S / dP double buffer: [0,128) [128,256)   dV ring O0: [256,320) O1: [320,384)   dQ: [384,448)   dK: [448,512)
-constexpr int kTmemO = 256, kTmemQK = 384;   // dQ / dK have accumulators of their own: phase D never waits for the dV tiles to drain
-constexpr int kRegsSoft = 104, kRegsEpi = 128, kRegsConvB = 48;
-static_assert(reg_pool_ok(kRegsSoft, kRegsEpi, kRegsConvB), "setmaxnreg pool");
-constexpr int kZeroBuf = 2048;
-
 struct BwdParams {
     ItemSpace sp;
     int C, Cq;
     long npix;
     const float *lse;
     float *delta;              // [B,H,W] <dout, out> per pixel, written by the producer items (first bytes of the workspace)
-    unsigned int *zdone;       // [B] zero shares of sample b completed
     unsigned int *ddone;       // [B] delta producers of sample b done (delta_mode 1)
     int delta_mode;            // 0: every item computes its own delta; 1: column / first-key-block items produce, the rest wait
-    int out_mode;              // 1: producers store, consumers add after cdone (one tile per line); 0: zero-ahead, everything adds
+    int out_mode;              // 1: producers store, consumers add after cdone (one tile per line); 0: cleared outputs, everything adds
     unsigned int *cdone;       // [B] producer items of sample b whose stores have completed (out_mode 1)
     int lag;                   // item order (cca_items.cuh): 1 = consumers trail the producers by one block
-    int hints;                 // L2 eviction hints on the bulk copies
-    uint8_t *dq, *dk, *dv;
-    long sb_q, sb_v;           // bytes per sample of dq (= dk) and dv
-    long share_q, share_v;     // zero share per item
-    int ahead;
-    long long *dbg;
+    int hints;                 // L2 eviction hints on the loads
+    void *dq, *dk, *dv;
 };
-
-#ifdef CCA_TIMELINE
-#define CCA_STAMP(role)                                                                          \
-    do {                                                                                         \
-        if (p.dbg && blockIdx.x == 0 && dbg_n < 512) p.dbg[(role) * 512 + dbg_n++] = clock64();  \
-    } while (0)
-#else
-#define CCA_STAMP(role) do { } while (0)
-#endif
 
 template <int LK, bool BF> struct BwdSmem {
     using T = Tiles<LK, BF>;
-    static constexpr int kNLd = BF ? 6 : 5;                // every slot is the UMMA operand itself: a bf16 tile as loaded, an fp32
-                                                           // tile once the converters have rewritten it in place (hi/lo planes)
-    static constexpr int off_ld = 0;                       // kNLd load slots
-    static constexpr int kNOut = BF ? 3 : 1;               // staging slots (fp32: shared memory is full; bf16: the epilogue -> TMA
-                                                           // store -> slot-free chain of a single slot paced the whole item)
-    static constexpr int off_out = off_ld + kNLd * T::kSlot;
-    static constexpr int off_p = off_out + kNOut * T::kSlot; // P / dS planes (hi, lo); M=128 over-reads of a slot land in the next slot / here
-    static constexpr int off_tail = off_p + T::kP + (16 - LK / 8) * T::kPlane;   // pad for the P^T over-read (16 planes of 8 key pixels)
-    static constexpr int off_zero = off_tail + (128 - LK) * 16 + 256;            // zero tile of the zero-ahead copies
-    static constexpr int off_dpart = off_zero + kZeroBuf;  // float [4][128]: per-pixel delta quarters from the converters, then
-                                                           // unsigned [8]: readers of an O slot (one counter per ring slot)
-    static constexpr int off_bar = off_dpart + 2048 + 32;
-    static constexpr int kBytes = off_bar + 8 * 48 + 32;
+    static constexpr int off_qk = 0;                                // Q slot, K slot (held for the whole item: dQ, dK read them)
+    static constexpr int off_p = off_qk + 2 * T::kSlot;             // P / dS planes (hi block, lo block)
+    // (pad: 64-row P^T operands read up to 16 planes; TMA destinations with SWIZZLE_128B must be 1024-byte aligned)
+    static constexpr int off_ld = (off_p + T::kP + (16 - LK / 8) * T::kPlane + 1023) / 1024 * 1024;
+    static constexpr int kNLd = (224 * 1024 - 4096 - off_ld) / T::kSlot < 8 ? (224 * 1024 - 4096 - off_ld) / T::kSlot : 8;
+    static constexpr int off_tail = off_ld + kNLd * T::kSlot;       // over-read of the last slot by the second warpgroup
+    static constexpr int off_dsum = off_tail + (128 - LK) * 128 + 256;   // float [2][128]: delta halves per pixel row
+    static constexpr int off_bar = off_dsum + 1024;
+    static constexpr int kBytes = off_bar + 8 * (2 + 2 * kNLd);
+    static_assert(kNLd >= 3, "ring depth: V, dO, O of one chunk");
     static_assert(kBytes <= 232448, "shared memory budget");
 };
-
-enum { B_LD_FULL = 0, B_LD_EMPTY = 6, B_OP_FULL = 12, B_S_FULL = 18, B_S_EMPTY = 20, B_P_FULL = 22,
-       B_P_EMPTY = 23, B_O_FULL = 24, B_O_EMPTY = 26, B_OUT_FULL = 28, B_STAGED = 29, B_DP_FULL = 30, B_DS_FULL = 31,
-       B_DELTA_FULL = 32, B_DELTA_EMPTY = 33, B_OUT_FREE = 34, B_STAGED_W = 37, B_QK_FULL = 43, B_QK_EMPTY = 45,
-       B_COUNT = 47 };   // B_OUT_FREE[slot], B_STAGED_W[store warp][slot], B_QK_*[dQ, dK]
 
 // does this item compute delta itself (its ring carries the O chunks)?
 __device__ __forceinline__ bool calc_delta(const BwdParams &p, const Item &it) { return p.delta_mode == 0 || (it.col && it.ik == 0); }
 
-// Converter step for a (dO, O) pair of ring slots: returns this thread's part of sum_c dO[r][c] * O[r][c] over its 16 channels of
-// the chunk and (fp32) rewrites the dO slot in place as bf16 hi/lo planes (layout and thread mapping of convert_slot_inplace: two
-// independent groups of 256 threads, one per 32-channel box; thread = (pixel row, 16-channel half)).  The O slot goes back to the
-// producer once BOTH groups have read it: the second group leader to bump o_cnt arrives on the slot's LD_EMPTY barrier.
-template <int LK, bool BF>
-__device__ __forceinline__ float convert_dot(uint8_t *dslot, const uint8_t *oslot, int t, uint64_t *o_empty, unsigned int *o_cnt)
-{
-    using T = Tiles<LK, BF>;
-    const int grp = t >> 8, r = t & 127, hq = (t >> 7) & 1;
-    const int rr = r < LK ? r : LK - 1;
-    const int sw = rr & 7;
-    float acc = 0.f;
-    auto group_sync_and_release = [&]() {
-        if (grp == 0) asm volatile("bar.sync 1, 256;" ::: "memory");
-        else asm volatile("bar.sync 3, 256;" ::: "memory");
-        if ((t & 255) == 0 && atomicAdd(o_cnt, 1u) == 1u) {    // both groups have read the O tile
-            *o_cnt = 0u;
-            mbar_arrive(o_empty);
-        }
-    };
-    if constexpr (BF) {
-        // one 128-byte-wide tile = 64 bf16 channels: 8 chunks of 16 B; this thread takes chunks 2*(2*grp + hq), +1
-        const uint8_t *a = dslot + rr * 128, *b = oslot + rr * 128;
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            const int j = (grp * 2 + hq) * 2 + i;
-            const uint4 x = *reinterpret_cast<const uint4 *>(a + ((j ^ sw) * 16));
-            const uint4 y = *reinterpret_cast<const uint4 *>(b + ((j ^ sw) * 16));
-            const uint32_t xw[4] = {x.x, x.y, x.z, x.w}, yw[4] = {y.x, y.y, y.z, y.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) acc += bf_lo(xw[e]) * bf_lo(yw[e]) + bf_hi(xw[e]) * bf_hi(yw[e]);
-        }
-        group_sync_and_release();
-    } else {
-        float4 raw[4];
-        uint8_t *box = dslot + grp * T::kTile;
-        const uint8_t *src = box + rr * 128;
-        const uint8_t *osrc = oslot + grp * T::kTile + rr * 128;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) raw[j] = *reinterpret_cast<const float4 *>(src + (((hq * 4 + j) ^ sw) * 16));
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const float4 o = *reinterpret_cast<const float4 *>(osrc + (((hq * 4 + j) ^ sw) * 16));
-            acc += raw[j].x * o.x + raw[j].y * o.y + raw[j].z * o.z + raw[j].w * o.w;
-        }
-        group_sync_and_release();
-        if (r < LK) {
-            uint8_t *d = box + r * 16 + hq * 2 * T::kPStride;
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                const float4 a = raw[2 * j], b = raw[2 * j + 1];
-                const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-                uint4 hi, lo;
-                split8(v, hi, lo);
-                *reinterpret_cast<uint4 *>(d + j * T::kPStride) = hi;
-                *reinterpret_cast<uint4 *>(d + j * T::kPStride + T::kLoOff) = lo;
-            }
-        }
-    }
-    return acc;
-}
-
-// Per item the ring carries  Q K | (V_n dO_n [O_n])* | Q' K' (next item) | Q K (again, for dQ / dK); item g lives in load slot
-// g % kNLd (fp32: converted in place), so the loads and conversions of the next chunks overlap the MMAs of the current one.
-// MMAs per item: S (phase A), per chunk dP += dO V^T then dV = P^T dO (phase B; the V buffer is released right after the dP
-// MMAs), dS by the P/dS group (phase C), dQ = dS K and dK = dS^T Q (phase D).
 template <int LK, bool BF>
 __global__ void __launch_bounds__(kThreads, 1)
 cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant__ CUtensorMap mqr,
                   const __grid_constant__ CUtensorMap mkc, const __grid_constant__ CUtensorMap mkr,
                   const __grid_constant__ CUtensorMap mvc, const __grid_constant__ CUtensorMap mvr,
                   const __grid_constant__ CUtensorMap mdoc, const __grid_constant__ CUtensorMap mdor,
-                  const __grid_constant__ CUtensorMap moc, const __grid_constant__ CUtensorMap mor,
-                  const __grid_constant__ CUtensorMap mdqc, const __grid_constant__ CUtensorMap mdqr,
-                  const __grid_constant__ CUtensorMap mdkc, const __grid_constant__ CUtensorMap mdkr,
-                  const __grid_constant__ CUtensorMap mdvc, const __grid_constant__ CUtensorMap mdvr, BwdParams p)
+                  const __grid_constant__ CUtensorMap moc, const __grid_constant__ CUtensorMap mor, BwdParams p)
 {
     using T = Tiles<LK, BF>;
     using S = BwdSmem<LK, BF>;
+    using E = typename std::conditional<BF, __nv_bfloat16, float>::type;
     constexpr int TERMS = BF ? 1 : 3;
     constexpr int kNLd = S::kNLd;
-    constexpr int kNOut = S::kNOut;
+    constexpr int KP = LK / 16;
+    constexpr uint32_t LOP = T::kPP * T::kPlane;   // P / dS planes: hi block -> lo block
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + S::off_bar);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + S::off_bar + 8 * B_COUNT);
-    float *dpart = reinterpret_cast<float *>(smem + S::off_dpart);
-    unsigned int *o_cnt = reinterpret_cast<unsigned int *>(smem + S::off_dpart + 2048);
+    uint64_t *qk_full = bars, *qk_empty = bars + 1, *full = bars + 2, *empty = bars + 2 + kNLd;
+    float *dsum = reinterpret_cast<float *>(smem + S::off_dsum);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int NCH = p.C / kNC;
     const int KQ = p.Cq / 16;
-    const int NO = NCH + 2;                   // output tiles per item: dV chunks, dQ, dK
     const int nk = p.sp.total > (int)blockIdx.x ? (p.sp.total - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
     auto item_of = [&](int k) { return decode_item_order(p.sp, (int)blockIdx.x + k * (int)gridDim.x, p.lag); };
 
     if (tid == 0) {
-        for (int i = 0; i < kNLd; ++i) {
-            mbar_init(&bars[B_LD_FULL + i], 1); mbar_init(&bars[B_LD_EMPTY + i], 1); mbar_init(&bars[B_OP_FULL + i], kConvThreads);
-        }
-        for (int i = 0; i < 2; ++i) { mbar_init(&bars[B_O_FULL + i], 1); mbar_init(&bars[B_O_EMPTY + i], 128); }
-        for (int i = 0; i < 3; ++i) { mbar_init(&bars[B_OUT_FREE + i], 1); mbar_init(&bars[B_STAGED_W + i], 128); mbar_init(&bars[B_STAGED_W + 3 + i], 128); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&bars[B_S_FULL + i], 1); mbar_init(&bars[B_S_EMPTY + i], 128); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&bars[B_QK_FULL + i], 1); mbar_init(&bars[B_QK_EMPTY + i], 128); }
-        mbar_init(&bars[B_P_FULL], 128); mbar_init(&bars[B_P_EMPTY], 1);
-        mbar_init(&bars[B_DP_FULL], 1);  mbar_init(&bars[B_DS_FULL], 128);
-        mbar_init(&bars[B_DELTA_FULL], kConvThreads); mbar_init(&bars[B_DELTA_EMPTY], 128);
+        mbar_init(qk_full, 1); mbar_init(qk_empty, kConsumers);
+        for (int i = 0; i < kNLd; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kConsumers); }
         fence_mbar_init();
         prefetch_tmap(&mqc); prefetch_tmap(&mqr); prefetch_tmap(&mkc); prefetch_tmap(&mkr); prefetch_tmap(&mvc); prefetch_tmap(&mvr);
         prefetch_tmap(&mdoc); prefetch_tmap(&mdor); prefetch_tmap(&moc); prefetch_tmap(&mor);
-        prefetch_tmap(&mdqc); prefetch_tmap(&mdqr); prefetch_tmap(&mdkc); prefetch_tmap(&mdkr); prefetch_tmap(&mdvc); prefetch_tmap(&mdvr);
     }
-    if (tid < kZeroBuf / 16) {                                 // zero tile (read by the async proxy: fence before the barrier)
-        reinterpret_cast<uint4 *>(smem + S::off_zero)[tid] = make_uint4(0, 0, 0, 0);
-        fence_proxy_async();
-    }
-    if (tid < 8) o_cnt[tid] = 0u;
-    if (warp == 0) tmem_alloc<kTmemCols>(tmem_slot);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
-    if (warp >= kWarpProducer) {
-        reg_dec<kRegsMisc>();
-        if (warp == kWarpProducer) {
-            // =============================== TMA producer ===============================
-            if (lane == 0) {
-                uint32_t g = 0;
-                int dbg_n = 0;
-                (void)dbg_n;
-                const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
-                auto emit = [&](const CUtensorMap *mc, const CUtensorMap *mr, int c0, const Item &it, int start, bool last_use = false) {
-                    const CUtensorMap *m = it.col ? mc : mr;
-                    const int cw = it.col ? it.line : start, ch = it.col ? start : it.line;
-                    const int slot = g % kNLd;
-                    mbar_wait(&bars[B_LD_EMPTY + slot], ((g / kNLd) & 1) ^ 1);
-                    CCA_STAMP(0);
-                    uint8_t *dst = smem + S::off_ld + slot * T::kSlot;
-                    mbar_expect_tx(&bars[B_LD_FULL + slot], T::kSlot);
-                    if (p.hints == 1) {     // what the sample's consumers read again stays; O and the consumers' own operands stream
-                        const uint64_t pol = (is_producer(it) && !last_use) ? pol_keep : pol_stream;   // (hints == 2: keep outputs only)
-                        tma_load_4d(dst, m, &bars[B_LD_FULL + slot], c0, cw, ch, it.b, pol);
-                        if constexpr (!BF) tma_load_4d(dst + T::kTile, m, &bars[B_LD_FULL + slot], c0 + 32, cw, ch, it.b, pol);
-                    } else {
-                        tma_load_4d(dst, m, &bars[B_LD_FULL + slot], c0, cw, ch, it.b);
-                        if constexpr (!BF) tma_load_4d(dst + T::kTile, m, &bars[B_LD_FULL + slot], c0 + 32, cw, ch, it.b);
-                    }
-                    ++g;
-                };
-                // ring:  Q0 K0 | (V dO [O])* Q1 K1 Q0 K0 | (V dO [O])* Q2 K2 Q1 K1 | ...   (S of the next item is issued while the
-                // dS of the current one is being computed; Q,K of the current item come back for dQ/dK)
-                if (nk > 0) {
-                    const Item it0 = item_of(0);
-                    emit(&mqc, &mqr, 0, it0, it0.q0);
-                    emit(&mkc, &mkr, 0, it0, it0.k0);
+    if (warp == 0) {
+        // =============================== TMA producer ===============================
+        if (lane == 0) {
+            const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
+            auto load = [&](uint8_t *dst, uint64_t *bar, const CUtensorMap *m, int c0, const Item &it, int start, bool last_use) {
+                const int cw = it.col ? it.line : start, ch = it.col ? start : it.line;
+                if (p.hints == 1) {     // what the sample's consumers read again stays; O and the consumers' own operands stream
+                    const uint64_t pol = (is_producer(it) && !last_use) ? pol_keep : pol_stream;
+                    tma_load_4d(dst, m, bar, c0, cw, ch, it.b, pol);
+                    if constexpr (!BF) tma_load_4d(dst + T::kTile, m, bar, c0 + 32, cw, ch, it.b, pol);
+                } else {
+                    tma_load_4d(dst, m, bar, c0, cw, ch, it.b);
+                    if constexpr (!BF) tma_load_4d(dst + T::kTile, m, bar, c0 + 32, cw, ch, it.b);
                 }
-                for (int k = 0; k < nk; ++k) {
-                    const Item it = item_of(k);
-                    const bool calc = calc_delta(p, it);
-                    for (int n = 0; n < NCH; ++n) {
-                        emit(&mvc, &mvr, n * kNC, it, it.k0);
-                        emit(&mdoc, &mdor, n * kNC, it, it.q0);
-                        if (calc) emit(&moc, &mor, n * kNC, it, it.q0, p.delta_mode == 1);   // (mode 1: nobody reads O again)
-                    }
-                    if (k + 1 < nk) {
-                        const Item nx = item_of(k + 1);
-                        emit(&mqc, &mqr, 0, nx, nx.q0);
-                        emit(&mkc, &mkr, 0, nx, nx.k0);
-                    }
-                    emit(&mqc, &mqr, 0, it, it.q0);
-                    emit(&mkc, &mkr, 0, it, it.k0);
-                }
-            }
-        } else if (warp == kWarpMma) {
-            // =============================== MMA issuer ===============================
-            const uint32_t id_kk_s = instr_desc(kFmtBF16, kFmtBF16, 128, LK, false, false);    // S, dP : K-major x K-major, N = LK
-            const uint32_t id_mn_mn = instr_desc(kFmtBF16, kFmtBF16, 128, kNC, true, true);    // dV, dK: A^T planes x channel planes
-            const uint32_t id_k_mn = instr_desc(kFmtBF16, kFmtBF16, 128, kNC, false, true);    // dQ
-            const uint32_t pb = smem_u32(smem + S::off_p);
-            const uint32_t LO8 = BF ? 0 : T::kLoOff, LOP = T::kPP * T::kPlane;     // channel tiles: hi -> lo plane; P / dS planes: hi block -> lo block
-            uint32_t u = 0, oc = 0;
-            int dbg_n = lane == 0 ? 0 : 512;
-            (void)dbg_n;
-            // operand of ring item g = load slot g % kNLd: fp32 -> bf16 hi/lo planes written in place (K-major / MN-major by descriptor);
-            //                  bf16 -> the TMA tile itself read with SWIZZLE_128B descriptors:
-            //                          K-major use: k-step = +32 B; MN-major use: k-step = +2048 B (16 pixel rows)
-            const uint32_t ld_base = smem_u32(smem + S::off_ld);
-            auto opb = [&](uint32_t g) { return ld_base + (g % kNLd) * T::kSlot; };
-            auto wait_op = [&](uint32_t g) { mbar_wait(&bars[B_OP_FULL + g % kNLd], (g / kNLd) & 1); };
-            auto free_op = [&](uint32_t g) { commit_to(&bars[B_LD_EMPTY + g % kNLd]); };
-            // channel-tile operand parameters: (k-step, lbo, sbo, layout) when the contraction runs over channels (kmaj) or
-            // over pixels (mnmaj)
-            constexpr uint32_t KS_K = BF ? 32 : 2 * T::kPStride, LBO_K = BF ? 16 : T::kPStride, SBO_K = BF ? 1024 : 128;
-            constexpr uint32_t KS_MN = BF ? 2048 : 256, LBO_MN = BF ? 16 : 128, SBO_MN = BF ? 1024 : T::kPStride;
-            constexpr uint32_t LAY = BF ? kSw128 : 0;
-            auto issue_s = [&](int k) {                       // S(k) = Q K^T into S buffer k&1
-                const uint32_t q = opb(u), kk = opb(u + 1);
-                wait_op(u); wait_op(u + 1);
-                mbar_wait(&bars[B_S_EMPTY + (k & 1)], ((k >> 1) & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t d = tmem + (k & 1) * 128;
-                for (int ks = 0; ks < KQ; ++ks) {
-                    const uint32_t ao = ks * KS_K;
-                    mma_split3<TERMS>(d, smem_desc(q + ao, LBO_K, SBO_K, LAY), smem_desc(q + LO8 + ao, LBO_K, SBO_K, LAY),
-                                      smem_desc(kk + ao, LBO_K, SBO_K, LAY), smem_desc(kk + LO8 + ao, LBO_K, SBO_K, LAY), id_kk_s, ks > 0);
-                }
-                commit_to(&bars[B_S_FULL + (k & 1)]);
-                free_op(u); free_op(u + 1);
-                u += 2;
             };
-            if (nk > 0) issue_s(0);
-            for (int k = 0; k < nk; ++k) {
-                const bool calc = calc_delta(p, item_of(k));
-                CCA_STAMP(2);
-                const uint32_t sdp = tmem + (k & 1) * 128;        // S(k), then dP(k)
-                mbar_wait(&bars[B_P_FULL], k & 1);
-                CCA_STAMP(2);
-                // ---- phase B: per chunk  dP += dO V^T  and  dV = P^T dO
-                for (int n = 0; n < NCH; ++n, u += calc ? 3 : 2, ++oc) {
-                    const uint32_t vb = opb(u), db = opb(u + 1);
-                    wait_op(u); wait_op(u + 1);                   // (calc: the converters have also read dO for delta)
-                    tc_fence_after();
-                    mma_split3_loop<kNC / 16, TERMS>(sdp, db, db + LO8, KS_K, LBO_K, SBO_K,
-                                                     vb, vb + LO8, KS_K, LBO_K, SBO_K, id_kk_s, n > 0, LAY, LAY);
-                    free_op(u);                                   // V is only needed by dP
-                    mbar_wait(&bars[B_O_EMPTY + (oc & 1)], ((oc >> 1) & 1) ^ 1);
-                    tc_fence_after();
-                    mma_split3_loop<LK / 16, TERMS>(tmem + kTmemO + (oc & 1) * kNC, pb, pb + LOP, 256, 128, T::kPlane,
-                                                    db, db + LO8, KS_MN, LBO_MN, SBO_MN, id_mn_mn, false, 0, LAY);
-                    commit_to(&bars[B_O_FULL + (oc & 1)]);
-                    free_op(u + 1);
-                    CCA_STAMP(2);
-                }
-                commit_to(&bars[B_DP_FULL]);
-                if (k + 1 < nk) issue_s(k + 1);                   // overlaps the dS computation of this item
-                // ---- phase D: dQ = dS K,  dK = dS^T Q      (dS in the P planes)
-                mbar_wait(&bars[B_DS_FULL], k & 1);
-                CCA_STAMP(2);
-                {
-                    const uint32_t q = opb(u), kk = opb(u + 1);
-                    wait_op(u); wait_op(u + 1);
-                    mbar_wait(&bars[B_QK_EMPTY + 0], (k & 1) ^ 1);
-                    mbar_wait(&bars[B_QK_EMPTY + 1], (k & 1) ^ 1);
-                    tc_fence_after();
-                    mma_split3_loop<LK / 16, TERMS>(tmem + kTmemQK, pb, pb + LOP, 2 * T::kPlane, T::kPlane, 128,
-                                                    kk, kk + LO8, KS_MN, LBO_MN, SBO_MN, id_k_mn, false, 0, LAY);
-                    commit_to(&bars[B_QK_FULL + 0]);
-                    free_op(u + 1);
-                    mma_split3_loop<LK / 16, TERMS>(tmem + kTmemQK + kNC, pb, pb + LOP, 256, 128, T::kPlane,
-                                                    q, q + LO8, KS_MN, LBO_MN, SBO_MN, id_mn_mn, false, 0, LAY);
-                    commit_to(&bars[B_QK_FULL + 1]);
-                    free_op(u);
-                    commit_to(&bars[B_P_EMPTY]);
-                    u += 2;
-                }
-                CCA_STAMP(2);
-            }
-        } else if (warp >= kWarpStore) {
-            // =============================== store warps (one lane each): the output staging slot -> global ===============================
-            // Two warps alternate items: while one waits for the global completion of its item's stores (to publish them), the
-            // other already issues the next item's tiles.
-            if (lane == 0) {
-                pdl_wait();                                // prep kernel complete: counters (and the first samples of dq/dk/dv) cleared
-                const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
-                int pending = -1;
-                // each store warp has its own STAGED barriers (a parity wait must never fall a whole phase pair behind)
-                const int sel = warp - kWarpStore;
-                uint32_t use[3] = {0, 0, 0};
-                for (int k = sel; k < nk; k += 2) {
-                    uint32_t c = (uint32_t)k * NO;         // global tile index (selects the staging slot)
-                    const Item it = item_of(k);
-                    const bool prod = p.out_mode == 1 && is_producer(it);
-                    const int zb = it.b + p.ahead;
-                    if (p.out_mode == 0 && zb < p.sp.B) {  // zero-ahead: this item's share of sample zb (dq, dk, dv)
-                        uint8_t *dst[3] = {p.dq + (long)zb * p.sb_q, p.dk + (long)zb * p.sb_q, p.dv + (long)zb * p.sb_v};
-                        for (int t = 0; t < 3; ++t) {
-                            const long sh = t < 2 ? p.share_q : p.share_v, sb = t < 2 ? p.sb_q : p.sb_v;
-                            const long lo = (long)it.j * sh;
-                            const long hi = lo + sh < sb ? lo + sh : sb;
-                            for (long o = lo; o < hi; o += kZeroBuf)
-                                bulk_store(dst[t] + o, smem + S::off_zero, (uint32_t)(hi - o < kZeroBuf ? hi - o : kZeroBuf));
-                        }
-                        tma_store_commit();
-                        pending = zb;
-                    }
-                    for (int i = 0; i < NO; ++i, ++c) {
-                        // output tile i of the item: i < NCH -> dV chunk i (rows = key pixels); NCH -> dQ (query pixels); NCH+1 -> dK
-                        const CUtensorMap *m = i < NCH ? (it.col ? &mdvc : &mdvr) : (i == NCH ? (it.col ? &mdqc : &mdqr) : (it.col ? &mdkc : &mdkr));
-                        const int c0 = i < NCH ? i * kNC : 0;
-                        const int start = i == NCH ? it.q0 : it.k0;
-                        const int cw = it.col ? it.line : start, ch = it.col ? start : it.line;
-                        const int os = c % kNOut;
-                        uint8_t *slot = smem + S::off_out + os * T::kSlot;
-                        mbar_wait(&bars[B_STAGED_W + sel * 3 + os], use[os] & 1);
-                        ++use[os];
-                        if (i == 0) {
-                            if (pending >= 0) {
-                                tma_store_wait_all<0>();
-                                publish_count(p.zdone + pending);
-                                pending = -1;
-                            }
-                            if (p.out_mode == 0 && it.b >= p.ahead) {
-                                wait_count(p.zdone + it.b, (unsigned)p.sp.per_sample);
-                                fence_proxy_async_all();
-                            }
-                            if (p.out_mode == 1 && !prod) {    // every producer of this sample has stored its tiles
-                                wait_count(p.cdone + it.b, (unsigned)p.sp.seg0);
-                                fence_proxy_async_all();
-                            }
-                        }
-                        if (prod) {
-                            if (p.hints) {
-                                tma_store_4d(m, slot, c0, cw, ch, it.b, pol_keep);
-                                if constexpr (!BF) tma_store_4d(m, slot + T::kTile, c0 + 32, cw, ch, it.b, pol_keep);
-                            } else {
-                                tma_store_4d(m, slot, c0, cw, ch, it.b);
-                                if constexpr (!BF) tma_store_4d(m, slot + T::kTile, c0 + 32, cw, ch, it.b);
-                            }
-                        } else if (p.hints && p.out_mode == 1) {   // the one and only add onto these lines: they are final
-                            tma_reduce_add_4d(m, slot, c0, cw, ch, it.b, pol_stream);
-                            if constexpr (!BF) tma_reduce_add_4d(m, slot + T::kTile, c0 + 32, cw, ch, it.b, pol_stream);
-                        } else {
-                            tma_reduce_add_4d(m, slot, c0, cw, ch, it.b);
-                            if constexpr (!BF) tma_reduce_add_4d(m, slot + T::kTile, c0 + 32, cw, ch, it.b);
-                        }
-                        tma_store_commit();
-                        tma_store_wait_read<0>();          // the tile has been read out of shared memory: hand the slot back
-                        mbar_arrive(&bars[B_OUT_FREE + os]);
-                    }
-                    if (prod) {                            // publish: all stores of this item have completed
-                        tma_store_wait_all<0>();
-                        publish_count(p.cdone + it.b);
-                    }
-                }
-                tma_store_wait_all<0>();
-                if (pending >= 0) publish_count(p.zdone + pending);
-            }
-        }
-    } else if (warp >= kWarpConv0) {
-        // =============================== converters (256 threads) ===============================
-        reg_dec<kRegsConvB>();
-        const int t = tid - kWarpConv0 * 32;
-        int dbg_n = t == 0 ? 0 : 512;
-        (void)dbg_n;
-        uint32_t g = 0, ncalc = 0;
-        // every ring slot passes through the converters (bf16 tiles only for the hand-shake: OP_FULL is what the MMA warp
-        // waits for in both dtypes, so a slot the converters read for delta is never released before they are done).
-        uint32_t pend = 0;                                             // bit s: slot s converted, not yet published
-        auto publish = [&]() {
-            if (pend) {
-                if constexpr (!BF) fence_proxy_async();
-                for (int sl = 0; sl < kNLd; ++sl)
-                    if (pend & (1u << sl)) mbar_arrive(&bars[B_OP_FULL + sl]);
-                pend = 0;
-            }
-        };
-        auto wait_full = [&](uint32_t gg) {
-            const int slot = gg % kNLd;
-            if (!mbar_try_wait(&bars[B_LD_FULL + slot], (gg / kNLd) & 1)) {
-                publish();
-                mbar_wait(&bars[B_LD_FULL + slot], (gg / kNLd) & 1);
-            }
-        };
-        auto conv = [&](int count) {
-            for (int e = 0; e < count; ++e, ++g) {
+            uint32_t g = 0;
+            auto ring = [&](const CUtensorMap *m, int c0, const Item &it, int start, bool last_use) {
                 const int slot = g % kNLd;
-                wait_full(g);
-                CCA_STAMP(1);
-                if constexpr (!BF) {
-                    convert_slot_inplace<LK>(smem + S::off_ld + slot * T::kSlot, t);
-                    pend |= 1u << slot;
-                    publish();                                         // (deferring it past the next slot's loads cost 7 % here)
-                } else {
-                    mbar_arrive(&bars[B_OP_FULL + slot]);              // bf16: nothing to convert, nothing to fence
-                }
-                CCA_STAMP(1);
-            }
-        };
-        if (nk > 0) conv(2);
-        for (int k = 0; k < nk; ++k) {
-            const bool calc = calc_delta(p, item_of(k));
-            float dacc = 0.f;
-            for (int n = 0; n < NCH; ++n) {
-                conv(1);                                               // V
-                if (calc) {                                            // dO + O: dot products, then dO as operand
-                    const int sd = g % kNLd, so = (g + 1) % kNLd;
-                    wait_full(g);
-                    wait_full(g + 1);
-                    publish();
-                    dacc += convert_dot<LK, BF>(smem + S::off_ld + sd * T::kSlot, smem + S::off_ld + so * T::kSlot, t, &bars[B_LD_EMPTY + so],
-                                                o_cnt + so);
-                    if constexpr (!BF) {
-                        pend |= (1u << sd) | (1u << so);               // (nobody waits for the O slot; keeps its phase in step)
-                        publish();
-                    } else {
-                        mbar_arrive(&bars[B_OP_FULL + sd]);
-                        mbar_arrive(&bars[B_OP_FULL + so]);
-                    }
-                    g += 2;
-                } else {
-                    conv(1);                                           // dO
+                mbar_wait(&empty[slot], ((g / kNLd) & 1) ^ 1);
+                mbar_expect_tx(&full[slot], T::kSlot);
+                load(smem + S::off_ld + slot * T::kSlot, &full[slot], m, c0, it, start, last_use);
+                ++g;
+            };
+            for (int k = 0; k < nk; ++k) {
+                const Item it = item_of(k);
+                const bool calc = calc_delta(p, it);
+                mbar_wait(qk_empty, (k & 1) ^ 1);
+                mbar_expect_tx(qk_full, 2 * T::kSlot);
+                load(smem + S::off_qk, qk_full, it.col ? &mqc : &mqr, 0, it, it.q0, false);
+                load(smem + S::off_qk + T::kSlot, qk_full, it.col ? &mkc : &mkr, 0, it, it.k0, false);
+                for (int n = 0; n < NCH; ++n) {
+                    ring(it.col ? &mvc : &mvr, n * kNC, it, it.k0, false);
+                    ring(it.col ? &mdoc : &mdor, n * kNC, it, it.q0, false);
+                    if (calc) ring(it.col ? &moc : &mor, n * kNC, it, it.q0, p.delta_mode == 1);   // (mode 1: nobody reads O again)
                 }
             }
-            if (calc) {                                                // hand the per-pixel sums to the P/dS group
-                publish();                                             // (never block on anything but a load with a slot withheld)
-                mbar_wait(&bars[B_DELTA_EMPTY], (ncalc & 1) ^ 1);
-                dpart[(t >> 7) * 128 + (t & 127)] = dacc;          // (t >> 7) = 2 * group + channel half
-                mbar_arrive(&bars[B_DELTA_FULL]);
-                ++ncalc;
-            }
-            if (k + 1 < nk) conv(2);
-            conv(2);
         }
-        publish();
-    } else if (warp >= 4) {
-        // =============================== P / dS group (128 threads, TMEM lane == query pixel) ===============================
-        reg_inc<kRegsSoft>();
-        const int r = tid - 128;
-        const uint32_t tl = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-        int dbg_n = r == 0 ? 0 : 512;
-        (void)dbg_n;
-        uint32_t ncalc = 0;
-        pdl_wait();                                                   // counters / delta buffer belong to this call from here on
+    } else if (tid >= 128) {
+        // =============================== consumers (warpgroup wg = rows [64 wg, 64 wg + 64) of each product) ===============================
+        const int t = tid - 128, wg = t >> 7, wq = (t >> 5) & 3;
+        const int rbase = 64 * wg + 16 * wq + (lane >> 2);         // accumulator rows rbase, rbase + 8
+        const int cq = 2 * (lane & 3);                             // first accumulator column of this thread (+ 8j)
+        const uint32_t qb = smem_u32(smem + S::off_qk), kb = qb + T::kSlot, ld_base = smem_u32(smem + S::off_ld);
+        const uint32_t pb = smem_u32(smem + S::off_p);
+        uint8_t *pgen = smem + S::off_p;
+        E *const dq = reinterpret_cast<E *>(p.dq), *const dk = reinterpret_cast<E *>(p.dk), *const dv = reinterpret_cast<E *>(p.dv);
+        pdl_wait();                                                // prep kernel complete: counters (and the outputs) cleared
+        uint32_t g = 0;
         for (int k = 0; k < nk; ++k) {
             const Item it = item_of(k);
             const bool calc = calc_delta(p, it);
-            const bool rvalid = r < it.lq;
-            const long pix = item_pixel(p.sp, it, rvalid ? r : 0);
-            const float nlse = rvalid ? -p.lse[pix] * kLog2e : -INFINITY;     // rows beyond the tile: P = exp2(-inf) = 0
-            const int self = it.col ? it.q0 + r - it.k0 : -1;
-            // predicated path only for the 16-key chunks holding the tail of the key block or the self entry of one of this
-            // warp's 32 query pixels (warp-uniform test); see cca_tc_fwd.cu
-            const int sw0 = it.col ? it.q0 - it.k0 + 32 * (warp & 3) : -(1 << 20);
-            uint8_t *ph = smem + S::off_p + r * 16, *pl = ph + T::kPP * T::kPlane;
-            // ---------------- P = exp(S - lse)
-            const uint32_t tsd = tl + (k & 1) * 128;           // S(k) / dP(k) buffer
-            CCA_STAMP(3);
-            mbar_wait(&bars[B_S_FULL + (k & 1)], (k >> 1) & 1);
-            tc_fence_after();
-            CCA_STAMP(3);
-            // both phases stream the TMEM row 16 columns at a time (small loops: the instruction footprint of a fully
-            // unrolled LK-element register array cost more than the extra tcgen05.wait::ld round trips)
-            float nx[16];                                      // next 16 columns, in flight while the current ones are processed
-            tmem_ld16(tsd, reinterpret_cast<uint32_t *>(nx));
-            mbar_wait(&bars[B_P_EMPTY], (k & 1) ^ 1);
+            const bool prod = p.out_mode == 1 && is_producer(it);
+            Item kit = it;                                         // key pixels of the item as "query rows" (pixel addressing)
+            kit.q0 = it.k0;
+            long qpix[2], kpix[2];
+            bool qok[2], kok[2];
+            float nlse[2];
+            int self[2];
 #pragma unroll
-            for (int c0 = 0; c0 < LK; c0 += 16) {
-                float s[16];
-                tmem_ld_wait16(reinterpret_cast<uint32_t *>(nx));
-#pragma unroll
-                for (int e = 0; e < 16; ++e) s[e] = nx[e];
-                if (c0 + 16 < LK) tmem_ld16(tsd + c0 + 16, reinterpret_cast<uint32_t *>(nx));
-                if (!((c0 + 16 > it.lk) || (c0 + 16 > sw0 && c0 < sw0 + 32))) {
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) s[e] = exp2f(fmaf(s[e], kLog2e, nlse));
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) {
-                        const int j = c0 + e;
-                        s[e] = (j < it.lk && j != self) ? exp2f(fmaf(s[e], kLog2e, nlse)) : 0.f;
+            for (int h = 0; h < 2; ++h) {
+                const int r = rbase + 8 * h;
+                qok[h] = r < it.lq; kok[h] = r < it.lk;
+                qpix[h] = item_pixel(p.sp, it, qok[h] ? r : 0);
+                kpix[h] = item_pixel(p.sp, kit, kok[h] ? r : 0);
+                nlse[h] = qok[h] ? -p.lse[qpix[h]] * kLog2e : 0.f;
+                self[h] = it.col ? it.q0 + r - it.k0 : -1;
+            }
+            // ---------------- S = Q K^T, P = exp(S - lse) -> planes
+            mbar_wait(qk_full, k & 1);
+            if constexpr (!BF) {
+                convert_slot<LK, BF>(smem + S::off_qk, t);
+                convert_slot<LK, BF>(smem + S::off_qk + T::kSlot, t);
+            }
+            {
+                float acc[LK / 2];
+                wg_fence();
+                for (int ks = 0; ks < KQ; ++ks) {
+                    wgmma_ss<LK>(acc, desc_kmaj<LK, BF>(qb, 64 * wg, ks, false), desc_kmaj<LK, BF>(kb, 0, ks, false), ks > 0, 0, 0);
+                    if constexpr (TERMS == 3) {
+                        wgmma_ss<LK>(acc, desc_kmaj<LK, BF>(qb, 64 * wg, ks, false), desc_kmaj<LK, BF>(kb, 0, ks, true), 1, 0, 0);
+                        wgmma_ss<LK>(acc, desc_kmaj<LK, BF>(qb, 64 * wg, ks, true), desc_kmaj<LK, BF>(kb, 0, ks, false), 1, 0, 0);
                     }
                 }
-                if (r < LK) {
+                wg_commit();
+                wg_wait<0>();
+                wg_acc_fence<LK / 2>(acc);
+#pragma unroll
+                for (int j = 0; j < LK / 8; ++j)
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
-                        const int kc = c0 / 8 + h;
-                        const float *v8 = s + h * 8;
-                        if constexpr (BF) {
-                            *reinterpret_cast<uint4 *>(ph + kc * T::kPlane) =
-                                make_uint4(pack_bf16(v8[0], v8[1]), pack_bf16(v8[2], v8[3]), pack_bf16(v8[4], v8[5]), pack_bf16(v8[6], v8[7]));
-                        } else {
-                            uint4 hi, lo;
-                            split8(v8, hi, lo);
-                            *reinterpret_cast<uint4 *>(ph + kc * T::kPlane) = hi;
-                            *reinterpret_cast<uint4 *>(pl + kc * T::kPlane) = lo;
+                        const int r = rbase + 8 * h, c = 8 * j + cq;
+                        const bool ok0 = qok[h] && c < it.lk && c != self[h];
+                        const bool ok1 = qok[h] && c + 1 < it.lk && c + 1 != self[h];
+                        const float p0 = ok0 ? exp2f(fmaf(acc[4 * j + 2 * h], kLog2e, nlse[h])) : 0.f;
+                        const float p1 = ok1 ? exp2f(fmaf(acc[4 * j + 2 * h + 1], kLog2e, nlse[h])) : 0.f;
+                        if (r < LK) {
+                            uint8_t *d = pgen + j * T::kPlane + r * 16 + cq * 2;
+                            if constexpr (BF) {
+                                *reinterpret_cast<uint32_t *>(d) = pack_bf16(p0, p1);
+                            } else {
+                                uint32_t hi, lo;
+                                split2(p0, p1, hi, lo);
+                                *reinterpret_cast<uint32_t *>(d) = hi;
+                                *reinterpret_cast<uint32_t *>(d + LOP) = lo;
+                            }
                         }
                     }
-                }
             }
-            tc_fence_before();
             fence_proxy_async();
-            mbar_arrive(&bars[B_P_FULL]);
-            CCA_STAMP(3);
-            // ---------------- delta of this query pixel
-            float dl = 0.f;
+            consumers_sync();
+            if (!prod && p.out_mode == 1) wait_count(p.cdone + it.b, (unsigned)p.sp.seg0);   // producers of the sample have stored
+            // ---------------- per chunk: dP += dO V^T, dV = P^T dO
+            float dp[LK / 2];
+            float dacc = 0.f;
+            for (int n = 0; n < NCH; ++n) {
+                const uint32_t gv = g++, gd = g++, go = calc ? g++ : 0;
+                mbar_wait(&full[gv % kNLd], (gv / kNLd) & 1);
+                mbar_wait(&full[gd % kNLd], (gd / kNLd) & 1);
+                if (calc) mbar_wait(&full[go % kNLd], (go / kNLd) & 1);
+                uint8_t *vs = smem + S::off_ld + (gv % kNLd) * T::kSlot, *ds = smem + S::off_ld + (gd % kNLd) * T::kSlot;
+                if constexpr (!BF) convert_slot<LK, BF>(vs, t);
+                if (calc) {
+                    dacc += convert_slot<LK, BF>(ds, t, smem + S::off_ld + (go % kNLd) * T::kSlot);
+                    if constexpr (BF) consumers_sync();            // (fp32: the conversion ends on a consumer barrier)
+                    mbar_arrive(&empty[go % kNLd]);
+                } else if constexpr (!BF) {
+                    convert_slot<LK, BF>(ds, t);
+                }
+                const uint32_t vb = ld_base + (gv % kNLd) * T::kSlot, db = ld_base + (gd % kNLd) * T::kSlot;
+                float o[32];
+                wg_fence();
+#pragma unroll
+                for (int ks = 0; ks < kNC / 16; ++ks) {
+                    wgmma_ss<LK>(dp, desc_kmaj<LK, BF>(db, 64 * wg, ks, false), desc_kmaj<LK, BF>(vb, 0, ks, false), n > 0 || ks > 0, 0, 0);
+                    if constexpr (TERMS == 3) {
+                        wgmma_ss<LK>(dp, desc_kmaj<LK, BF>(db, 64 * wg, ks, false), desc_kmaj<LK, BF>(vb, 0, ks, true), 1, 0, 0);
+                        wgmma_ss<LK>(dp, desc_kmaj<LK, BF>(db, 64 * wg, ks, true), desc_kmaj<LK, BF>(vb, 0, ks, false), 1, 0, 0);
+                    }
+                }
+#pragma unroll
+                for (int ks = 0; ks < KP; ++ks) {
+                    const uint32_t pa = pb + 8 * wg * T::kPlane + ks * 256;      // P^T: rows = key pixels [64 wg, +64), k = query rows
+                    wgmma_ss_n64(o, smem_desc(pa, 128, T::kPlane), desc_mnmaj<LK, BF>(db, ks, false), ks > 0, 1, 1);
+                    if constexpr (TERMS == 3) {
+                        wgmma_ss_n64(o, smem_desc(pa, 128, T::kPlane), desc_mnmaj<LK, BF>(db, ks, true), 1, 1, 1);
+                        wgmma_ss_n64(o, smem_desc(pa + LOP, 128, T::kPlane), desc_mnmaj<LK, BF>(db, ks, false), 1, 1, 1);
+                    }
+                }
+                wg_commit();
+                wg_wait<0>();
+                wg_acc_fence<LK / 2>(dp);
+                wg_acc_fence<32>(o);
+                mbar_arrive(&empty[gv % kNLd]);
+                mbar_arrive(&empty[gd % kNLd]);
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    if (kok[h]) {
+                        E *row = dv + kpix[h] * p.C + n * kNC + cq;
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) put2(row + 8 * j, o[4 * j + 2 * h], o[4 * j + 2 * h + 1], !prod);
+                    }
+            }
+            // ---------------- delta of the query rows
+            float dl[2] = {0.f, 0.f};
             if (calc) {
-                mbar_wait(&bars[B_DELTA_FULL], ncalc & 1);
-                dl = (dpart[r] + dpart[128 + r]) + (dpart[256 + r] + dpart[384 + r]);
-                mbar_arrive(&bars[B_DELTA_EMPTY]);
-                ++ncalc;
-                // delta[B,H,W] always ends up in the workspace (the caller's d gamma = sum of it); in mode 1 it is also how the
-                // other items of the sample get it
-                if (rvalid && is_producer(it)) p.delta[pix] = dl;
+                dsum[(t >> 7) * 128 + (t & 127)] = dacc;
+                consumers_sync();
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = rbase + 8 * h;
+                    dl[h] = dsum[r] + dsum[128 + r];
+                    // delta[B,H,W] always ends up in the workspace (the caller's d gamma = sum of it); in mode 1 it is also how
+                    // the other items of the sample get it
+                    if (qok[h] && is_producer(it) && (lane & 3) == 0) p.delta[qpix[h]] = dl[h];
+                }
                 if (p.delta_mode == 1) {
-                    named_bar_sync(2, 128);
-                    if (r == 0) { __threadfence(); atomicAdd(p.ddone + it.b, 1u); }
+                    __threadfence();
+                    consumers_sync();
+                    if (t == 0) atomicAdd(p.ddone + it.b, 1u);
                 }
             } else {
                 wait_count(p.ddone + it.b, (unsigned)p.sp.seg0);
-                if (rvalid) dl = __ldcg(p.delta + pix);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) dl[h] = qok[h] ? __ldcg(p.delta + qpix[h]) : 0.f;
             }
-            // ---------------- dS = P * (dP - delta)   (all MMAs that read P have completed: DP_FULL is committed after them)
-            mbar_wait(&bars[B_DP_FULL], k & 1);
-            tc_fence_after();
-            CCA_STAMP(3);
-            tmem_ld16(tsd, reinterpret_cast<uint32_t *>(nx));
+            // ---------------- dS = P * (dP - delta) -> planes (every dV product of both warpgroups has read P)
+            consumers_sync();
 #pragma unroll
-            for (int c0 = 0; c0 < LK; c0 += 16) {
-                float dp[16];
-                tmem_ld_wait16(reinterpret_cast<uint32_t *>(nx));
+            for (int j = 0; j < LK / 8; ++j)
 #pragma unroll
-                for (int e = 0; e < 16; ++e) dp[e] = nx[e];
-                if (c0 + 16 < LK) tmem_ld16(tsd + c0 + 16, reinterpret_cast<uint32_t *>(nx));
-                if (r < LK) {
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int kc = c0 / 8 + h;
-                        const uint4 hi = *reinterpret_cast<const uint4 *>(ph + kc * T::kPlane);
-                        uint4 lo = make_uint4(0, 0, 0, 0);
-                        if constexpr (!BF) lo = *reinterpret_cast<const uint4 *>(pl + kc * T::kPlane);
-                        const uint32_t hw[4] = {hi.x, hi.y, hi.z, hi.w}, lw[4] = {lo.x, lo.y, lo.z, lo.w};
-                        float ds[8];
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const float p0 = bf_lo(hw[e]) + bf_lo(lw[e]), p1 = bf_hi(hw[e]) + bf_hi(lw[e]);
-                            ds[2 * e] = p0 * (dp[h * 8 + 2 * e] - dl);       // masked / padded entries have P == 0 exactly
-                            ds[2 * e + 1] = p1 * (dp[h * 8 + 2 * e + 1] - dl);
-                        }
+                for (int h = 0; h < 2; ++h) {
+                    const int r = rbase + 8 * h;
+                    if (r < LK) {
+                        uint8_t *d = pgen + j * T::kPlane + r * 16 + cq * 2;
+                        const uint32_t hw = *reinterpret_cast<const uint32_t *>(d);
+                        const uint32_t lw = BF ? 0u : *reinterpret_cast<const uint32_t *>(d + LOP);
+                        const float p0 = bf_lo(hw) + bf_lo(lw), p1 = bf_hi(hw) + bf_hi(lw);
+                        // masked / padded entries have P == 0 exactly; rows past the tile are cleared (their dP is not defined)
+                        const float s0 = qok[h] ? p0 * (dp[4 * j + 2 * h] - dl[h]) : 0.f;
+                        const float s1 = qok[h] ? p1 * (dp[4 * j + 2 * h + 1] - dl[h]) : 0.f;
                         if constexpr (BF) {
-                            *reinterpret_cast<uint4 *>(ph + kc * T::kPlane) =
-                                make_uint4(pack_bf16(ds[0], ds[1]), pack_bf16(ds[2], ds[3]), pack_bf16(ds[4], ds[5]), pack_bf16(ds[6], ds[7]));
+                            *reinterpret_cast<uint32_t *>(d) = pack_bf16(s0, s1);
                         } else {
-                            uint4 dh, dlo;
-                            split8(ds, dh, dlo);
-                            *reinterpret_cast<uint4 *>(ph + kc * T::kPlane) = dh;
-                            *reinterpret_cast<uint4 *>(pl + kc * T::kPlane) = dlo;
+                            uint32_t hi, lo;
+                            split2(s0, s1, hi, lo);
+                            *reinterpret_cast<uint32_t *>(d) = hi;
+                            *reinterpret_cast<uint32_t *>(d + LOP) = lo;
+                        }
+                    }
+                }
+            fence_proxy_async();
+            consumers_sync();
+            // ---------------- dQ = dS K (rows = query pixels), dK = dS^T Q (rows = key pixels)
+            {
+                float aq[32], ak[32];
+                wg_fence();
+#pragma unroll
+                for (int ks = 0; ks < KP; ++ks) {
+                    const uint32_t a = pb + 64 * wg * 16 + ks * 2 * T::kPlane;     // dS, K-major (k = key pixels)
+                    wgmma_ss_n64(aq, smem_desc(a, T::kPlane, 128), desc_mnmaj<LK, BF>(kb, ks, false), ks > 0, 0, 1);
+                    if constexpr (TERMS == 3) {
+                        wgmma_ss_n64(aq, smem_desc(a, T::kPlane, 128), desc_mnmaj<LK, BF>(kb, ks, true), 1, 0, 1);
+                        wgmma_ss_n64(aq, smem_desc(a + LOP, T::kPlane, 128), desc_mnmaj<LK, BF>(kb, ks, false), 1, 0, 1);
+                    }
+                    const uint32_t at = pb + 8 * wg * T::kPlane + ks * 256;         // dS^T, MN-major (k = query pixels)
+                    wgmma_ss_n64(ak, smem_desc(at, 128, T::kPlane), desc_mnmaj<LK, BF>(qb, ks, false), ks > 0, 1, 1);
+                    if constexpr (TERMS == 3) {
+                        wgmma_ss_n64(ak, smem_desc(at, 128, T::kPlane), desc_mnmaj<LK, BF>(qb, ks, true), 1, 1, 1);
+                        wgmma_ss_n64(ak, smem_desc(at + LOP, 128, T::kPlane), desc_mnmaj<LK, BF>(qb, ks, false), 1, 1, 1);
+                    }
+                }
+                wg_commit();
+                wg_wait<0>();
+                wg_acc_fence<32>(aq);
+                wg_acc_fence<32>(ak);
+                mbar_arrive(qk_empty);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        const int c = 8 * j + cq;
+                        if (c < p.Cq) {
+                            if (qok[h]) put2(dq + qpix[h] * p.Cq + c, aq[4 * j + 2 * h], aq[4 * j + 2 * h + 1], !prod);
+                            if (kok[h]) put2(dk + kpix[h] * p.Cq + c, ak[4 * j + 2 * h], ak[4 * j + 2 * h + 1], !prod);
                         }
                     }
                 }
             }
-            tc_fence_before();
-            mbar_arrive(&bars[B_S_EMPTY + (k & 1)]);
-            fence_proxy_async();
-            mbar_arrive(&bars[B_DS_FULL]);
-            CCA_STAMP(3);
-        }
-    } else {
-        // =============================== epilogue group (128 threads, TMEM lane == output pixel) ===============================
-        reg_inc<kRegsEpi>();
-        const int r = tid;
-        const uint32_t tl = tmem + ((uint32_t)(warp * 32) << 16);
-        uint32_t oc = 0, nt = 0;                              // dV accumulators consumed, tiles staged
-        int dbg_n = tid == 0 ? 0 : 512;
-        (void)dbg_n;
-        for (int k = 0; k < nk; ++k) {
-            for (int i = 0; i < NO; ++i, ++nt) {
-                const bool qk = i >= NCH;                     // dQ (i == NCH), dK (NCH + 1): accumulators of their own
-                const int ob = oc & 1;
-                const int os = nt % kNOut;
-                uint8_t *slot = smem + S::off_out + os * T::kSlot;
-                CCA_STAMP(4);
-                mbar_wait(&bars[B_OUT_FREE + os], ((nt / kNOut) & 1) ^ 1);   // the store of tile nt - kNOut has left the slot
-                if (qk) mbar_wait(&bars[B_QK_FULL + (i - NCH)], k & 1);
-                else mbar_wait(&bars[B_O_FULL + ob], (oc >> 1) & 1);
-                tc_fence_after();
-                CCA_STAMP(4);
-                float o[kNC];
-                const uint32_t src = tl + (qk ? kTmemQK + (i - NCH) * kNC : kTmemO + ob * kNC);
-#pragma unroll
-                for (int c0 = 0; c0 < kNC; c0 += 16) tmem_ld16(src + c0, reinterpret_cast<uint32_t *>(o + c0));
-                tmem_ld_wait();
-                tc_fence_before();
-                if (qk) mbar_arrive(&bars[B_QK_EMPTY + (i - NCH)]);
-                else { mbar_arrive(&bars[B_O_EMPTY + ob]); ++oc; }
-                // rows beyond the tile are exact zeros (P and dS are zero there): inside the image they add nothing, outside the
-                // TMA clips them
-                if (r < LK) {
-                    uint8_t *row = slot + r * 128;
-                    const int sw = r & 7;
-                    if constexpr (BF) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j)
-                            *reinterpret_cast<uint4 *>(row + ((j ^ sw) * 16)) =
-                                make_uint4(pack_bf16(o[8 * j], o[8 * j + 1]), pack_bf16(o[8 * j + 2], o[8 * j + 3]),
-                                           pack_bf16(o[8 * j + 4], o[8 * j + 5]), pack_bf16(o[8 * j + 6], o[8 * j + 7]));
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j)
-                            *reinterpret_cast<float4 *>(row + (j >> 3) * T::kTile + (((j & 7) ^ sw) * 16)) =
-                                make_float4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
-                    }
-                }
-                fence_proxy_async();
-                mbar_arrive(&bars[B_STAGED_W + (k & 1) * 3 + os]);
-                CCA_STAMP(4);
-            }
+            if (prod) __threadfence();
+            consumers_sync();                                      // (also: the planes and dsum are free for the next item)
+            if (prod && t == 0) atomicAdd(p.cdone + it.b, 1u);     // publish: all stores of this item are visible
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc<kTmemCols>(tmem);
 }
 
-// Prologue of the backward: clears the first `head` samples of dq, dk, dv and the per-sample counters.
+// Prologue of the backward: clears the outputs (tiled lines) and the per-sample counters.
 __global__ void __launch_bounds__(256) cca_bwd_prep_kernel(uint4 *dq, uint4 *dk, uint4 *dv, long nq16, long nv16,
                                                            unsigned int *counters, int n_counters)
 {
@@ -709,50 +367,37 @@ __global__ void __launch_bounds__(256) cca_bwd_prep_kernel(uint4 *dq, uint4 *dk,
     for (long i = tid; i < n_counters; i += nth) counters[i] = 0u;
 }
 
-long long *g_bwd_dbg = nullptr;
-
 template <int LK, bool BF>
 cudaError_t launch_bwd(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse, float *delta,
-                       unsigned int *counters, void *dq, void *dk, void *dv, Dims d, int ahead, int delta_mode, cudaStream_t st,
+                       unsigned int *counters, void *dq, void *dk, void *dv, Dims d, int delta_mode, cudaStream_t st,
                        const char **why)
 {
-    CUtensorMap m[16];
-    const void *base[8] = {q, k, v, dout, out, dq, dk, dv};
-    const int ch[8] = {d.Cq, d.Cq, d.C, d.C, d.C, d.Cq, d.Cq, d.C};
+    CUtensorMap m[10];
+    const void *base[5] = {q, k, v, dout, out};
+    const int ch[5] = {d.Cq, d.Cq, d.C, d.C, d.C};
     BwdParams p;
     p.sp = make_space(d.B, d.H, d.W);
-    for (int t = 0; t < 8; ++t)
-        for (int r = 0; r < 2; ++r) {
-            // loads: LK-pixel boxes (zero-filled past the image); outputs: boxes of exactly one tile of the direction
-            const int rows = t < 5 ? LK : (r == 0 ? p.sp.col.tl : p.sp.row.tl);
-            if (!get_map(&m[2 * t + r], base[t], d.B, d.H, d.W, ch[t], rows, r == 0, BF)) {
+    for (int t = 0; t < 5; ++t)
+        for (int r = 0; r < 2; ++r)
+            // LK-pixel boxes, zero-filled past the line
+            if (!get_map(&m[2 * t + r], base[t], d.B, d.H, d.W, ch[t], LK, r == 0, BF)) {
                 if (why) *why = "cuTensorMapEncodeTiled failed";
                 return cudaErrorInvalidValue;
             }
-        }
     p.C = d.C; p.Cq = d.Cq;
     p.npix = (long)d.B * d.H * d.W;
     p.lse = lse; p.delta = delta;
-    p.zdone = counters; p.ddone = counters + d.B; p.cdone = counters + 2 * d.B;
+    p.ddone = counters; p.cdone = counters + d.B;
     p.delta_mode = delta_mode;
     const bool one_tile = p.sp.col.nt == 1 && p.sp.row.nt == 1;
     p.out_mode = one_tile ? 1 : 0;
-    // item order: lagged by default (measured 0.30 ms vs 0.35 ms at BASELINE config 2: the consumers' waits for their producers
-    // cost more than the larger L2 working set).  Zero-ahead (tiled lines) needs the plain order: an item of sample b waits for
-    // the zero shares issued by ALL items of sample b-1, and in the lagged order some of those come later in the walk.
-    p.lag = (p.out_mode == 1 && tc_lag() != 0) ? 1 : 0;
+    p.lag = tc_lag() != 0 ? 1 : 0;
     p.hints = tc_l2_hints();
-    p.dq = reinterpret_cast<uint8_t *>(dq); p.dk = reinterpret_cast<uint8_t *>(dk); p.dv = reinterpret_cast<uint8_t *>(dv);
+    p.dq = dq; p.dk = dk; p.dv = dv;
     const long es = BF ? 2 : 4;
-    p.sb_q = (long)d.H * d.W * d.Cq * es; p.sb_v = (long)d.H * d.W * d.C * es;
-    p.share_q = zero_share_bytes(p.sb_q, p.sp.per_sample); p.share_v = zero_share_bytes(p.sb_v, p.sp.per_sample);
-    p.ahead = ahead;
-    p.dbg = g_bwd_dbg;
-    // prologue: counters and (zero-ahead mode) the first `ahead` samples of the outputs
-    const int head = p.out_mode == 1 ? 0 : (ahead < d.B ? ahead : d.B);
+    const long nq = p.out_mode == 1 ? 0 : p.npix * d.Cq * es, nv = p.out_mode == 1 ? 0 : p.npix * d.C * es;
     cca_bwd_prep_kernel<<<p.out_mode == 1 ? 1 : sm_count(), 256, 0, st>>>(
-        reinterpret_cast<uint4 *>(dq), reinterpret_cast<uint4 *>(dk), reinterpret_cast<uint4 *>(dv), head * p.sb_q / 16,
-        head * p.sb_v / 16, counters, 3 * d.B);
+        reinterpret_cast<uint4 *>(dq), reinterpret_cast<uint4 *>(dk), reinterpret_cast<uint4 *>(dv), nq / 16, nv / 16, counters, 3 * d.B);
     count_launch();
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
@@ -768,15 +413,12 @@ cudaError_t launch_bwd(const void *dout, const void *q, const void *k, const voi
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = tc_pdl() ? 1 : 0;
-    e = cudaLaunchKernelEx(&cfg, kern, m[0], m[1], m[2], m[3], m[4], m[5], m[6], m[7], m[8], m[9], m[10], m[11], m[12], m[13],
-                           m[14], m[15], p);
+    e = cudaLaunchKernelEx(&cfg, kern, m[0], m[1], m[2], m[3], m[4], m[5], m[6], m[7], m[8], m[9], p);
     count_launch();
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 
 }  // namespace
-
-void set_tc_bwd_debug_buffer(void *p) { g_bwd_dbg = reinterpret_cast<long long *>(p); }
 
 bool tc_backward_supported(Dims d, int dtype) { return tc::shape_supported(d, dtype); }
 
@@ -797,15 +439,13 @@ cudaError_t tc_backward(const void *dout, const void *q, const void *k, const vo
     const ItemSpace sp = make_space(d.B, d.H, d.W);
     const int lk = lk_for(max_tile(sp));
     const bool bf = dtype == CCA_BF16;
-    int ahead = tc_zero_ahead();
-    if (ahead < 1) ahead = 1;
     int mode = tc_delta_mode();                       // -1: automatic = producers compute delta for their sample (the consumers
     if (mode < 0) mode = 1;                           // only ever wait for lower-indexed items, tiled or not)
     if (bf)
-        return lk == 80 ? launch_bwd<80, true>(dout, q, k, v, out, lse, delta, counters, dq, dk, dv, d, ahead, mode, st, why)
-                        : launch_bwd<112, true>(dout, q, k, v, out, lse, delta, counters, dq, dk, dv, d, ahead, mode, st, why);
-    return lk == 80 ? launch_bwd<80, false>(dout, q, k, v, out, lse, delta, counters, dq, dk, dv, d, ahead, mode, st, why)
-                    : launch_bwd<112, false>(dout, q, k, v, out, lse, delta, counters, dq, dk, dv, d, ahead, mode, st, why);
+        return lk == 80 ? launch_bwd<80, true>(dout, q, k, v, out, lse, delta, counters, dq, dk, dv, d, mode, st, why)
+                        : launch_bwd<112, true>(dout, q, k, v, out, lse, delta, counters, dq, dk, dv, d, mode, st, why);
+    return lk == 80 ? launch_bwd<80, false>(dout, q, k, v, out, lse, delta, counters, dq, dk, dv, d, mode, st, why)
+                    : launch_bwd<112, false>(dout, q, k, v, out, lse, delta, counters, dq, dk, dv, d, mode, st, why);
 }
 
 }  // namespace cca

@@ -1,42 +1,24 @@
-// Pieces shared by the tcgen05 forward and backward kernels (channels-last, fp32 I/O, bf16x3 split).
+// Pieces shared by the wgmma statistics, forward and backward kernels (channels-last, fp32 I/O as a bf16x3 split, or bf16 I/O).
 #pragma once
 #include <mutex>
 
 #include "cca_common.cuh"
-#include "cca_sm100.cuh"
+#include "cca_sm90.cuh"
 
 namespace cca {
 namespace tc {
-using namespace sm100;
+using namespace sm90;
 
 constexpr int kNC = 64;   // channels per chunk (one ring slot = [LK px][64 ch] fp32 = two swizzled TMA tiles)
-constexpr uint32_t kSw128 = 2;   // UMMA smem-descriptor layout type SWIZZLE_128B: a bf16 TMA tile [rows][128 B] is directly a
-                                 // K-major operand (rows = M/N, k-step = +32 B) or an MN-major one (rows = K, k-step = +2048 B)
 
-// Thread layout of the kernels (seven warpgroups, registers rebalanced with setmaxnreg):
-//   warps 0-3   (128 thr) : epilogue group        (TMEM lane == pixel; accumulators -> staging)
-//   warps 4-7   (128 thr) : softmax / P / dS group (TMEM lane == pixel)
-//   warps 8-23  (512 thr) : converters -- fp32 staging tile -> bf16 hi/lo operand planes.  The conversion is ~1200 warp
-//                           instructions per 28 KB slot and a slot used to take ~1000 cycles with 8 warps (two per scheduler,
-//                           mostly waiting on their own dependent instructions), which paced every fp32 chunk; 16 warps
-//                           halve the work per warp and double the warps a scheduler can pick from.
-//   warp 24               : TMA producer (one elected lane)
-//   warp 25               : MMA issuer (whole warp converged, tcgen05.mma under elect.sync)
-//   warps 26, 27          : store warps (one lane each, alternating items): staging slots -> global, counters
-constexpr int kThreads = 896;
-constexpr int kConvThreads = 512;
-constexpr int kWarpConv0 = 8, kWarpProducer = 24, kWarpMma = 25, kWarpStore = 26;
-constexpr int kRegsLaunch = 72;           // 65536 / 896 rounded down to a multiple of 8
-constexpr int kRegsMisc = 56;
-// setmaxnreg moves registers through a per-CTA pool that only holds what the CTA itself released: the increases must be
-// covered by the decreases relative to the launch allocation (kRegsLaunch per thread).
-constexpr bool reg_pool_ok(int soft, int epi, int conv)
-{
-    return kConvThreads * (kRegsLaunch - conv) + 128 * (kRegsLaunch - kRegsMisc) >= 128 * (soft - kRegsLaunch) + 128 * (epi - kRegsLaunch);
-}
-
-template <int N> __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
-template <int N> __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+// Thread layout of the attention kernels (three warpgroups):
+//   warpgroup 0           : TMA producer (one elected lane of warp 0), the rest idle
+//   warpgroups 1, 2       : consumers.  Consumer warpgroup w owns query rows [64w, 64w + 64) of an item's 128-row tile in
+//                           the wgmma accumulator layout; both convert fp32 tiles to bf16 operand planes together (256 threads)
+constexpr int kThreads = 384;
+constexpr int kConsumers = 256;
+constexpr int kBarConsumers = 1;   // named barrier of the 256 consumer threads
+constexpr int kBarConvert = 2;     // named barrier inside a conversion
 
 // BF = false: fp32 I/O, every operand split into bf16 hi + lo (3 MMAs per product).
 // BF = true : bf16 I/O, operands used as they are (1 MMA per product); a 64-channel chunk is ONE 128-byte-wide TMA tile.
@@ -79,93 +61,100 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads)
 {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-__device__ __forceinline__ bool elect_one()
-{
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n\t.reg .b32 rx;\n\t.reg .pred px;\n\t"
-        "elect.sync rx|px, %1;\n\t"
-        "selp.u32 %0, 1, 0, px;\n\t}"
-        : "=r"(pred) : "r"(0xFFFFFFFFu));
-    return pred != 0;
-}
+__device__ __forceinline__ void consumers_sync() { named_bar_sync(kBarConsumers, kConsumers); }
 
-// Converter: one staged slot ([LK px][64 ch] fp32 as two swizzled 32-channel TMA boxes) -> bf16 hi/lo operand planes
-// [8-channel chunk][pixel][16 B], IN PLACE.  Each box is rewritten inside its own bytes (planes hi0 lo0 .. hi3 lo3 of its 32
-// channels take exactly the box's LK x 128 B), so the two boxes are handled by two independent groups of 256 threads (group =
-// t >> 8; inside a group thread = (pixel row, 16-channel half)): every thread reads and splits its 64 B, the group meets on its
-// own named barrier (1 or 3), then overwrites.  `mid` runs after the loads have been issued and before the group barrier.
-struct ConvertNoMid { __device__ __forceinline__ void operator()() const {} };
-template <int LK, typename Mid = ConvertNoMid>
-__device__ __forceinline__ void convert_slot_inplace(uint8_t *slot, int t, Mid mid = Mid())
+// Conversion of one staged slot ([LK px][64 ch] fp32 as two swizzled 32-channel TMA boxes) into bf16 hi/lo operand planes
+// [8-channel chunk][pixel][16 B], IN PLACE, by the 256 consumer threads (thread t: pixel row t & 127, 32-channel half t >> 7 of
+// the slot, i.e. 16 channels of each box).  Every thread reads its 2 x 64 B, the consumers meet, then overwrite; the planes are
+// made visible to wgmma (async proxy) and every consumer has passed the closing barrier on return.
+// With `dot` (the O tile of the same pixels, same layout): returns this thread's part of sum_c slot[r][c] * dot[r][c].
+// bf16 slots need no conversion; only the dot product is computed.
+template <int LK, bool BF>
+__device__ __forceinline__ float convert_slot(uint8_t *slot, int t, const uint8_t *dot = nullptr)
 {
-    using T = Tiles<LK, false>;
-    const int grp = t >> 8, r = t & 127, hq = (t >> 7) & 1;
-    uint8_t *box = slot + grp * T::kTile;
-    float4 raw[4];                                              // the thread's 16 channels
-    {
-        const int rr = r < LK ? r : LK - 1;                     // idle threads re-read the last row (unconditional loads keep raw[] in registers)
-        const uint8_t *src = box + rr * 128;
-        const int sw = rr & 7;
+    using T = Tiles<LK, BF>;
+    const int r = t & 127, hq = t >> 7;
+    const int rr = r < LK ? r : LK - 1, sw = rr & 7;
+    float acc = 0.f;
+    if constexpr (BF) {
+        if (dot) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) raw[j] = *reinterpret_cast<const float4 *>(src + (((hq * 4 + j) ^ sw) * 16));
-    }
-    mid();
-    if (grp == 0) asm volatile("bar.sync 1, 256;" ::: "memory");
-    else asm volatile("bar.sync 3, 256;" ::: "memory");
-    if (r < LK) {
-        uint8_t *d = box + r * 16 + hq * 2 * T::kPStride;
+            for (int j = 0; j < 4; ++j) {
+                const int c = (hq * 4 + j) ^ sw;
+                const uint4 x = *reinterpret_cast<const uint4 *>(slot + rr * 128 + c * 16);
+                const uint4 y = *reinterpret_cast<const uint4 *>(dot + rr * 128 + c * 16);
+                const uint32_t xw[4] = {x.x, x.y, x.z, x.w}, yw[4] = {y.x, y.y, y.z, y.w};
 #pragma unroll
-        for (int j = 0; j < 2; ++j) {
-            const float4 a = raw[2 * j], b = raw[2 * j + 1];
-            const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-            uint4 hi, lo;
-            split8(v, hi, lo);
-            *reinterpret_cast<uint4 *>(d + j * T::kPStride) = hi;
-            *reinterpret_cast<uint4 *>(d + j * T::kPStride + T::kLoOff) = lo;
-        }
-    }
-}
-
-// D (+)= A*B with the bf16x3 split: Ah*Bh + Ah*Bl + Al*Bh (TERMS = 3), or just Ah*Bh for bf16 I/O (TERMS = 1).
-// Executed by the whole (converged) MMA warp.
-template <int TERMS = 3>
-__device__ __forceinline__ void mma_split3(uint32_t d, uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl,
-                                           uint32_t idesc, bool accumulate)
-{
-    if (elect_one()) {
-        mma_f16(d, ah, bh, idesc, accumulate);
-        if constexpr (TERMS == 3) {
-            mma_f16(d, ah, bl, idesc, true);
-            mma_f16(d, al, bh, idesc, true);
-        }
-    }
-    __syncwarp();
-}
-// Same, for a whole K loop: NK k-steps, descriptors advance by (a_step, b_step) bytes per step.  One election.
-template <int NK, int TERMS = 3>
-__device__ __forceinline__ void mma_split3_loop(uint32_t d, uint32_t a_hi, uint32_t a_lo, uint32_t a_step, uint32_t a_lbo, uint32_t a_sbo,
-                                                uint32_t b_hi, uint32_t b_lo, uint32_t b_step, uint32_t b_lbo, uint32_t b_sbo,
-                                                uint32_t idesc, bool accumulate_first, uint32_t a_layout = 0, uint32_t b_layout = 0)
-{
-    if (elect_one()) {
-#pragma unroll
-        for (int ks = 0; ks < NK; ++ks) {
-            const uint64_t ah = smem_desc(a_hi + ks * a_step, a_lbo, a_sbo, a_layout), al = smem_desc(a_lo + ks * a_step, a_lbo, a_sbo, a_layout);
-            const uint64_t bh = smem_desc(b_hi + ks * b_step, b_lbo, b_sbo, b_layout), bl = smem_desc(b_lo + ks * b_step, b_lbo, b_sbo, b_layout);
-            mma_f16(d, ah, bh, idesc, accumulate_first || ks > 0);
-            if constexpr (TERMS == 3) {
-                mma_f16(d, ah, bl, idesc, true);
-                mma_f16(d, al, bh, idesc, true);
+                for (int e = 0; e < 4; ++e) acc += bf_lo(xw[e]) * bf_lo(yw[e]) + bf_hi(xw[e]) * bf_hi(yw[e]);
             }
         }
+        return r < LK ? acc : 0.f;
+    } else {
+        float4 raw[8];
+#pragma unroll
+        for (int bx = 0; bx < 2; ++bx)
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                raw[4 * bx + j] = *reinterpret_cast<const float4 *>(slot + bx * T::kTile + rr * 128 + (((hq * 4 + j) ^ sw) * 16));
+        if (dot) {
+#pragma unroll
+            for (int bx = 0; bx < 2; ++bx)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float4 o = *reinterpret_cast<const float4 *>(dot + bx * T::kTile + rr * 128 + (((hq * 4 + j) ^ sw) * 16));
+                    const float4 x = raw[4 * bx + j];
+                    acc += x.x * o.x + x.y * o.y + x.z * o.z + x.w * o.w;
+                }
+        }
+        named_bar_sync(kBarConvert, kConsumers);
+        if (r < LK) {
+#pragma unroll
+            for (int bx = 0; bx < 2; ++bx) {
+                uint8_t *d = slot + bx * T::kTile + r * 16 + hq * 2 * T::kPStride;
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    const float4 a = raw[4 * bx + 2 * j], b = raw[4 * bx + 2 * j + 1];
+                    const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+                    uint4 hi, lo;
+                    split8(v, hi, lo);
+                    *reinterpret_cast<uint4 *>(d + j * T::kPStride) = hi;
+                    *reinterpret_cast<uint4 *>(d + j * T::kPStride + T::kLoOff) = lo;
+                }
+            }
+        }
+        fence_proxy_async();
+        consumers_sync();
+        return r < LK ? acc : 0.f;
     }
-    __syncwarp();
 }
-__device__ __forceinline__ void commit_to(uint64_t *bar)
+
+// Operand descriptors of a [LK px][64 ch] slot (bf16 tile or fp32 planes; `lo`: the lo planes), 16-element k-step ks:
+//   channels as the contraction (K-major, rows = pixels starting at row0)
+template <int LK, bool BF> __device__ __forceinline__ uint64_t desc_kmaj(uint32_t slot, int row0, int ks, bool lo)
 {
-    if (elect_one()) mma_commit(bar);
-    __syncwarp();
+    using T = Tiles<LK, BF>;
+    if constexpr (BF) return smem_desc(slot + row0 * 128 + ks * 32, 16, 1024, kSw128);
+    else return smem_desc(slot + row0 * 16 + ks * 2 * T::kPStride + (lo ? T::kLoOff : 0), T::kPStride, 128);
+}
+//   pixels as the contraction (MN-major: the 64 channels are the N dimension)
+template <int LK, bool BF> __device__ __forceinline__ uint64_t desc_mnmaj(uint32_t slot, int ks, bool lo)
+{
+    using T = Tiles<LK, BF>;
+    if constexpr (BF) return smem_desc(slot + ks * 2048, 16, 1024, kSw128);
+    else return smem_desc(slot + ks * 256 + (lo ? T::kLoOff : 0), 128, T::kPStride);
+}
+
+// global row stores of the accumulator layout: two consecutive channels per thread
+__device__ __forceinline__ void put2(float *p, float a, float b, bool add)
+{
+    if (add) atomicAdd(reinterpret_cast<float2 *>(p), make_float2(a, b));
+    else *reinterpret_cast<float2 *>(p) = make_float2(a, b);
+}
+__device__ __forceinline__ void put2(__nv_bfloat16 *p, float a, float b, bool add)
+{
+    const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+    if (add) atomicAdd(reinterpret_cast<__nv_bfloat162 *>(p), v);
+    else *reinterpret_cast<__nv_bfloat162 *>(p) = v;
 }
 
 // ---- host: TMA tensor maps over channels-last fp32 tensors -------------------------------------

@@ -1,4 +1,4 @@
-// tcgen05 / TMA forward (values) kernel of criss-cross attention for sm_100a (channels-last tensors).
+// wgmma / TMA forward (values) kernel of criss-cross attention for sm_90a (channels-last tensors).
 //
 // Layout: q,k [B,H,W,Cq], v,out [B,H,W,C] (torch channels_last).  In this layout an image row and an image column are
 // the same object -- L pixels with a fixed pixel stride, each pixel's channels contiguous -- so one kernel serves both
@@ -7,34 +7,27 @@
 // Formulation (DESIGN.md 3): the statistics pre-pass (cca_tc_stats.cu) has left the log-sum-exp of every pixel's logits
 // per (direction, key block).  An item (cca_items.cuh: direction, sample, line, query tile, key block) combines those few
 // planes into the pixel's final lse and computes its share of the output with the FINAL normalisation,
-//     P = exp(S - lse)        O_item = P V_block        out[query pixels] += O_item      (TMA reduce-add, at L2)
+//     P = exp(S - lse)        O_item = P V_block        out[query pixels] += O_item
 // so items never exchange anything: no partial output is written and read back, no per-pixel merge, and lines longer
 // than one tile are just more items.  ONE persistent launch walks the items sample by sample: the second direction of a
-// sample finds q,k,v in L2 and adds onto output lines that are still L2-resident, so DRAM sees q,k,v once and out once.
+// sample finds q,k,v in L2 and adds onto output lines that are still L2-resident.
 //
-// Two touches per output element, ordered (the L2 write path is the scarce resource: ~5 TB/s for plain stores, ~4 TB/s for
-// reduce-adds that hit L2, 2.4 TB/s when they miss -- tools/tma_red_bench.cu): the "producer" items of a sample (column
-// lines, first key block) STORE their tile, every other item of the sample ADDS onto it with a TMA reduce-add once the
-// per-sample counter cdone[b] says all producers have completed their stores.  Items are walked in the lagged order of
-// cca_items.cuh -- P(0) | P(1) C(0) | P(2) C(1) ... -- so a consumer practically never waits; only items with a LOWER index
-// are ever waited for and each persistent CTA walks its items in increasing order, so the wait cannot cycle.  Store / add
-// boxes are exactly one tile long (tensor maps with box = tile length), so a store never touches a neighbouring tile.
-// L2 eviction hints keep what the consumers will touch again (producer loads and stores: evict_last) and let the rest
-// stream (consumer loads: evict_first).  With one tile per line every output element is one store plus one add: the result
-// is bit-reproducible; with key-block tiling a pixel gets 2*nt-1 adds whose order is not fixed (last-bit differences).
+// Two touches per output element, ordered: the "producer" items of a sample (column lines, first key block) STORE their
+// rows, every other item of the sample ADDS onto them (vector reductions at L2) once the per-sample counter cdone[b] says all
+// producers have completed their stores.  Items are walked in the lagged order of cca_items.cuh -- P(0) | P(1) C(0) | ... --
+// so a consumer practically never waits; only items with a LOWER index are ever waited for and each persistent CTA walks its
+// items in increasing order, so the wait cannot cycle.  With one tile per line every output element is one store plus one
+// add: the result is bit-reproducible; with key-block tiling a pixel gets 2*nt-1 adds whose order is not fixed.
 //
-// Roles (warpgroups, registers rebalanced with setmaxnreg), software-pipelined across items:
-//   TMA producer (1 thread)   : 4-D tiled loads [LK px][32 ch] fp32 / [LK px][64 ch] bf16, SWIZZLE_128B, OOB pixels
-//                               zero-filled; ring of 5 (6) slots: Q, K of the NEXT item are slipped in after the first V
-//                               chunks of the current one.
-//   converter warps (256 thr) : fp32 only: fp32 -> bf16 hi + lo (x = hi + lo to ~2^-17), in place, as UMMA canonical
-//                               no-swizzle operand planes [8-channel chunk][pixel][16 B].
-//   MMA warp (elect.sync)     : S = Q K^T (SS; 3 bf16 MMAs per k-step for fp32 I/O), then per 64-channel V chunk
-//                               O = P V with A = P read from TMEM (TS), fp32 accumulation in TMEM.
-//   softmax group (128 thr)   : one pass over the S row in TMEM (lane = query pixel): P = exp2(S log2e - lse2) -> TMEM as
-//                               packed bf16 (hi/lo); also writes the final lse (row items, first key block).
-//   epilogue group (128 thr)  : per chunk TMEM -> swizzled staging tile (no scaling left to do).
-//   store warp (1 lane)       : TMA store / reduce-add of the staged tiles, per-sample counters.
+// Roles (cca_tc_common.cuh):
+//   producer lane       : Q, K of an item into their own stage; the item's 64-channel V chunks into a ring.  4-D tiled loads,
+//                         SWIZZLE_128B, pixels past the line zero-filled.
+//   consumer warpgroups : fp32 only: tiles -> bf16 hi + lo planes in place (x = hi + lo to ~2^-17).  S = Q K^T (wgmma, both
+//                         operands in shared memory), P = exp2(S log2e - lse2) in registers, re-packed as the bf16 A operand of
+//                         O = P V (wgmma with A from registers, 3 MMAs per k-step for fp32 I/O), O rows stored / added
+//                         straight from the accumulators.
+#include <type_traits>
+
 #include "cca_items.cuh"
 #include "cca_tc_common.cuh"
 
@@ -42,450 +35,220 @@ namespace cca {
 namespace {
 using namespace tc;
 
-constexpr int kTmemCols = 512;      // S [0,128)   P double buffer (hi/lo) [128,256) [256,384)   O ring 2 x 64 [384,512)
-constexpr int kTmemP = 128, kTmemO = 384, kNOB = 2;
-constexpr int kRegsSoft = 104, kRegsEpi = 128, kRegsConvF = 48;
-static_assert(reg_pool_ok(kRegsSoft, kRegsEpi, kRegsConvF), "setmaxnreg pool");
-constexpr int kNOutMax = 4;         // staging slots: 2 (fp32: shared memory is full) or 4 (bf16: 14 KB each; the store path -- one TMA
-                                    // instruction per chunk, ~500 cycles until the tile has left shared memory -- needs the slack)
-
 struct FwdParams {
     ItemSpace sp;
     int C, Cq;
     long npix;
     const float *parts;    // [nparts][B*H*W] partial log2-sum-exp2 (statistics pre-pass)
     float *lse;            // [B,H,W] natural-log lse (saved for backward)
+    void *out;             // [B,H,W,C] fp32 or bf16
     unsigned int *cdone;   // [B] producer items of sample b whose stores have completed (cleared by the statistics kernel)
     int lag;               // item order: 1 = consumers trail the producers by one block, 0 = sample after sample
-    int hints;             // L2 eviction hints on the bulk copies
-    long long *dbg;        // optional timeline buffer (CTA 0), -DCCA_TIMELINE builds only
+    int hints;             // L2 eviction hints on the loads
 };
-
-#ifdef CCA_TIMELINE
-#define CCA_STAMP(role)                                                                          \
-    do {                                                                                         \
-        if (p.dbg && blockIdx.x == 0 && dbg_n < 512) p.dbg[(role) * 512 + dbg_n++] = clock64();  \
-    } while (0)
-#else
-#define CCA_STAMP(role) do { } while (0)
-#endif
 
 template <int LK, bool BF> struct FwdSmem {
     using T = Tiles<LK, BF>;
-    static constexpr int kNLd = BF ? 8 : 6;
-    static constexpr int kNOut = BF ? 4 : 2;
-    static constexpr int off_ld = 0;                          // kNLd load slots; every slot is the UMMA operand itself: a bf16 tile as
-                                                              // loaded, an fp32 tile once the converters have rewritten it in place
-    static constexpr int off_out = off_ld + kNLd * T::kSlot;  // kNOut staging slots
-    // (An M=128 MMA reads (128 - LK) rows past the end of its Q slot: they land in the next slot / the staging slots and
-    // only feed S rows >= LK, which are discarded.)
-    static constexpr int off_bar = off_out + kNOut * T::kSlot + 1024;
-    static constexpr int kBytes = off_bar + 8 * 48 + 32;
+    static constexpr int off_qk = 0;                               // Q slot, K slot
+    static constexpr int off_ld = off_qk + 2 * T::kSlot;           // ring of V chunks
+    static constexpr int kNLd = (200 * 1024 - off_ld) / T::kSlot < 8 ? (200 * 1024 - off_ld) / T::kSlot : 8;
+    static constexpr int off_tail = off_ld + kNLd * T::kSlot;      // 64-row wgmmas of the second warpgroup read up to
+                                                                   // (128 - LK) rows past a tile; they only feed discarded rows
+    static constexpr int off_bar = off_tail + (128 - LK) * 128 + 1024;
+    static constexpr int kBytes = off_bar + 8 * (2 + 2 * kNLd);
+    static_assert(kNLd >= 2, "ring depth");
     static_assert(kBytes <= 232448, "shared memory budget");
 };
-
-enum { B_LD_FULL = 0, B_LD_EMPTY = 8, B_OP_FULL = 16, B_S_FULL = 24, B_S_EMPTY = 25, B_P_FULL = 26,
-       B_P_EMPTY = 28, B_O_FULL = 30, B_O_EMPTY = 32, B_OUT_FREE = 34, B_STAGED = 38, B_COUNT = 46 };   // B_OUT_FREE: [slot], B_STAGED: [store warp][slot]
 
 template <int LK, bool BF>
 __global__ void __launch_bounds__(kThreads, 1)
 cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant__ CUtensorMap mqr,
                   const __grid_constant__ CUtensorMap mkc, const __grid_constant__ CUtensorMap mkr,
-                  const __grid_constant__ CUtensorMap mvc, const __grid_constant__ CUtensorMap mvr,
-                  const __grid_constant__ CUtensorMap moc, const __grid_constant__ CUtensorMap mor, FwdParams p)
+                  const __grid_constant__ CUtensorMap mvc, const __grid_constant__ CUtensorMap mvr, FwdParams p)
 {
     using T = Tiles<LK, BF>;
     using S = FwdSmem<LK, BF>;
+    using E = typename std::conditional<BF, __nv_bfloat16, float>::type;
     constexpr int kNLd = S::kNLd;
-    constexpr int kNOut = S::kNOut;
+    constexpr int TERMS = BF ? 1 : 3;
+    constexpr int KP = LK / 16;               // k-steps of O = P V
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + S::off_bar);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + S::off_bar + 8 * B_COUNT);
+    uint64_t *qk_full = bars, *qk_empty = bars + 1, *full = bars + 2, *empty = bars + 2 + kNLd;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int NCH = p.C / kNC;
-    const int KQ = p.Cq / 16;                 // k-steps of the S MMA
+    const int KQ = p.Cq / 16;
     const int nk = p.sp.total > (int)blockIdx.x ? (p.sp.total - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
     auto item_of = [&](int k) { return decode_item_order(p.sp, (int)blockIdx.x + k * (int)gridDim.x, p.lag); };
-    // ring order:  Q0 K0 | V0[0..qkpos) Q1 K1 V0[qkpos..NCH) | V1[0..qkpos) Q2 K2 ...   (Q,K of the next item are slipped in
-    // after the first chunks of the current one, so neither S(k+1) nor the first P V chunk of an item waits for the other)
-    const int qkpos = NCH >= 3 ? 2 : NCH - 1;
 
     if (tid == 0) {
-        for (int i = 0; i < kNLd; ++i) {
-            mbar_init(&bars[B_LD_FULL + i], 1); mbar_init(&bars[B_LD_EMPTY + i], 1); mbar_init(&bars[B_OP_FULL + i], kConvThreads);
-        }
-        for (int i = 0; i < kNOB; ++i) { mbar_init(&bars[B_O_FULL + i], 1); mbar_init(&bars[B_O_EMPTY + i], 128); }
-        for (int i = 0; i < kNOut; ++i) { mbar_init(&bars[B_OUT_FREE + i], 1); mbar_init(&bars[B_STAGED + i], 128); mbar_init(&bars[B_STAGED + kNOut + i], 128); }
-        mbar_init(&bars[B_S_FULL], 1); mbar_init(&bars[B_S_EMPTY], 128);
-        for (int i = 0; i < 2; ++i) { mbar_init(&bars[B_P_FULL + i], 128); mbar_init(&bars[B_P_EMPTY + i], 1); }
+        mbar_init(qk_full, 1); mbar_init(qk_empty, kConsumers);
+        for (int i = 0; i < kNLd; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kConsumers); }
         fence_mbar_init();
-        prefetch_tmap(&mqc); prefetch_tmap(&mqr); prefetch_tmap(&mkc); prefetch_tmap(&mkr);
-        prefetch_tmap(&mvc); prefetch_tmap(&mvr); prefetch_tmap(&moc); prefetch_tmap(&mor);
+        prefetch_tmap(&mqc); prefetch_tmap(&mqr); prefetch_tmap(&mkc); prefetch_tmap(&mkr); prefetch_tmap(&mvc); prefetch_tmap(&mvr);
     }
-    if (warp == 0) tmem_alloc<kTmemCols>(tmem_slot);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
-    if (warp >= kWarpProducer) {
-        reg_dec<kRegsMisc>();
-        if (warp == kWarpProducer) {
-            // =============================== TMA producer ===============================
-            if (lane == 0) {
-                uint32_t g = 0;
-                int dbg_n = 0;
-                (void)dbg_n;
-                const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
-                auto emit = [&](const CUtensorMap *mc, const CUtensorMap *mr, int c0, const Item &it, int start) {
-                    const CUtensorMap *m = it.col ? mc : mr;
-                    const int cw = it.col ? it.line : start, ch = it.col ? start : it.line;
-                    const int slot = g % kNLd;
-                    mbar_wait(&bars[B_LD_EMPTY + slot], ((g / kNLd) & 1) ^ 1);
-                    CCA_STAMP(0);
-                    uint8_t *dst = smem + S::off_ld + slot * T::kSlot;
-                    mbar_expect_tx(&bars[B_LD_FULL + slot], T::kSlot);
-                    if (p.hints == 1) {     // producers' operands are read again by the sample's consumers; theirs are not
-                        // (hints == 2: no hints on the loads, only the output tiles are kept -- a reduce-add that misses L2 costs a
-                        //  DRAM read-modify-write at 2.4 TB/s, an operand re-read that misses is a plain read)
-                        const uint64_t pol = is_producer(it) ? pol_keep : pol_stream;
-                        tma_load_4d(dst, m, &bars[B_LD_FULL + slot], c0, cw, ch, it.b, pol);
-                        if constexpr (!BF) tma_load_4d(dst + T::kTile, m, &bars[B_LD_FULL + slot], c0 + 32, cw, ch, it.b, pol);
-                    } else {
-                        tma_load_4d(dst, m, &bars[B_LD_FULL + slot], c0, cw, ch, it.b);
-                        if constexpr (!BF) tma_load_4d(dst + T::kTile, m, &bars[B_LD_FULL + slot], c0 + 32, cw, ch, it.b);
-                    }
-                    ++g;
-                };
-                if (nk > 0) {
-                    const Item it0 = item_of(0);
-                    emit(&mqc, &mqr, 0, it0, it0.q0);
-                    emit(&mkc, &mkr, 0, it0, it0.k0);
+    if (warp == 0) {
+        // =============================== TMA producer ===============================
+        if (lane == 0) {
+            const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
+            auto load = [&](uint8_t *dst, uint64_t *bar, const CUtensorMap *m, int c0, const Item &it, int start) {
+                const int cw = it.col ? it.line : start, ch = it.col ? start : it.line;
+                if (p.hints == 1) {     // producers' operands are read again by the sample's consumers; theirs are not
+                    const uint64_t pol = is_producer(it) ? pol_keep : pol_stream;
+                    tma_load_4d(dst, m, bar, c0, cw, ch, it.b, pol);
+                    if constexpr (!BF) tma_load_4d(dst + T::kTile, m, bar, c0 + 32, cw, ch, it.b, pol);
+                } else {
+                    tma_load_4d(dst, m, bar, c0, cw, ch, it.b);
+                    if constexpr (!BF) tma_load_4d(dst + T::kTile, m, bar, c0 + 32, cw, ch, it.b);
                 }
-                for (int k = 0; k < nk; ++k) {
-                    const Item it = item_of(k);
-                    for (int n = 0; n < NCH; ++n) {
-                        if (n == qkpos && k + 1 < nk) {
-                            const Item nx = item_of(k + 1);
-                            emit(&mqc, &mqr, 0, nx, nx.q0);
-                            emit(&mkc, &mkr, 0, nx, nx.k0);
-                        }
-                        emit(&mvc, &mvr, n * kNC, it, it.k0);
-                    }
-                }
-            }
-        } else if (warp == kWarpMma) {
-            // =============================== MMA issuer (whole warp, elect.sync inside) ===============================
-            const uint32_t idesc_s = instr_desc(kFmtBF16, kFmtBF16, 128, LK, false, false);
-            const uint32_t idesc_o = instr_desc(kFmtBF16, kFmtBF16, 128, kNC, false, true);
-            uint32_t u = 0, oc = 0;
-            int dbg_n = lane == 0 ? 0 : 512;
-            (void)dbg_n;
-            const uint32_t ld_base = smem_u32(smem + S::off_ld);
-            auto wait_item = [&](uint32_t g) { mbar_wait(&bars[(BF ? B_LD_FULL : B_OP_FULL) + g % kNLd], (g / kNLd) & 1); };
-            auto free_item = [&](uint32_t g) { commit_to(&bars[B_LD_EMPTY + g % kNLd]); };
-            auto item_addr = [&](uint32_t g) { return ld_base + (g % kNLd) * T::kSlot; };
-            auto issue_s = [&](int k) {            // S(k) = Q K^T from ring items u (Q) and u+1 (K)
-                const uint32_t qb = item_addr(u), kb = item_addr(u + 1);
-                wait_item(u); wait_item(u + 1);
-                mbar_wait(&bars[B_S_EMPTY], (k & 1) ^ 1);
-                tc_fence_after();
-                CCA_STAMP(2);
-                for (int ks = 0; ks < KQ; ++ks) {
-                    if constexpr (BF) {
-                        mma_split3<1>(tmem, smem_desc(qb + ks * 32, 16, 1024, kSw128), 0, smem_desc(kb + ks * 32, 16, 1024, kSw128), 0,
-                                      idesc_s, ks > 0);
-                    } else {
-                        const uint32_t ao = ks * 2 * T::kPStride;
-                        mma_split3<3>(tmem, smem_desc(qb + ao, T::kPStride, 128), smem_desc(qb + T::kLoOff + ao, T::kPStride, 128),
-                                      smem_desc(kb + ao, T::kPStride, 128), smem_desc(kb + T::kLoOff + ao, T::kPStride, 128),
-                                      idesc_s, ks > 0);
-                    }
-                }
-                commit_to(&bars[B_S_FULL]);
-                free_item(u); free_item(u + 1);
-                u += 2;
             };
-            if (nk > 0) issue_s(0);
+            uint32_t g = 0;
             for (int k = 0; k < nk; ++k) {
-                CCA_STAMP(2);
-                mbar_wait(&bars[B_P_FULL + (k & 1)], (k >> 1) & 1);
-                tc_fence_after();
-                CCA_STAMP(2);
-                const uint32_t pbuf = tmem + kTmemP + (k & 1) * 128;
-                for (int n = 0; n < NCH; ++n, ++u, ++oc) {
-                    if (n == qkpos && k + 1 < nk) issue_s(k + 1);
-                    const uint32_t vb = item_addr(u);
-                    const uint32_t ob = oc % kNOB;
-                    wait_item(u);
-                    mbar_wait(&bars[B_O_EMPTY + ob], ((oc / kNOB) & 1) ^ 1);
-                    tc_fence_after();
-                    CCA_STAMP(2);
-                    if (elect_one()) {
-                        const uint32_t d = tmem + kTmemO + ob * kNC;
-#pragma unroll
-                        for (int ks = 0; ks < LK / 16; ++ks) {
-                            const uint32_t ph = pbuf + ks * 8, pl = ph + LK / 2;
-                            if constexpr (BF) {
-                                mma_f16_ts(d, ph, smem_desc(vb + ks * 2048, 16, 1024, kSw128), idesc_o, ks > 0);
-                            } else {
-                                const uint64_t vh = smem_desc(vb + ks * 256, 128, T::kPStride);
-                                const uint64_t vl = smem_desc(vb + T::kLoOff + ks * 256, 128, T::kPStride);
-                                mma_f16_ts(d, ph, vh, idesc_o, ks > 0);
-                                mma_f16_ts(d, ph, vl, idesc_o, true);
-                                mma_f16_ts(d, pl, vh, idesc_o, true);
-                            }
-                        }
-                    }
-                    __syncwarp();
-                    commit_to(&bars[B_O_FULL + ob]);
-                    free_item(u);
-                    CCA_STAMP(2);
+                const Item it = item_of(k);
+                mbar_wait(qk_empty, (k & 1) ^ 1);
+                mbar_expect_tx(qk_full, 2 * T::kSlot);
+                load(smem + S::off_qk, qk_full, it.col ? &mqc : &mqr, 0, it, it.q0);
+                load(smem + S::off_qk + T::kSlot, qk_full, it.col ? &mkc : &mkr, 0, it, it.k0);
+                for (int n = 0; n < NCH; ++n, ++g) {
+                    const int slot = g % kNLd;
+                    mbar_wait(&empty[slot], ((g / kNLd) & 1) ^ 1);
+                    mbar_expect_tx(&full[slot], T::kSlot);
+                    load(smem + S::off_ld + slot * T::kSlot, &full[slot], it.col ? &mvc : &mvr, n * kNC, it, it.k0);
                 }
-                commit_to(&bars[B_P_EMPTY + (k & 1)]);
-            }
-        } else if (warp >= kWarpStore) {
-            // =============================== store warps (one lane each) ===============================
-            // Two warps alternate items: while one waits for the global completion of its producer item's stores (to publish
-            // them), the other already issues the next item's tiles.
-            if (lane == 0) {
-                pdl_wait();                                // statistics kernel complete: the counters are cleared
-                const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
-                const bool one_tile = p.sp.col.nt == 1 && p.sp.row.nt == 1;
-                // each store warp has its own STAGED barriers (a parity wait must never fall a whole phase pair behind, which
-                // it would if it shared the barrier with the chunks of the other warp's items)
-                const int sel = warp - kWarpStore;
-                uint32_t use[kNOutMax] = {0, 0, 0, 0};
-                for (int k = sel; k < nk; k += 2) {
-                    const Item it = item_of(k);
-                    const bool prod = is_producer(it);
-                    const CUtensorMap *mo = it.col ? &moc : &mor;          // box = one tile of this direction, exactly
-                    const int cw = it.col ? it.line : it.q0, ch = it.col ? it.q0 : it.line;
-                    for (int n = 0; n < NCH; ++n) {
-                        const uint32_t c = (uint32_t)k * NCH + n;
-                        const int os = c % kNOut;
-                        mbar_wait(&bars[B_STAGED + sel * kNOut + os], use[os] & 1);
-                        ++use[os];
-                        if (n == 0 && !prod) {             // every producer of this sample has stored its tile
-                            wait_count(p.cdone + it.b, (unsigned)p.sp.seg0);
-                            fence_proxy_async_all();
-                        }
-                        const uint8_t *slot = smem + S::off_out + os * T::kSlot;
-                        if (prod) {
-                            if (p.hints) {
-                                tma_store_4d(mo, slot, n * kNC, cw, ch, it.b, pol_keep);
-                                if constexpr (!BF) tma_store_4d(mo, slot + T::kTile, n * kNC + 32, cw, ch, it.b, pol_keep);
-                            } else {
-                                tma_store_4d(mo, slot, n * kNC, cw, ch, it.b);
-                                if constexpr (!BF) tma_store_4d(mo, slot + T::kTile, n * kNC + 32, cw, ch, it.b);
-                            }
-                        } else if (p.hints && one_tile) {  // the one and only add onto these lines: they are final
-                            tma_reduce_add_4d(mo, slot, n * kNC, cw, ch, it.b, pol_stream);
-                            if constexpr (!BF) tma_reduce_add_4d(mo, slot + T::kTile, n * kNC + 32, cw, ch, it.b, pol_stream);
-                        } else {
-                            tma_reduce_add_4d(mo, slot, n * kNC, cw, ch, it.b);
-                            if constexpr (!BF) tma_reduce_add_4d(mo, slot + T::kTile, n * kNC + 32, cw, ch, it.b);
-                        }
-                        tma_store_commit();
-                        tma_store_wait_read<0>();          // the tile has been read out of shared memory: hand the slot back
-                        mbar_arrive(&bars[B_OUT_FREE + os]);
-                    }
-                    if (prod) {                            // publish once the stores have completed (the other store warp carries on)
-                        tma_store_wait_all<0>();
-                        publish_count(p.cdone + it.b);
-                    }
-                }
-                tma_store_wait_all<0>();
             }
         }
-    } else if (warp >= kWarpConv0) {
-        // =============================== converters (256 threads) ===============================
-        reg_dec<kRegsConvF>();
-        const int t = tid - kWarpConv0 * 32;
-        int dbg_n = t == 0 ? 0 : 512;
-        (void)dbg_n;
+    } else if (tid >= 128) {
+        // =============================== consumers (warpgroup wg = query rows [64 wg, 64 wg + 64)) ===============================
+        const int t = tid - 128, wg = t >> 7, wq = (t >> 5) & 3;
+        const int rbase = 64 * wg + 16 * wq + (lane >> 2);         // rows rbase, rbase + 8 of the accumulators
+        const uint32_t qb = smem_u32(smem + S::off_qk), kb = qb + T::kSlot, ld_base = smem_u32(smem + S::off_ld);
+        E *const out = reinterpret_cast<E *>(p.out);
+        pdl_wait();                                                // parts and the counters come from the statistics kernel
         uint32_t g = 0;
-        int pend = -1;                                             // slot converted but not yet fenced / published
-        auto publish = [&]() {
-            if (pend >= 0) {
-                fence_proxy_async();
-                mbar_arrive(&bars[B_OP_FULL + pend]);
-                pend = -1;
-            }
-        };
-        auto convert_next = [&](int count) {                       // the next `count` ring slots, whatever they hold
-            for (int e = 0; e < count; ++e, ++g) {
-                const int slot = g % kNLd;
-                // the previous slot is published after this slot's loads are in flight -- unless this slot has not landed yet
-                if (!mbar_try_wait(&bars[B_LD_FULL + slot], (g / kNLd) & 1)) {
-                    publish();
-                    mbar_wait(&bars[B_LD_FULL + slot], (g / kNLd) & 1);
-                }
-                CCA_STAMP(1);
-                convert_slot_inplace<LK>(smem + S::off_ld + slot * T::kSlot, t, publish);
-                pend = slot;
-                CCA_STAMP(1);
-            }
-        };
-        if constexpr (!BF) {                                       // bf16 tiles need no conversion
-            if (nk > 0) convert_next(2);                           // Q, K of the first item
-            for (int k = 0; k < nk; ++k)                           // mirrors the ring order of the producer
-                for (int n = 0; n < NCH; ++n) {
-                    if (n == qkpos && k + 1 < nk) convert_next(2);
-                    convert_next(1);
-                }
-            publish();
-        }
-    } else if (warp >= 4) {
-        // =============================== softmax group (128 threads, TMEM lane == query pixel) ===============================
-        reg_inc<kRegsSoft>();
-        const int r = tid - 128;
-        const uint32_t tl = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-        int dbg_n = r == 0 ? 0 : 512;
-        (void)dbg_n;
-        pdl_wait();                                                // parts come from the statistics kernel
         for (int k = 0; k < nk; ++k) {
             const Item it = item_of(k);
-            const bool rvalid = r < it.lq;
-            // final log2-sum-exp2 of this query pixel from the per-(direction, key block) planes
-            float lse2 = 0.f;
-            if (rvalid) {
-                const long pix = item_pixel(p.sp, it, r);
-                float m = -INFINITY;
-                for (int i = 0; i < p.sp.nparts; ++i) m = fmaxf(m, __ldcg(p.parts + (long)i * p.npix + pix));
-                float s = 0.f;
-                for (int i = 0; i < p.sp.nparts; ++i) s += exp2f(__ldcg(p.parts + (long)i * p.npix + pix) - m);
-                lse2 = m + log2f(s);
-                if (!it.col && it.ik == 0) p.lse[pix] = lse2 * kLn2;
+            const bool prod = is_producer(it);
+            // ---- S = Q K^T
+            mbar_wait(qk_full, k & 1);
+            if constexpr (!BF) {
+                convert_slot<LK, BF>(smem + S::off_qk, t);
+                convert_slot<LK, BF>(smem + S::off_qk + T::kSlot, t);
             }
-            const int self = it.col ? it.q0 + r - it.k0 : -1;          // masked key of this query (column branch only)
-            // The masks cost more ALU issue slots than the exponentials (ISETP/FSEL run at half rate): a 16-key chunk takes
-            // the predicated path only if it holds the tail of the key block or the self entry of one of this warp's 32
-            // query pixels -- a warp-uniform test; rows beyond the query tile get P = exp2(-inf) = 0 through their lse.
-            const int sw0 = it.col ? it.q0 - it.k0 + 32 * (warp & 3) : -(1 << 20);
-            const float nlse = rvalid ? -lse2 : -INFINITY;
-            CCA_STAMP(3);
-            mbar_wait(&bars[B_S_FULL], k & 1);
-            mbar_wait(&bars[B_P_EMPTY + (k & 1)], ((k >> 1) & 1) ^ 1);    // P V of item k-2 has finished reading this buffer
-            tc_fence_after();
-            CCA_STAMP(3);
-            // P = exp2(s log2e - lse2) -> TMEM as packed bf16 pairs (hi at [pdst, +LK/2), lo at [pdst+LK/2, +LK/2))
-            const uint32_t pdst = tl + kTmemP + (k & 1) * 128;
-#pragma unroll 1
-            for (int c0 = 0; c0 < LK; c0 += 16) {
-                float s[16];
-                tmem_ld16(tl + c0, reinterpret_cast<uint32_t *>(s));
-                tmem_ld_wait();
-                uint32_t hi[8], lo[8];
-                const bool masked = (c0 + 16 > it.lk) || (c0 + 16 > sw0 && c0 < sw0 + 32);
-                if (!masked) {
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        const float p0 = exp2f(fmaf(s[2 * e], kLog2e, nlse));
-                        const float p1 = exp2f(fmaf(s[2 * e + 1], kLog2e, nlse));
-                        if constexpr (BF) hi[e] = pack_bf16(p0, p1);
-                        else split2(p0, p1, hi[e], lo[e]);
-                    }
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        const int j = c0 + 2 * e;
-                        const bool ok0 = j < it.lk && j != self;
-                        const bool ok1 = j + 1 < it.lk && j + 1 != self;
-                        const float p0 = ok0 ? exp2f(fmaf(s[2 * e], kLog2e, nlse)) : 0.f;
-                        const float p1 = ok1 ? exp2f(fmaf(s[2 * e + 1], kLog2e, nlse)) : 0.f;
-                        if constexpr (BF) hi[e] = pack_bf16(p0, p1);
-                        else split2(p0, p1, hi[e], lo[e]);
-                    }
+            float acc[LK / 2];
+            wg_fence();
+            for (int ks = 0; ks < KQ; ++ks) {
+                wgmma_ss<LK>(acc, desc_kmaj<LK, BF>(qb, 64 * wg, ks, false), desc_kmaj<LK, BF>(kb, 0, ks, false), ks > 0, 0, 0);
+                if constexpr (TERMS == 3) {
+                    wgmma_ss<LK>(acc, desc_kmaj<LK, BF>(qb, 64 * wg, ks, false), desc_kmaj<LK, BF>(kb, 0, ks, true), 1, 0, 0);
+                    wgmma_ss<LK>(acc, desc_kmaj<LK, BF>(qb, 64 * wg, ks, true), desc_kmaj<LK, BF>(kb, 0, ks, false), 1, 0, 0);
                 }
-                tmem_st8(pdst + c0 / 2, hi);
-                if constexpr (!BF) tmem_st8(pdst + LK / 2 + c0 / 2, lo);
             }
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(&bars[B_P_FULL + (k & 1)]);
-            mbar_arrive(&bars[B_S_EMPTY]);
-            CCA_STAMP(3);
-        }
-    } else {
-        // =============================== epilogue group (128 threads, TMEM lane == query pixel) ===============================
-        reg_inc<kRegsEpi>();
-        const int r = tid;
-        const uint32_t tl = tmem + ((uint32_t)(warp * 32) << 16);
-        uint32_t oc = 0;
-        int dbg_n = tid == 0 ? 0 : 512;
-        (void)dbg_n;
-        for (int k = 0; k < nk; ++k) {
-            for (int n = 0; n < NCH; ++n, ++oc) {
-                const int os = oc % kNOut;
-                const uint32_t ob = oc % kNOB;
-                uint8_t *slot = smem + S::off_out + os * T::kSlot;
-                CCA_STAMP(4);
-                mbar_wait(&bars[B_OUT_FREE + os], ((oc / kNOut) & 1) ^ 1);   // the store of chunk oc - kNOut has left the slot
-                mbar_wait(&bars[B_O_FULL + ob], (oc / kNOB) & 1);
-                tc_fence_after();
-                CCA_STAMP(4);
-                float o[kNC];
+            wg_commit();
+            wg_wait<0>();
+            wg_acc_fence<LK / 2>(acc);
+            mbar_arrive(qk_empty);
+            // ---- P = exp2(S log2e - lse2) for rows rbase (h = 0), rbase + 8 (h = 1), as bf16 A fragments (hi, lo)
+            long pix[2];
+            float nlse[2];
+            int self[2];
+            bool rok[2];
 #pragma unroll
-                for (int c0 = 0; c0 < kNC; c0 += 16) tmem_ld16(tl + kTmemO + ob * kNC + c0, reinterpret_cast<uint32_t *>(o + c0));
-                tmem_ld_wait();
-                tc_fence_before();
-                mbar_arrive(&bars[B_O_EMPTY + ob]);
-                // rows >= lq are exact zeros (their P row is zero): inside the image they add nothing, outside the TMA clips them
-                if (r < LK) {
-                    uint8_t *row = slot + r * 128;
-                    const int sw = r & 7;
+            for (int h = 0; h < 2; ++h) {
+                const int r = rbase + 8 * h;
+                rok[h] = r < it.lq;
+                pix[h] = item_pixel(p.sp, it, rok[h] ? r : 0);
+                self[h] = it.col ? it.q0 + r - it.k0 : -1;
+                float lse2 = 0.f;
+                if (rok[h]) {
+                    float m = -INFINITY;
+                    for (int i = 0; i < p.sp.nparts; ++i) m = fmaxf(m, __ldcg(p.parts + (long)i * p.npix + pix[h]));
+                    float sum = 0.f;
+                    for (int i = 0; i < p.sp.nparts; ++i) sum += exp2f(__ldcg(p.parts + (long)i * p.npix + pix[h]) - m);
+                    lse2 = m + log2f(sum);
+                    if (!it.col && it.ik == 0 && (lane & 3) == 0) p.lse[pix[h]] = lse2 * kLn2;
+                }
+                nlse[h] = -lse2;
+            }
+            uint32_t ph[KP][4], pl[KP][4];
+#pragma unroll
+            for (int j = 0; j < LK / 8; ++j)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int c = 8 * j + 2 * (lane & 3);
+                    const bool ok0 = rok[h] && c < it.lk && c != self[h];
+                    const bool ok1 = rok[h] && c + 1 < it.lk && c + 1 != self[h];
+                    const float p0 = ok0 ? exp2f(fmaf(acc[4 * j + 2 * h], kLog2e, nlse[h])) : 0.f;
+                    const float p1 = ok1 ? exp2f(fmaf(acc[4 * j + 2 * h + 1], kLog2e, nlse[h])) : 0.f;
+                    // A fragment of k-step j/2: {row r, cols 0-7}, {row r+8, cols 0-7}, {row r, cols 8-15}, {row r+8, cols 8-15}
+                    const int reg = (j & 1) * 2 + h;
                     if constexpr (BF) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j)
-                            *reinterpret_cast<uint4 *>(row + ((j ^ sw) * 16)) =
-                                make_uint4(pack_bf16(o[8 * j], o[8 * j + 1]), pack_bf16(o[8 * j + 2], o[8 * j + 3]),
-                                           pack_bf16(o[8 * j + 4], o[8 * j + 5]), pack_bf16(o[8 * j + 6], o[8 * j + 7]));
+                        ph[j / 2][reg] = pack_bf16(p0, p1);
+                        pl[j / 2][reg] = 0u;
                     } else {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j)
-                            *reinterpret_cast<float4 *>(row + (j >> 3) * T::kTile + (((j & 7) ^ sw) * 16)) =
-                                make_float4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
+                        split2(p0, p1, ph[j / 2][reg], pl[j / 2][reg]);
                     }
                 }
-                fence_proxy_async();
-                mbar_arrive(&bars[B_STAGED + (k & 1) * kNOut + os]);     // the store warp of this item takes over
-                CCA_STAMP(4);
+            if (!prod) wait_count(p.cdone + it.b, (unsigned)p.sp.seg0);   // every producer of this sample has stored its rows
+            // ---- O = P V, 64 channels at a time
+            for (int n = 0; n < NCH; ++n, ++g) {
+                const int slot = g % kNLd;
+                mbar_wait(&full[slot], (g / kNLd) & 1);
+                if constexpr (!BF) convert_slot<LK, BF>(smem + S::off_ld + slot * T::kSlot, t);
+                const uint32_t vb = ld_base + slot * T::kSlot;
+                float o[32];
+                wg_fence();
+#pragma unroll
+                for (int ks = 0; ks < KP; ++ks) {
+                    wgmma_rs_n64_tb(o, ph[ks], desc_mnmaj<LK, BF>(vb, ks, false), ks > 0);
+                    if constexpr (TERMS == 3) {
+                        wgmma_rs_n64_tb(o, ph[ks], desc_mnmaj<LK, BF>(vb, ks, true), 1);
+                        wgmma_rs_n64_tb(o, pl[ks], desc_mnmaj<LK, BF>(vb, ks, false), 1);
+                    }
+                }
+                wg_commit();
+                wg_wait<0>();
+                wg_acc_fence<32>(o);
+                mbar_arrive(&empty[slot]);
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    if (rok[h]) {
+                        E *row = out + pix[h] * p.C + n * kNC + 2 * (lane & 3);
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) put2(row + 8 * j, o[4 * j + 2 * h], o[4 * j + 2 * h + 1], !prod);
+                    }
+            }
+            if (prod) {                                            // publish: all stores of this item are visible
+                __threadfence();
+                consumers_sync();
+                if (t == 0) atomicAdd(p.cdone + it.b, 1u);
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc<kTmemCols>(tmem);
 }
-
-long long *g_dbg = nullptr;   // timeline buffer (tools/tc_timeline.py, -DCCA_TIMELINE builds)
 
 template <int LK, bool BF>
 cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, float *lse, const float *parts, unsigned int *cdone,
                        Dims d, cudaStream_t st, const char **why)
 {
-    CUtensorMap m[8];
-    const void *base[4] = {q, k, v, out};
-    const int ch[4] = {d.Cq, d.Cq, d.C, d.C};
+    CUtensorMap m[6];
+    const void *base[3] = {q, k, v};
+    const int ch[3] = {d.Cq, d.Cq, d.C};
     FwdParams p;
     p.sp = make_space(d.B, d.H, d.W);
-    for (int t = 0; t < 4; ++t)
-        for (int r = 0; r < 2; ++r) {
-            // loads: LK-pixel boxes (pixels past the image are zero-filled = the padding the MMAs need);
-            // output: boxes of exactly one tile of the direction, so a store never reaches into the next tile
-            const int rows = t < 3 ? LK : (r == 0 ? p.sp.col.tl : p.sp.row.tl);
-            if (!get_map(&m[2 * t + r], base[t], d.B, d.H, d.W, ch[t], rows, r == 0, BF)) {
+    for (int t = 0; t < 3; ++t)
+        for (int r = 0; r < 2; ++r)
+            // LK-pixel boxes: pixels past the line are zero-filled
+            if (!get_map(&m[2 * t + r], base[t], d.B, d.H, d.W, ch[t], LK, r == 0, BF)) {
                 if (why) *why = "cuTensorMapEncodeTiled failed";
                 return cudaErrorInvalidValue;
             }
-        }
     p.C = d.C; p.Cq = d.Cq;
     p.npix = (long)d.B * d.H * d.W;
-    p.parts = parts; p.lse = lse; p.cdone = cdone;
+    p.parts = parts; p.lse = lse; p.cdone = cdone; p.out = out;
     p.lag = tc_lag() != 0 ? 1 : 0;                 // default (-1): lagged
     p.hints = tc_l2_hints();
-    p.dbg = g_dbg;
     auto kern = cca_tc_fwd_kernel<LK, BF>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem<LK, BF>::kBytes);
     if (e != cudaSuccess) return e;
@@ -498,14 +261,12 @@ cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, f
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = tc_pdl() ? 1 : 0;     // may start ahead of the statistics kernel's completion (griddepcontrol.wait inside)
-    e = cudaLaunchKernelEx(&cfg, kern, m[0], m[1], m[2], m[3], m[4], m[5], m[6], m[7], p);
+    e = cudaLaunchKernelEx(&cfg, kern, m[0], m[1], m[2], m[3], m[4], m[5], p);
     count_launch();
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 
 }  // namespace
-
-void set_tc_debug_buffer(void *p) { g_dbg = reinterpret_cast<long long *>(p); }
 
 bool tc_forward_supported(Dims d, int dtype) { return tc::shape_supported(d, dtype); }
 

@@ -1,4 +1,4 @@
-// Host-side helpers of the tcgen05 kernels: tensor-map cache, per-device SM count.
+// Host-side helpers of the wgmma kernels: tensor-map cache, per-device SM count.
 #include <mutex>
 #include <unordered_map>
 
@@ -55,7 +55,7 @@ int sm_count()
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
     std::lock_guard<std::mutex> lk(g_sm_mu);
     if (!g_sm_count[dev]) cudaDeviceGetAttribute(&g_sm_count[dev], cudaDevAttrMultiProcessorCount, dev);
-    return g_sm_count[dev] > 0 ? g_sm_count[dev] : 148;
+    return g_sm_count[dev] > 0 ? g_sm_count[dev] : 132;
 }
 
 }  // namespace tc

@@ -1,4 +1,4 @@
-// tcgen05 / TMA statistics pre-pass of criss-cross attention for sm_100a (channels-last q, k).
+// wgmma / TMA statistics pre-pass of criss-cross attention for sm_90a (channels-last q, k).
 //
 // The joint softmax of cc_attention/functions.py:40 couples a pixel's column line and its row line.  This kernel reads
 // only q and k (1/9 of the forward's bytes at C = 8 Cq) and leaves, per pixel and per (direction, key block), the
@@ -9,25 +9,18 @@
 // other, which is what lets ONE launch process column and row lines in an L2-friendly per-sample order and what lifts
 // the line-length limit (key-block tiling without an online-softmax chain).
 //
-// Persistent grid (<= 1 CTA per SM), static round-robin over the items of cca_items.cuh.  Roles:
-//   warp 16 (1 lane)   TMA producer: Q tile, K tile per item, [LK px][64 ch] boxes, ring of 6 slots
-//   warps 8-15         fp32 only: fp32 -> bf16 hi/lo operand planes, in place (256 threads, both 32-channel boxes of a slot)
-//   warp 25            MMA issuer: S = Q K^T (bf16x3 split for fp32 I/O), four S buffers in TMEM
-//   warps 0-7, 16-23   FOUR statistics groups (TMEM lane == query pixel), one S buffer each, items k = g, g+4, ...: the row
-//                      statistics (112 exp2 per thread and item, dependent on tensor-memory loads) are what paces this kernel,
-//                      the conversion of two 28 KB slots per item is not
-//   warps 18-19        clear the per-sample counters of the values kernel (and, if asked, a byte range)
+// Persistent grid (<= 1 CTA per SM), static round-robin over the items of cca_items.cuh.  Roles (cca_tc_common.cuh):
+//   producer lane      : Q tile and K tile of an item ([LK px][64 ch] boxes) into a ring of kNS stages
+//   consumer warpgroups: fp32 only: convert both tiles in place to bf16 hi/lo planes; S = Q K^T with wgmma (bf16x3 split for
+//                        fp32 I/O, accumulators in registers, warpgroup w = query rows [64w, 64w+64)); then each row's
+//                        max and sum over the four threads that hold it.  They also clear the per-sample counters of the
+//                        values kernel (and, if asked, a byte range).
 #include "cca_items.cuh"
 #include "cca_tc_common.cuh"
 
 namespace cca {
 namespace {
 using namespace tc;
-
-constexpr int kNS = 6;            // load slots
-constexpr int kStatConvThreads = 256;   // converter threads of this kernel (warps 8-15)
-constexpr int kStatGroups = 4;          // statistics groups: warps 0-3, 4-7, 16-19, 20-23
-constexpr int kNSB = 4;           // S buffers in TMEM (4 x 128 columns)
 
 struct StatsParams {
     ItemSpace sp;
@@ -38,28 +31,19 @@ struct StatsParams {
     long zero_bytes;
     unsigned int *counters;       // n_counters words cleared
     int n_counters;
-    long long *dbg;               // timeline buffer (CTA 0), -DCCA_TIMELINE builds only
 };
-
-#ifdef CCA_TIMELINE
-#define CCA_STAMP(role)                                                                          \
-    do {                                                                                         \
-        if (p.dbg && blockIdx.x == 0 && dbg_n < 512) p.dbg[(role) * 512 + dbg_n++] = clock64();  \
-    } while (0)
-#else
-#define CCA_STAMP(role) do { } while (0)
-#endif
 
 template <int LK, bool BF> struct StatsSmem {
     using T = Tiles<LK, BF>;
+    static constexpr int kNS = (200 * 1024) / (2 * T::kSlot) < 4 ? (200 * 1024) / (2 * T::kSlot) : 4;   // Q+K stages
     static constexpr int off_ld = 0;
-    static constexpr int off_tail = off_ld + kNS * T::kSlot;       // M=128 MMAs read (128 - LK) rows past the last slot
+    static constexpr int off_tail = off_ld + kNS * 2 * T::kSlot;   // 64-row wgmmas of the second warpgroup read (128 - LK) rows
+                                                                    // past the last tile; they only feed discarded S rows
     static constexpr int off_bar = off_tail + (128 - LK) * 128 + 1024;
-    static constexpr int kBytes = off_bar + 8 * 32 + 16;
+    static constexpr int kBytes = off_bar + 8 * 2 * kNS;
+    static_assert(kNS >= 2, "ring depth");
     static_assert(kBytes <= 232448, "shared memory budget");
 };
-
-enum { SB_LD_FULL = 0, SB_LD_EMPTY = 6, SB_OP_FULL = 12, SB_S_FULL = 18, SB_S_EMPTY = 22, SB_COUNT = 26 };
 
 template <int LK, bool BF>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -68,218 +52,109 @@ cca_tc_stats_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_consta
 {
     using T = Tiles<LK, BF>;
     using S = StatsSmem<LK, BF>;
+    constexpr int kNS = S::kNS;
     constexpr int TERMS = BF ? 1 : 3;
     extern __shared__ __align__(1024) uint8_t smem[];
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + S::off_bar);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + S::off_bar + 8 * SB_COUNT);
+    uint64_t *full = reinterpret_cast<uint64_t *>(smem + S::off_bar), *empty = full + kNS;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int KQ = p.Cq / 16;
     const int nk = p.sp.total > (int)blockIdx.x ? (p.sp.total - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
     auto item_of = [&](int k) { return decode_item(p.sp, (int)blockIdx.x + k * (int)gridDim.x); };
 
     if (tid == 0) {
-        for (int i = 0; i < kNS; ++i) {
-            mbar_init(&bars[SB_LD_FULL + i], 1); mbar_init(&bars[SB_LD_EMPTY + i], 1); mbar_init(&bars[SB_OP_FULL + i], kStatConvThreads);
-        }
-        for (int i = 0; i < kNSB; ++i) { mbar_init(&bars[SB_S_FULL + i], 1); mbar_init(&bars[SB_S_EMPTY + i], 128); }
+        for (int i = 0; i < kNS; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kConsumers); }
         fence_mbar_init();
         prefetch_tmap(&mqc); prefetch_tmap(&mqr); prefetch_tmap(&mkc); prefetch_tmap(&mkr);
     }
-    if (warp == 0) tmem_alloc<512>(tmem_slot);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
     pdl_launch_dependents();          // the values kernel may start its prologue / operand loads; it waits (griddepcontrol.wait)
                                       // before it reads parts, the counters or adds onto the output
 
-    if (warp == kWarpProducer) {
+    if (warp == 0) {
         if (lane == 0) {
-            uint32_t g = 0;
-            int dbg_n = 0;
-            (void)dbg_n;
             for (int k = 0; k < nk; ++k) {
                 const Item it = item_of(k);
-                for (int t = 0; t < 2; ++t, ++g) {
+                const int slot = k % kNS;
+                mbar_wait(&empty[slot], ((k / kNS) & 1) ^ 1);
+                uint8_t *dst = smem + S::off_ld + slot * 2 * T::kSlot;
+                mbar_expect_tx(&full[slot], 2 * T::kSlot);
+                for (int t = 0; t < 2; ++t) {
                     const CUtensorMap *m = t == 0 ? (it.col ? &mqc : &mqr) : (it.col ? &mkc : &mkr);
                     const int start = t == 0 ? it.q0 : it.k0;
                     const int cw = it.col ? it.line : start, ch = it.col ? start : it.line;
-                    const int slot = g % kNS;
-                    mbar_wait(&bars[SB_LD_EMPTY + slot], ((g / kNS) & 1) ^ 1);
-                    CCA_STAMP(0);
-                    uint8_t *dst = smem + S::off_ld + slot * T::kSlot;
-                    mbar_expect_tx(&bars[SB_LD_FULL + slot], T::kSlot);
-                    tma_load_4d(dst, m, &bars[SB_LD_FULL + slot], 0, cw, ch, it.b);
-                    if constexpr (!BF) tma_load_4d(dst + T::kTile, m, &bars[SB_LD_FULL + slot], 32, cw, ch, it.b);
+                    tma_load_4d(dst + t * T::kSlot, m, &full[slot], 0, cw, ch, it.b);
+                    if constexpr (!BF) tma_load_4d(dst + t * T::kSlot + T::kTile, m, &full[slot], 32, cw, ch, it.b);
                 }
             }
         }
-    } else if (warp == kWarpMma) {
-        const uint32_t idesc_s = instr_desc(kFmtBF16, kFmtBF16, 128, LK, false, false);
+    } else if (tid >= 128) {
+        const int t = tid - 128, wg = t >> 7, wq = (t >> 5) & 3;
+        // ---- clear the head of the forward's output and the values kernel's counters
+        {
+            const long n16 = p.zero_bytes / 16;
+            const long per = (n16 + gridDim.x - 1) / gridDim.x;
+            const long lo = per * blockIdx.x, hi = lo + per < n16 ? lo + per : n16;
+            uint4 *dst = reinterpret_cast<uint4 *>(p.zero_ptr);
+            for (long i = lo + t; i < hi; i += kConsumers) dst[i] = make_uint4(0, 0, 0, 0);
+            if (blockIdx.x == 0)
+                for (int i = t; i < p.n_counters; i += kConsumers) p.counters[i] = 0u;
+        }
         const uint32_t ld_base = smem_u32(smem + S::off_ld);
-        uint32_t g = 0;
-        int dbg_n = lane == 0 ? 0 : 512;
-        (void)dbg_n;
-        for (int k = 0; k < nk; ++k, g += 2) {
-            const uint32_t qb = ld_base + (g % kNS) * T::kSlot, kb = ld_base + ((g + 1) % kNS) * T::kSlot;
-            mbar_wait(&bars[(BF ? SB_LD_FULL : SB_OP_FULL) + g % kNS], (g / kNS) & 1);
-            mbar_wait(&bars[(BF ? SB_LD_FULL : SB_OP_FULL) + (g + 1) % kNS], ((g + 1) / kNS) & 1);
-            CCA_STAMP(2);
-            mbar_wait(&bars[SB_S_EMPTY + (k % kNSB)], ((k / kNSB) & 1) ^ 1);
-            tc_fence_after();
-            CCA_STAMP(2);
-            const uint32_t d = tmem + (k % kNSB) * 128;
-            for (int ks = 0; ks < KQ; ++ks) {
-                if constexpr (BF) {
-                    mma_split3<1>(d, smem_desc(qb + ks * 32, 16, 1024, kSw128), 0, smem_desc(kb + ks * 32, 16, 1024, kSw128), 0,
-                                  idesc_s, ks > 0);
-                } else {
-                    const uint32_t ao = ks * 2 * T::kPStride;
-                    mma_split3<3>(d, smem_desc(qb + ao, T::kPStride, 128), smem_desc(qb + T::kLoOff + ao, T::kPStride, 128),
-                                  smem_desc(kb + ao, T::kPStride, 128), smem_desc(kb + T::kLoOff + ao, T::kPStride, 128),
-                                  idesc_s, ks > 0);
-                }
-            }
-            commit_to(&bars[SB_S_FULL + (k % kNSB)]);
-            commit_to(&bars[SB_LD_EMPTY + g % kNS]);
-            commit_to(&bars[SB_LD_EMPTY + (g + 1) % kNS]);
-        }
-        (void)TERMS;
-    } else if (warp >= kWarpStore) {
-        // ---- clear the head of the forward's output and the values kernel's counters (64 threads per CTA)
-        const int t = tid - kWarpStore * 32;
-        const long n16 = p.zero_bytes / 16;
-        const long per = (n16 + gridDim.x - 1) / gridDim.x;
-        const long lo = per * blockIdx.x, hi = lo + per < n16 ? lo + per : n16;
-        uint4 *dst = reinterpret_cast<uint4 *>(p.zero_ptr);
-        for (long i = lo + t; i < hi; i += 64) dst[i] = make_uint4(0, 0, 0, 0);
-        if (blockIdx.x == 0)
-            for (int i = t; i < p.n_counters; i += 64) p.counters[i] = 0u;
-    } else if (warp >= kWarpConv0 && warp < kWarpConv0 + kStatConvThreads / 32) {
-        const int t = tid - kWarpConv0 * 32;
-        int dbg_n = t == 0 ? 0 : 512;
-        (void)dbg_n;
-        if constexpr (!BF) {
-            int pend = -1;                       // slot converted but not yet fenced / published
-            auto publish = [&]() {
-                if (pend >= 0) {
-                    fence_proxy_async();
-                    mbar_arrive(&bars[SB_OP_FULL + pend]);
-                    pend = -1;
-                }
-            };
-            for (uint32_t g = 0; g < (uint32_t)(2 * nk); ++g) {
-                const int slot = g % kNS;
-                if (!mbar_try_wait(&bars[SB_LD_FULL + slot], (g / kNS) & 1)) {
-                    publish();
-                    mbar_wait(&bars[SB_LD_FULL + slot], (g / kNS) & 1);
-                }
-                CCA_STAMP(1);
-                // both 32-channel boxes of the slot by the same 256 threads (thread = pixel row x 16-channel half): read 2 x 64 B,
-                // meet, overwrite in place as hi/lo planes (layout of convert_slot_inplace)
-                {
-                    using TT = Tiles<LK, false>;
-                    uint8_t *sl = smem + S::off_ld + slot * T::kSlot;
-                    const int r = t & 127, hq = t >> 7;
-                    const int rr = r < LK ? r : LK - 1, sw = rr & 7;
-                    float4 raw[8];
-#pragma unroll
-                    for (int bx = 0; bx < 2; ++bx)
-#pragma unroll
-                        for (int j = 0; j < 4; ++j)
-                            raw[4 * bx + j] = *reinterpret_cast<const float4 *>(sl + bx * TT::kTile + rr * 128 + (((hq * 4 + j) ^ sw) * 16));
-                    publish();
-                    asm volatile("bar.sync 1, 256;" ::: "memory");
-                    if (r < LK) {
-#pragma unroll
-                        for (int bx = 0; bx < 2; ++bx) {
-                            uint8_t *d = sl + bx * TT::kTile + r * 16 + hq * 2 * TT::kPStride;
-#pragma unroll
-                            for (int j = 0; j < 2; ++j) {
-                                const float4 a = raw[4 * bx + 2 * j], b = raw[4 * bx + 2 * j + 1];
-                                const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-                                uint4 hi, lo;
-                                split8(v, hi, lo);
-                                *reinterpret_cast<uint4 *>(d + j * TT::kPStride) = hi;
-                                *reinterpret_cast<uint4 *>(d + j * TT::kPStride + TT::kLoOff) = lo;
-                            }
-                        }
-                    }
-                }
-                pend = slot;
-                CCA_STAMP(1);
-            }
-            publish();
-        }
-        (void)t;
-    } else if (warp < 8 || (warp >= 16 && warp < 24)) {
-        // =============================== statistics groups (4 x 128 threads, TMEM lane == query pixel) ===============================
-        const int grp = warp < 8 ? warp >> 2 : 2 + ((warp - 16) >> 2), r = tid & 127;
-        const uint32_t tl = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-        int dbg_n = tid == 0 ? 0 : 512;          // group 0 only (role 3)
-        (void)dbg_n;
-        for (int k = grp; k < nk; k += kStatGroups) {
+        for (int k = 0; k < nk; ++k) {
             const Item it = item_of(k);
-            CCA_STAMP(3);
-            mbar_wait(&bars[SB_S_FULL + (k % kNSB)], (k / kNSB) & 1);
-            tc_fence_after();
-            CCA_STAMP(3);
-            const uint32_t ts = tl + (k % kNSB) * 128;
-            const int self = it.col ? it.q0 + r - it.k0 : -1;      // masked key of this query (column branch only)
-            // predicated path only for the 16-key chunks that hold the tail of the key block or the self entry of one of this
-            // warp's 32 query pixels (warp-uniform test): the masks cost more ALU issue slots than the arithmetic
-            const int sw0 = it.col ? it.q0 - it.k0 + 32 * (warp & 3) : -(1 << 20);
-            // One pass over the S row, 16 columns at a time with the next 16 already in flight from tensor memory: running max m
-            // of the raw logits (log2e > 0: scaled on use) and l = sum 2^((s - m) log2e), rescaled when the max moves; two
-            // accumulators so that the additions do not form one dependent chain.  (Two passes with a wait after every
-            // tcgen05.ld -- max first, then the sum -- made these eight warps the pace of the whole kernel.)
-            float m = -INFINITY, l0 = 0.f, l1 = 0.f;
-            float nx[16];
-            tmem_ld16(ts, reinterpret_cast<uint32_t *>(nx));
-#pragma unroll 1
-            for (int c0 = 0; c0 < it.lk; c0 += 16) {
-                float s[16];
-                tmem_ld_wait16(reinterpret_cast<uint32_t *>(nx));
-#pragma unroll
-                for (int e = 0; e < 16; ++e) s[e] = nx[e];
-                if (c0 + 16 < it.lk) tmem_ld16(ts + c0 + 16, reinterpret_cast<uint32_t *>(nx));
-                const bool masked = (c0 + 16 > it.lk) || (c0 + 16 > sw0 && c0 < sw0 + 32);
-                if (masked) {
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) {
-                        const int j = c0 + e;
-                        s[e] = (j < it.lk && j != self) ? s[e] : -INFINITY;
-                    }
-                }
-                float cm = fmaxf(fmaxf(s[0], s[1]), fmaxf(s[2], s[3]));
-#pragma unroll
-                for (int e = 4; e < 16; e += 4) cm = fmaxf(cm, fmaxf(fmaxf(s[e], s[e + 1]), fmaxf(s[e + 2], s[e + 3])));
-                if (cm > m) {                                  // (never true for a fully masked chunk: cm = -inf)
-                    const float sc = exp2f((m - cm) * kLog2e);         // m = -inf: exp2(-inf) = 0 and l is still 0
-                    l0 *= sc; l1 *= sc;
-                    m = cm;
-                }
-                const float nm = (m == -INFINITY) ? 0.f : -m * kLog2e;
-#pragma unroll
-                for (int e = 0; e < 16; e += 2) {              // masked entries: exp2(-inf) = 0
-                    l0 += exp2f(fmaf(s[e], kLog2e, nm));
-                    l1 += exp2f(fmaf(s[e + 1], kLog2e, nm));
+            const int slot = k % kNS;
+            mbar_wait(&full[slot], (k / kNS) & 1);
+            uint8_t *qs = smem + S::off_ld + slot * 2 * T::kSlot;
+            if constexpr (!BF) {
+                convert_slot<LK, BF>(qs, t);
+                convert_slot<LK, BF>(qs + T::kSlot, t);
+            }
+            const uint32_t qb = ld_base + slot * 2 * T::kSlot, kb = qb + T::kSlot;
+            float acc[LK / 2];
+            wg_fence();
+            for (int ks = 0; ks < KQ; ++ks) {
+                wgmma_ss<LK>(acc, desc_kmaj<LK, BF>(qb, 64 * wg, ks, false), desc_kmaj<LK, BF>(kb, 0, ks, false), ks > 0, 0, 0);
+                if constexpr (TERMS == 3) {
+                    wgmma_ss<LK>(acc, desc_kmaj<LK, BF>(qb, 64 * wg, ks, false), desc_kmaj<LK, BF>(kb, 0, ks, true), 1, 0, 0);
+                    wgmma_ss<LK>(acc, desc_kmaj<LK, BF>(qb, 64 * wg, ks, true), desc_kmaj<LK, BF>(kb, 0, ks, false), 1, 0, 0);
                 }
             }
-            const float l = l0 + l1;
-            m *= kLog2e;
-            tc_fence_before();
-            mbar_arrive(&bars[SB_S_EMPTY + (k % kNSB)]);
-            CCA_STAMP(3);
-            if (r < it.lq) p.parts[(long)part_index(p.sp, it) * p.npix + item_pixel(p.sp, it, r)] = l > 0.f ? m + log2f(l) : -INFINITY;
+            wg_commit();
+            wg_wait<0>();
+            wg_acc_fence<LK / 2>(acc);
+            mbar_arrive(&empty[slot]);
+            // rows r (h = 0) and r + 8 (h = 1) of this thread, columns 8j + 2(lane % 4) + e
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = 64 * wg + 16 * wq + (lane >> 2) + 8 * h;
+                const int self = it.col ? it.q0 + r - it.k0 : -1;      // masked key of this query (column branch only)
+                float m = -INFINITY;
+#pragma unroll
+                for (int j = 0; j < LK / 8; ++j)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int c = 8 * j + 2 * (lane & 3) + e;
+                        if (c < it.lk && c != self) m = fmaxf(m, acc[4 * j + 2 * h + e]);
+                    }
+                m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+                m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+                const float nm = m == -INFINITY ? 0.f : -m * kLog2e;
+                float l = 0.f;
+#pragma unroll
+                for (int j = 0; j < LK / 8; ++j)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int c = 8 * j + 2 * (lane & 3) + e;
+                        if (c < it.lk && c != self) l += exp2f(fmaf(acc[4 * j + 2 * h + e], kLog2e, nm));
+                    }
+                l += __shfl_xor_sync(0xffffffffu, l, 1);
+                l += __shfl_xor_sync(0xffffffffu, l, 2);
+                if ((lane & 3) == 0 && r < it.lq)
+                    p.parts[(long)part_index(p.sp, it) * p.npix + item_pixel(p.sp, it, r)] = l > 0.f ? m * kLog2e + log2f(l) : -INFINITY;
+            }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc<512>(tmem);
 }
-
-long long *g_stats_dbg = nullptr;
 
 template <int LK, bool BF>
 cudaError_t launch_stats(const void *q, const void *k, float *parts, void *zero_ptr, long zero_bytes, unsigned int *counters,
@@ -300,7 +175,6 @@ cudaError_t launch_stats(const void *q, const void *k, float *parts, void *zero_
     p.parts = parts;
     p.zero_ptr = reinterpret_cast<uint8_t *>(zero_ptr); p.zero_bytes = zero_bytes;
     p.counters = counters; p.n_counters = n_counters;
-    p.dbg = g_stats_dbg;
     auto kern = cca_tc_stats_kernel<LK, BF>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, StatsSmem<LK, BF>::kBytes);
     if (e != cudaSuccess) return e;
@@ -312,8 +186,6 @@ cudaError_t launch_stats(const void *q, const void *k, float *parts, void *zero_
 }
 
 }  // namespace
-
-void set_tc_stats_debug_buffer(void *p) { g_stats_dbg = reinterpret_cast<long long *>(p); }
 
 // parts: [nparts][B*H*W] fp32.  Also clears zero_bytes bytes at zero_ptr and n_counters words at counters (both may be 0).
 cudaError_t tc_stats(const void *q, const void *k, float *parts, void *zero_ptr, long zero_bytes, unsigned int *counters,

@@ -16,7 +16,7 @@ _IMPL_FLAGS = {"auto": capi.CCA_FLAG_AUTO, "simt": capi.CCA_FLAG_FORCE_SIMT, "tc
 
 def _check_inputs(q, k, v):
     if not (q.is_cuda and k.is_cuda and v.is_cuda):
-        raise RuntimeError("ccnet_b200: criss-cross attention needs CUDA tensors on a B200 "
+        raise RuntimeError("ccnet_b200: criss-cross attention needs CUDA tensors on an H100 (sm_90) "
                            "(there is no CPU path in this package)")
     if q.dtype not in _DTYPES or k.dtype != q.dtype or v.dtype != q.dtype:
         raise RuntimeError(f"ccnet_b200: q,k,v must share dtype float32 or bfloat16, got "
@@ -42,7 +42,7 @@ def _stream_ptr(device) -> int:
 
 
 def tc_eligible(B: int, Cq: int, C: int, H: int, W: int, dtype: torch.dtype) -> bool:
-    """True if the tcgen05 (channels-last) kernels cover this problem, forward AND backward."""
+    """True if the wgmma (channels-last) kernels cover this problem, forward AND backward."""
     if dtype not in _DTYPES:
         return False
     lib = capi.load()
@@ -141,7 +141,7 @@ def cca_backward(dout, q, k, v, out, lse, impl: str = "auto", want_delta: bool =
 
 
 def qkv_gemm_eligible(x: torch.Tensor, Cq: int) -> bool:
-    """True if the hand-written tcgen05 projection GEMMs cover x [B,C,H,W] (fp32, C and Cq multiples of 64)."""
+    """True if the hand-written wgmma projection GEMMs cover x [B,C,H,W] (fp32, C and Cq multiples of 64)."""
     return (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4
             and capi.load().cca_b200_qkv_supported(x.shape[1], Cq) == 1)
 
@@ -153,7 +153,7 @@ def _as_matrix_ptr(t: torch.Tensor) -> int:
 
 
 def qkv_project(x, wq, bq, wk, bk, wv, bv):
-    """q, k, v = the three 1x1 convs of cc_attention/functions.py:29,32,35 applied to channels-last x, as ONE tcgen05 GEMM
+    """q, k, v = the three 1x1 convs of cc_attention/functions.py:29,32,35 applied to channels-last x, as ONE wgmma GEMM
     launch emitting channels-last q, k, v.  fp32, C % 64 == 0, Cq % 64 == 0 (``qkv_gemm_eligible``)."""
     lib = capi.load()
     B, C, H, W = x.shape
@@ -175,7 +175,7 @@ def qkv_project(x, wq, bq, wk, bk, wv, bv):
 
 
 def qkv_project_dgrad(dq, dk, dv, wq, wk, wv, scale=None):
-    """dx = s (dq Wq + dk Wk + dv Wv) (input gradient of the three projections), channels-last fp32, one tcgen05 GEMM launch.
+    """dx = s (dq Wq + dk Wk + dv Wv) (input gradient of the three projections), channels-last fp32, one wgmma GEMM launch.
     ``scale``: optional one-element CUDA tensor s (the residual's gamma), folded into the packed weights."""
     lib = capi.load()
     B, C, H, W = dv.shape
@@ -198,7 +198,7 @@ def qkv_wgrad_eligible(C: int, Cq: int) -> bool:
 
 
 def qkv_project_wgrad(x, dq, dk, dv, scale=None):
-    """(dWq, dbq, dWk, dbk, dWv, dbv) = s * (gradients of the three 1x1 convs' parameters), one split-K tcgen05 launch."""
+    """(dWq, dbq, dWk, dbk, dWv, dbv) = s * (gradients of the three 1x1 convs' parameters), one split-K wgmma launch."""
     lib = capi.load()
     B, C, H, W = x.shape
     Cq = dq.shape[1]

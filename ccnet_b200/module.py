@@ -19,8 +19,7 @@ class _QKVProject(torch.autograd.Function):
     """The three 1x1 convs of functions.py:29,32,35 on a channels-last tensor, as dense GEMMs on its [pixels, C] view
     (cuBLAS; same parameters and fp32 maths as ``conv(x)``).  The outputs are channels-last q, k, v -- exactly the layout
     the tensor-core kernels consume.  One autograd node instead of three so that the input gradient is accumulated inside
-    the GEMMs (beta = 1) rather than by two extra elementwise passes over [pixels, C].  On B200 the GEMM form is ~1.7x
-    faster than the cudnn fp32 1x1 conv (fwd+bwd of the three projections at B=8, C=512, 97x97: 3.9 ms vs 6.7 ms)."""
+    the GEMMs (beta = 1) rather than by two extra elementwise passes over [pixels, C]."""
 
     @staticmethod
     @torch.amp.custom_fwd(device_type="cuda")
@@ -53,7 +52,7 @@ class _QKVProject(torch.autograd.Function):
 
 class _FusedCCAStep(torch.autograd.Function):
     """y = gamma * cca(q(x), k(x), v(x)) + x  -- functions.py:29-49 as ONE autograd node on channels-last fp32 tensors:
-    projections and their input gradient on the hand-written tcgen05 GEMMs, the attention on the tcgen05 item kernels.
+    projections and their input gradient on the hand-written wgmma GEMMs, the attention on the wgmma item kernels.
 
     The backward exploits that the attention backward is linear in dout: it runs on dy itself and the factor gamma is applied
     to the three small weight matrices of the input-gradient GEMM (and to the weight gradients) instead of scaling the [B,C,H,W]
@@ -92,7 +91,7 @@ class _FusedCCAStep(torch.autograd.Function):
 
 
 class CrissCrossAttention(nn.Module):
-    """Criss-Cross Attention Module (B200-native operator behind the reference surface)."""
+    """Criss-Cross Attention Module (Hopper-native operator behind the reference surface)."""
 
     def __init__(self, in_dim: int, impl: str = "auto"):
         super().__init__()
@@ -106,12 +105,12 @@ class CrissCrossAttention(nn.Module):
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if not x.is_cuda:
-            raise RuntimeError("ccnet_b200.CrissCrossAttention runs on CUDA (B200) only; "
+            raise RuntimeError("ccnet_b200.CrissCrossAttention runs on CUDA (H100, sm_90) only; "
                                "the CPU restatement lives in oracle/ and is test-only")
         B, C, H, W = x.shape
         if (self.impl != "simt" and tc_eligible(B, C // 8, C, H, W, x.dtype) and qkv_gemm_eligible(x, C // 8)
                 and not torch.is_autocast_enabled()):
-            # everything on hand-written sm_100a kernels: projection GEMMs + attention + their backward, one autograd node
+            # everything on hand-written sm_90a kernels: projection GEMMs + attention + their backward, one autograd node
             x = x.contiguous(memory_format=torch.channels_last)
             return _FusedCCAStep.apply(x, self.query_conv.weight, self.query_conv.bias, self.key_conv.weight,
                                        self.key_conv.bias, self.value_conv.weight, self.value_conv.bias, self.gamma)

@@ -2,8 +2,7 @@
 
 `torch.nn.SyncBatchNorm` filters the gathered statistics of ranks with an empty batch through a boolean mask
 (`count_all[mask]`, torch/nn/modules/_functions.py), which copies the mask to the host in EVERY layer's forward.  With ~100
-normalisation layers in ResNet101+RCCA that serialises the CPU with the GPU a hundred times per step: measured 122 ms per step on
-two GPUs at per-GPU batch 4, against 67 ms for the same batch on one GPU (profiles/r02_train_step_vs_batch.jsonl).  The reference's
+normalisation layers in ResNet101+RCCA that serialises the CPU with the GPU a hundred times per step.  The reference's
 own `InPlaceABNSync` (networks/ccnet.py:16) has no such stall.  Every rank of this harness always holds a non-empty batch, so the
 mask is dropped; everything else is torch's SyncBatchNorm function: the same ATen kernels (batch_norm_stats, ..._gather_stats_with_counts,
 ..._elemt, ..._backward_reduce, ..._backward_elemt), one all-gather of [2C+1] in forward, one all-reduce of [2C] in backward."""

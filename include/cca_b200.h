@@ -1,5 +1,5 @@
 /*
- * cca_b200.h -- C ABI of the B200-native criss-cross attention operator.
+ * cca_b200.h -- C ABI of the Hopper-native (sm_90a) criss-cross attention operator.
  *
  * This is the drop-in boundary for CCNet's hot path.  The reference exposes the path
  * only as a Python nn.Module (cc_attention/functions.py:15-49; the mounted branch has
@@ -57,13 +57,13 @@ typedef enum cca_status {
     CCA_ERR_UNSUPPORTED = -2,  /* shape outside what the kernels cover (see limits)      */
     CCA_ERR_WORKSPACE = -3,    /* workspace too small                                    */
     CCA_ERR_CUDA = -4,         /* CUDA runtime error (message in cca_b200_last_error)    */
-    CCA_ERR_DEVICE = -5        /* current device is not sm_100                           */
+    CCA_ERR_DEVICE = -5        /* current device is not sm_90                            */
 } cca_status;
 
 /* flags (bit mask) */
 #define CCA_FLAG_AUTO 0u        /* pick the fastest kernel family that covers the shape  */
 #define CCA_FLAG_FORCE_SIMT 1u  /* generic CUDA-core kernels (any shape within limits)   */
-#define CCA_FLAG_FORCE_TC 2u    /* tcgen05 tensor-core kernels; error if not applicable  */
+#define CCA_FLAG_FORCE_TC 2u    /* wgmma tensor-core kernels; error if not applicable    */
 #define CCA_FLAG_NHWC 4u        /* tensors are channels-last: q,k [B,H,W,Cq]; v,out,dout,dq.. [B,H,W,C]
                                  * (torch.channels_last of the same logical NCHW shape).  This is the
                                  * layout of the tensor-core kernels: rows and columns of the image are
@@ -86,7 +86,7 @@ CCA_API int cca_b200_device_ok(void);
 /* Number of kernels this library has launched in this process so far (for audits). */
 CCA_API unsigned long long cca_b200_launch_count(void);
 
-/* 1 if the tensor-core (tcgen05) kernels cover this problem in NHWC layout on the current device, else 0.
+/* 1 if the tensor-core (wgmma) kernels cover this problem in NHWC layout on the current device, else 0.
  * which = CCA_WS_FORWARD or CCA_WS_BACKWARD (the two directions have separate predicates).
  * Covered: Cq in {16,32,48,64}, C % 64 == 0, H and W up to 896 (lines longer than 112 pixels are tiled). */
 CCA_API int cca_b200_tc_supported(int which, int B, int Cq, int C, int H, int W, int dtype);
@@ -126,7 +126,7 @@ CCA_API int cca_b200_backward(const void *dout, const void *q, const void *k, co
 
 /*
  * The three 1x1 projections in front of the step (replace functions.py:29,32,35 -- query_conv, key_conv, value_conv -- and
- * their input gradient) as hand-written tcgen05 GEMMs on the channels-last view: x, v, dx are [pixels, C], q, k, dq, dk are
+ * their input gradient) as hand-written wgmma GEMMs on the channels-last view: x, v, dx are [pixels, C], q, k, dq, dk are
  * [pixels, Cq] row-major fp32 (a channels-last [B,C,H,W] tensor IS that matrix with pixels = B*H*W); weights are the conv
  * weights [out, in] row-major ([out,in,1,1] contiguous).  fp32 accuracy via the bf16 hi/lo split (3 MMAs per product).
  *   qkv_project       : q = x Wq^T + bq,  k = x Wk^T + bk,  v = x Wv^T + bv

@@ -1,4 +1,4 @@
-"""GPU side of SURVEY.md 8(f) N4: sliding-window inference through the harness network with the B200 operator in its head
+"""GPU side of SURVEY.md 8(f) N4: sliding-window inference through the harness network with this repository's operator in its head
 against the SAME weights with the CPU oracle module in the head (logit difference on synthetic tiles), and a checkpoint round
 trip in the reference's on-disk format (utils/pyt_utils.py:47-85)."""
 import copy

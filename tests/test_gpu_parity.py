@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: ``pytest -m gpu``).  Every call goes through the C ABI
+"""GPU parity tests (H100: ``pytest -m gpu``).  Every call goes through the C ABI
 (ccnet_b200.functional -> ctypes -> libcca_b200.so); the oracle is only the checker.
 
 Tolerances (BASELINE.json north_star): fp32 max-abs <= 1e-3 on identical Q/K/V; bf16 <= 1e-2
@@ -80,7 +80,7 @@ TC_SHAPES = [
 
 @pytest.mark.parametrize("shape", TC_SHAPES)
 def test_forward_tensor_core_vs_oracle_and_simt(shape):
-    """tcgen05 path (channels-last, bf16x3 split) against the fp64 oracle and the generic kernels."""
+    """wgmma path (channels-last, bf16x3 split) against the fp64 oracle and the generic kernels."""
     from ccnet_b200 import cca_forward
     O = _oracle()
     dev = _dev()
@@ -107,7 +107,7 @@ def test_forward_tensor_core_vs_oracle_and_simt(shape):
                                    (1, 48, 192, 81, 112), (1, 16, 128, 1, 1), (2, 64, 512, 33, 47), (1, 64, 512, 97, 97),
                                    (1, 64, 512, 129, 129), (1, 64, 512, 193, 193), (1, 32, 128, 113, 200), (2, 16, 64, 230, 7)])
 def test_backward_tensor_core_vs_oracle(shape):
-    """tcgen05 backward (channels-last, bf16x3 split, P recomputed from lse) against the fp64 closed form."""
+    """wgmma backward (channels-last, bf16x3 split, P recomputed from lse) against the fp64 closed form."""
     from ccnet_b200 import cca_backward, cca_forward
     O = _oracle()
     dev = _dev()
@@ -131,7 +131,7 @@ def test_backward_tensor_core_vs_oracle(shape):
 @pytest.mark.parametrize("shape", [(2, 32, 256, 20, 97), (1, 64, 64, 112, 80), (3, 16, 64, 1, 5), (2, 64, 512, 33, 47), (2, 64, 512, 97, 97),
                                    (1, 64, 512, 129, 129), (1, 64, 512, 193, 193), (1, 32, 128, 113, 200)])
 def test_bf16_tensor_core_forward_backward_vs_oracle(shape):
-    """bf16 I/O on the tcgen05 kernels (single-term MMAs, bf16 staging / TMA reduce-add): against the fp64 oracle
+    """bf16 I/O on the wgmma kernels (single-term MMAs, bf16 stores / vector adds): against the fp64 oracle
     evaluated on the bf16-rounded inputs (SURVEY.md 8c), tolerance 1e-2 relative to max|ref| (north_star), forward and gradients."""
     from ccnet_b200 import cca_backward, cca_forward
     O = _oracle()
@@ -167,7 +167,7 @@ def test_launch_knobs_are_bit_identical(dtype):
     """Programmatic dependent launch (off / on), the item order (lagged or not), the L2 eviction hints and the backward's delta
     mode only change WHEN and WHERE bytes move, never the arithmetic: with one tile per line every output element is one
     store plus one add, so forward and backward must be bit-identical across knobs and repetitions.
-    Repeated at the BASELINE shape (all 148 CTAs busy) to give an ordering bug a chance to show."""
+    Repeated at the BASELINE shape (every SM busy) to give an ordering bug a chance to show."""
     import ctypes
     from ccnet_b200 import capi, cca_backward, cca_forward
     dev = _dev()
@@ -206,7 +206,7 @@ def test_launch_knobs_are_bit_identical(dtype):
 @pytest.mark.parametrize("dtype,tol", [("fp32", FP32_TOL), ("bf16", BF16_TOL)])
 def test_backward_full_batch_c2_vs_oracle(dtype, tol):
     """BASELINE config 2 (B=8, C=512, 97x97): forward AND backward of the persistent single-launch schedule (776 lines per
-    direction over 148 CTAs, zero-ahead and delta hand-off between CTAs) against the fp64 oracle on the first, a middle and
+    direction over one persistent CTA per SM, delta hand-off between CTAs) against the fp64 oracle on the first, a middle and
     the last sample."""
     from ccnet_b200 import cca_backward, cca_forward
     O = _oracle()
@@ -405,7 +405,7 @@ def _proj_params(C, seed):
 
 @pytest.mark.parametrize("shape", [(1, 512, 97, 97), (3, 512, 20, 31), (1, 512, 1, 5)])
 def test_qkv_projection_gemm_vs_fp64(shape):
-    """tcgen05 bf16x3 GEMM of the three 1x1 convs against fp64 matmul: fp32-level accuracy (north_star 1e-3, typical 1e-5)."""
+    """wgmma bf16x3 GEMM of the three 1x1 convs against fp64 matmul: fp32-level accuracy (north_star 1e-3, typical 1e-5)."""
     from ccnet_b200.functional import qkv_gemm_eligible, qkv_project, qkv_project_dgrad
     dev = _dev()
     B, C, H, W = shape

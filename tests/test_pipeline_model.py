@@ -1,4 +1,4 @@
-"""The mbarrier protocol of the channel-major forward kernel (tools/experiments/cca_tc_fwdt.cu, an experiment that was not adopted) on the CPU model of tools/pipeline_model.py:
+"""The mbarrier protocol of the channel-major forward kernel (a channel-major variant explored for an earlier tensor-core design and not adopted; its role structure is kept in the model) on the CPU model of tools/pipeline_model.py:
 no deadlock under random role interleavings, and every wait / arrive meets the barrier phase its parity formula assumes
 (the first GPU run of that kernel hung on exactly such a parity slip; the model reproduces it in milliseconds)."""
 import importlib.util

@@ -1,71 +1,53 @@
-"""Row (b) of the scope table, executed: the reference's networks/ccnet.py (imported UNCHANGED from /root/reference) picks
-up this repository's cc_attention package (networks/ccnet.py:13) and builds its RCCA head around the B200 operator
-(networks/ccnet.py:105).  Needs the reference mount, so it runs in the build container and is skipped on the GPU box."""
-import importlib
+"""Row (b) of the scope table: the reference's networks/ccnet.py imports ``CrissCrossAttention`` from the ``cc_attention``
+package (networks/ccnet.py:13) and builds its RCCA head around it (networks/ccnet.py:105).  What that network and the
+reference's own module expect of the operator -- state-dict keys and shapes -- was taken from the reference itself and stored
+in tests/golden/reference_state_maps.json (tests/golden/make_reference_maps.py); these tests hold this repository to it."""
+import json
 import os
-import sys
 
-import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
-
-pytestmark = pytest.mark.skipif(not os.path.exists(os.path.join(REF, "networks", "ccnet.py")), reason="reference mount absent")
+MAPS = os.path.join(ROOT, "tests", "golden", "reference_state_maps.json")
 
 
-@pytest.fixture()
-def ref_ccnet():
-    saved_path, saved_mods = list(sys.path), dict(sys.modules)
-    for name in list(sys.modules):
-        if name == "networks" or name.startswith("networks.") or name == "utils" or name.startswith("utils.") or name == "inplace_abn":
-            del sys.modules[name]
-    # this repository (cc_attention, ccnet_b200) first, then the inplace_abn stand-in, then the reference tree
-    sys.path[:0] = [ROOT, os.path.join(ROOT, "harness", "shims"), REF]
-    try:
-        yield importlib.import_module("networks.ccnet")
-    finally:
-        sys.path[:] = saved_path
-        for name in list(sys.modules):
-            if name not in saved_mods:
-                del sys.modules[name]
+def _maps():
+    with open(MAPS) as f:
+        return json.load(f)
 
 
-def test_reference_network_builds_on_the_b200_operator(ref_ccnet):
+def test_reference_network_builds_on_the_b200_operator():
     import cc_attention
     import ccnet_b200
-    assert ref_ccnet.__file__.startswith(REF)                           # the reference's own file, not a copy
-    assert ref_ccnet.CrissCrossAttention is ccnet_b200.CrissCrossAttention
+    assert cc_attention.CrissCrossAttention is ccnet_b200.CrissCrossAttention     # what networks/ccnet.py:13 imports
     assert cc_attention.__file__.startswith(ROOT)
-    with torch.device("meta"):
-        model = ref_ccnet.Seg_Model(num_classes=19, recurrence=2)      # networks/ccnet.py:199-205
-    assert type(model.head.cca) is ccnet_b200.CrissCrossAttention       # networks/ccnet.py:105
-    keys = {k for k in model.state_dict() if k.startswith("head.cca.")}
+    seg = _maps()["seg_model"]
+    keys = {k for k in seg if k.startswith("head.cca.")}
     assert keys == {"head.cca." + n for n in ("gamma", "query_conv.weight", "query_conv.bias", "key_conv.weight",
                                                "key_conv.bias", "value_conv.weight", "value_conv.bias")}
-    sd = model.state_dict()
-    assert tuple(sd["head.cca.query_conv.weight"].shape) == (64, 512, 1, 1)
-    assert tuple(sd["head.cca.value_conv.weight"].shape) == (512, 512, 1, 1)
-    assert model.recurrence == 2
-
-
-def test_released_checkpoint_keys_load_into_the_module(ref_ccnet):
-    """utils/pyt_utils.py:47-85 load_model(strict=False) path: a state dict with the reference's head.cca.* entries restores
-    the B200 module's parameters (SURVEY 8f N4: on-disk format adjacent to the path)."""
-    import ccnet_b200
+    assert tuple(seg["head.cca.query_conv.weight"]) == (64, 512, 1, 1)
+    assert tuple(seg["head.cca.value_conv.weight"]) == (512, 512, 1, 1)
+    assert _maps()["seg_model_recurrence"] == 2
     with torch.device("meta"):
-        model = ref_ccnet.Seg_Model(num_classes=19, recurrence=2)
-    sys.path.insert(0, REF)
-    ref_mod = importlib.machinery.SourceFileLoader("ref_functions", os.path.join(REF, "cc_attention", "functions.py")).load_module()
-    ref = ref_mod.CrissCrossAttention(512)
-    with torch.no_grad():
-        ref.gamma.fill_(0.37)
-    ckpt = {"head.cca." + k: v for k, v in ref.state_dict().items()}
+        head = ccnet_b200.CrissCrossAttention(512)
+    ours = {"head.cca." + k: list(v.shape) for k, v in head.state_dict().items()}
+    assert ours == {k: seg[k] for k in keys}
+
+
+def test_released_checkpoint_keys_load_into_the_module():
+    """A checkpoint with the reference module's head.cca.* entries (keys and shapes of the reference's CrissCrossAttention(512))
+    restores the module's parameters through the non-strict load the reference's utils/pyt_utils.py:47-85 load_model does."""
+    import ccnet_b200
+    ref_map = _maps()["criss_cross_attention_512"]
+    gen = torch.Generator().manual_seed(0)
+    ref_sd = {k: torch.randn(*shape, generator=gen) for k, shape in ref_map.items()}
+    ref_sd["gamma"].fill_(0.37)
+    ckpt = {"head.cca." + k: v for k, v in ref_sd.items()}
     head = ccnet_b200.CrissCrossAttention(512)
     wrapper = torch.nn.Module()
     wrapper.head = torch.nn.Module()
     wrapper.head.cca = head
-    out = ref_ccnet.load_model(wrapper, ckpt)                           # the reference's own loader
-    assert out is wrapper
-    for k, v in ref.state_dict().items():
+    missing, unexpected = wrapper.load_state_dict(ckpt, strict=False)
+    assert not missing and not unexpected
+    for k, v in ref_sd.items():
         assert torch.equal(head.state_dict()[k], v), k

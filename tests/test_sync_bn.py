@@ -1,5 +1,5 @@
 """harness/sync_bn.py on the CPU: the conversion keeps parameter / buffer names and values, evaluation mode and single-process
-training mode are plain batch norm (the all-rank statistics path needs CUDA + NCCL: tools/r2_gpu_syncbn.sh)."""
+training mode are plain batch norm (the all-rank statistics path needs CUDA + NCCL: tools/r2_gpu_syncbn.py under torch.distributed.run)."""
 import torch
 import torch.nn as nn
 

@@ -1,6 +1,6 @@
 """BASELINE config 5: resolution sweep H=W in {65,97,129,193}, C=512, R=2 -- op forward / backward time, % of the measured
 HBM roofline, and the CPU reference (oracle module port, B=1) beside it.  Writes one JSON line per size.
-All four sizes run on the tcgen05 kernels (channels-last); lines longer than 112 pixels are tiled (csrc/cca_items.cuh)."""
+All four sizes run on the wgmma kernels (channels-last); lines longer than 112 pixels are tiled (csrc/cca_items.cuh)."""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -34,7 +34,7 @@ for HW in (65, 97, 129, 193):
     tf = t_of(lambda: cca_forward(q, k, v))
     tb = t_of(lambda: cca_backward(do, q, k, v, out, lse))
     bf, bb = bench.alg_bytes(B, C, HW, HW, 4, True, False), bench.alg_bytes(B, C, HW, HW, 4, False, True)
-    rec = {"H": HW, "W": HW, "B": B, "C": C, "R": R, "kernels": "tcgen05 (channels-last)" if tc else "generic (NCHW)",
+    rec = {"H": HW, "W": HW, "B": B, "C": C, "R": R, "kernels": "wgmma (channels-last)" if tc else "generic (NCHW)",
            "fwd_ms": tf, "bwd_ms": tb, "fwd_frac_of_hbm_peak": bf / tf / 1e6 / peak, "bwd_frac_of_hbm_peak": bb / tb / 1e6 / peak,
            "op_fwd_bwd_pixels_per_s_R2": B * HW * HW / (R * (tf + tb) * 1e-3), "hbm_peak_gbs": peak, "peak_source": src}
     if cpu:
