@@ -48,19 +48,31 @@ struct BwdParams {
     void *dq, *dk, *dv;
 };
 
+// The V / dO / O ring holds chunks of ONE 128-byte TMA box each: 32 channels for fp32 (converted in place to hi/lo planes),
+// 64 for bf16.  Small slots buy depth: at LK = 112 fp32 the ring has 8 slots (2 2/3 chunks of V, dO, O), so chunk n + 1 lands
+// and is converted while chunk n's MMAs run and chunk n + 2 is on its way.
 template <int LK, bool BF> struct BwdSmem {
     using T = Tiles<LK, BF>;
+    static constexpr int kCh = BF ? kNC : kNC / 2;                  // channels per ring slot / per chunk
+    static constexpr int kRSlot = T::kTile;                         // ring slot bytes: [LK px][128 B]
     static constexpr int off_qk = 0;                                // Q slot, K slot (held for the whole item: dQ, dK read them)
     static constexpr int off_p = off_qk + 2 * T::kSlot;             // P / dS planes (hi block, lo block)
     // (pad: 64-row P^T operands read up to 16 planes; TMA destinations with SWIZZLE_128B must be 1024-byte aligned)
     static constexpr int off_ld = (off_p + T::kP + (16 - LK / 8) * T::kPlane + 1023) / 1024 * 1024;
-    static constexpr int kNLd = (224 * 1024 - 4096 - off_ld) / T::kSlot < 8 ? (224 * 1024 - 4096 - off_ld) / T::kSlot : 8;
-    static constexpr int off_tail = off_ld + kNLd * T::kSlot;       // over-read of the last slot by the second warpgroup
-    static constexpr int off_dsum = off_tail + (128 - LK) * 128 + 256;   // float [2][128]: delta halves per pixel row
-    static constexpr int off_bar = off_dsum + 1024;
+    static constexpr int kTail = (128 - LK) * 128 + 256;            // over-read of the last slot by the second warpgroup
+    static constexpr int kDsum = 1024;                              // float [2][128]: delta halves per pixel row
+    static constexpr int kBudget = 232448;                          // 227 KB: the opt-in maximum per block on sm_90
+    // every slot also needs its full / empty barriers (8 B each); qk_full, qk_empty take the rest
+    static constexpr int kNLd = (kBudget - off_ld - kTail - kDsum - 16) / (kRSlot + 16);
+    static constexpr int off_tail = off_ld + kNLd * kRSlot;
+    static constexpr int off_dsum = off_tail + kTail;
+    static constexpr int off_bar = off_dsum + kDsum;
     static constexpr int kBytes = off_bar + 8 * (2 + 2 * kNLd);
-    static_assert(kNLd >= 3, "ring depth: V, dO, O of one chunk");
-    static_assert(kBytes <= 232448, "shared memory budget");
+    // The chunk loop holds chunk n's V, dO (its MMAs are in flight) while it waits for chunk n + 1's V, dO, O: the ring must hold
+    // two full chunks, or the producer could not issue chunk n + 1 before chunk n is released and the pipeline would stall
+    // (or, below 5 slots, deadlock).
+    static_assert(kNLd >= 6, "ring depth: two chunks of V, dO, O");
+    static_assert(kBytes <= kBudget, "shared memory budget");
 };
 
 // does this item compute delta itself (its ring carries the O chunks)?
@@ -79,6 +91,7 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
     using E = typename std::conditional<BF, __nv_bfloat16, float>::type;
     constexpr int TERMS = BF ? 1 : 3;
     constexpr int kNLd = S::kNLd;
+    constexpr int kCh = S::kCh;
     constexpr int KP = LK / 16;
     constexpr uint32_t LOP = T::kPP * T::kPlane;   // P / dS planes: hi block -> lo block
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -86,7 +99,7 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
     uint64_t *qk_full = bars, *qk_empty = bars + 1, *full = bars + 2, *empty = bars + 2 + kNLd;
     float *dsum = reinterpret_cast<float *>(smem + S::off_dsum);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int NCH = p.C / kNC;
+    const int NCH = p.C / kCh;
     const int KQ = p.Cq / 16;
     const int nk = p.sp.total > (int)blockIdx.x ? (p.sp.total - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
     auto item_of = [&](int k) { return decode_item_order(p.sp, (int)blockIdx.x + k * (int)gridDim.x, p.lag); };
@@ -100,27 +113,27 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
     }
     __syncthreads();
 
-    if (warp == 0) {
+    if (tid < 128) {
         // =============================== TMA producer ===============================
-        if (lane == 0) {
+        setmaxnreg_dec<kProducerRegs>();
+        if (warp == 0 && lane == 0) {
             const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
-            auto load = [&](uint8_t *dst, uint64_t *bar, const CUtensorMap *m, int c0, const Item &it, int start, bool last_use) {
+            // boxes: 128-byte TMA boxes from channel c0 on (Q / K: the 64 channels of a fp32 slot are two boxes)
+            auto load = [&](uint8_t *dst, uint64_t *bar, const CUtensorMap *m, int c0, const Item &it, int start, bool last_use, int boxes) {
                 const int cw = it.col ? it.line : start, ch = it.col ? start : it.line;
                 if (p.hints == 1) {     // what the sample's consumers read again stays; O and the consumers' own operands stream
                     const uint64_t pol = (is_producer(it) && !last_use) ? pol_keep : pol_stream;
-                    tma_load_4d(dst, m, bar, c0, cw, ch, it.b, pol);
-                    if constexpr (!BF) tma_load_4d(dst + T::kTile, m, bar, c0 + 32, cw, ch, it.b, pol);
+                    for (int bx = 0; bx < boxes; ++bx) tma_load_4d(dst + bx * T::kTile, m, bar, c0 + 32 * bx, cw, ch, it.b, pol);
                 } else {
-                    tma_load_4d(dst, m, bar, c0, cw, ch, it.b);
-                    if constexpr (!BF) tma_load_4d(dst + T::kTile, m, bar, c0 + 32, cw, ch, it.b);
+                    for (int bx = 0; bx < boxes; ++bx) tma_load_4d(dst + bx * T::kTile, m, bar, c0 + 32 * bx, cw, ch, it.b);
                 }
             };
             uint32_t g = 0;
             auto ring = [&](const CUtensorMap *m, int c0, const Item &it, int start, bool last_use) {
                 const int slot = g % kNLd;
                 mbar_wait(&empty[slot], ((g / kNLd) & 1) ^ 1);
-                mbar_expect_tx(&full[slot], T::kSlot);
-                load(smem + S::off_ld + slot * T::kSlot, &full[slot], m, c0, it, start, last_use);
+                mbar_expect_tx(&full[slot], S::kRSlot);
+                load(smem + S::off_ld + slot * S::kRSlot, &full[slot], m, c0, it, start, last_use, 1);
                 ++g;
             };
             for (int k = 0; k < nk; ++k) {
@@ -128,17 +141,18 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 const bool calc = calc_delta(p, it);
                 mbar_wait(qk_empty, (k & 1) ^ 1);
                 mbar_expect_tx(qk_full, 2 * T::kSlot);
-                load(smem + S::off_qk, qk_full, it.col ? &mqc : &mqr, 0, it, it.q0, false);
-                load(smem + S::off_qk + T::kSlot, qk_full, it.col ? &mkc : &mkr, 0, it, it.k0, false);
+                load(smem + S::off_qk, qk_full, it.col ? &mqc : &mqr, 0, it, it.q0, false, BF ? 1 : 2);
+                load(smem + S::off_qk + T::kSlot, qk_full, it.col ? &mkc : &mkr, 0, it, it.k0, false, BF ? 1 : 2);
                 for (int n = 0; n < NCH; ++n) {
-                    ring(it.col ? &mvc : &mvr, n * kNC, it, it.k0, false);
-                    ring(it.col ? &mdoc : &mdor, n * kNC, it, it.q0, false);
-                    if (calc) ring(it.col ? &moc : &mor, n * kNC, it, it.q0, p.delta_mode == 1);   // (mode 1: nobody reads O again)
+                    ring(it.col ? &mvc : &mvr, n * kCh, it, it.k0, false);
+                    ring(it.col ? &mdoc : &mdor, n * kCh, it, it.q0, false);
+                    if (calc) ring(it.col ? &moc : &mor, n * kCh, it, it.q0, p.delta_mode == 1);   // (mode 1: nobody reads O again)
                 }
             }
         }
-    } else if (tid >= 128) {
+    } else {
         // =============================== consumers (warpgroup wg = rows [64 wg, 64 wg + 64) of each product) ===============================
+        setmaxnreg_inc<kConsumerRegs>();
         const int t = tid - 128, wg = t >> 7, wq = (t >> 5) & 3;
         const int rbase = 64 * wg + 16 * wq + (lane >> 2);         // accumulator rows rbase, rbase + 8
         const int cq = 2 * (lane & 3);                             // first accumulator column of this thread (+ 8j)
@@ -212,27 +226,37 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
             consumers_sync();
             if (!prod && p.out_mode == 1) wait_count(p.cdone + it.b, (unsigned)p.sp.seg0);   // producers of the sample have stored
             // ---------------- per chunk: dP += dO V^T, dV = P^T dO
+            // Pipelined over the chunks: issue chunk n's MMAs, convert chunk n + 1 (and accumulate its delta dot) while they run,
+            // wait, release chunk n's slots and write its dV.  One group in flight at a time: with a second one (wg_wait<1>
+            // and a second dV accumulator, so that the dV writes also overlap the MMAs) ptxas treats the groups chained
+            // through dP as one pipeline stage, sees the other dV accumulator read inside it and serialises every wgmma of
+            // the kernel (C7514); at LK = 112 fp32 the second accumulator also spills.
             float dp[LK / 2];
+            float o[kCh / 2];                                      // dV of the chunk
             float dacc = 0.f;
-            for (int n = 0; n < NCH; ++n) {
-                const uint32_t gv = g++, gd = g++, go = calc ? g++ : 0;
-                mbar_wait(&full[gv % kNLd], (gv / kNLd) & 1);
-                mbar_wait(&full[gd % kNLd], (gd / kNLd) & 1);
-                if (calc) mbar_wait(&full[go % kNLd], (go / kNLd) & 1);
-                uint8_t *vs = smem + S::off_ld + (gv % kNLd) * T::kSlot, *ds = smem + S::off_ld + (gd % kNLd) * T::kSlot;
-                if constexpr (!BF) convert_slot<LK, BF>(vs, t);
+            const uint32_t per = calc ? 3 : 2;                     // ring slots per chunk: V, dO (, O)
+            auto rslot = [&](uint32_t gi) { return gi % kNLd; };
+            auto convert_chunk = [&](int n) {
+                const uint32_t gv = g + per * n, gd = gv + 1, go = gv + 2;
+                mbar_wait(&full[rslot(gv)], (gv / kNLd) & 1);
+                mbar_wait(&full[rslot(gd)], (gd / kNLd) & 1);
+                if (calc) mbar_wait(&full[rslot(go)], (go / kNLd) & 1);
+                uint8_t *vs = smem + S::off_ld + rslot(gv) * S::kRSlot, *ds = smem + S::off_ld + rslot(gd) * S::kRSlot;
+                if constexpr (!BF) convert_slot<LK, BF, 1>(vs, t);
                 if (calc) {
-                    dacc += convert_slot<LK, BF>(ds, t, smem + S::off_ld + (go % kNLd) * T::kSlot);
+                    dacc += convert_slot<LK, BF, 1>(ds, t, smem + S::off_ld + rslot(go) * S::kRSlot);
                     if constexpr (BF) consumers_sync();            // (fp32: the conversion ends on a consumer barrier)
-                    mbar_arrive(&empty[go % kNLd]);
+                    mbar_arrive(&empty[rslot(go)]);
                 } else if constexpr (!BF) {
-                    convert_slot<LK, BF>(ds, t);
+                    convert_slot<LK, BF, 1>(ds, t);
                 }
-                const uint32_t vb = ld_base + (gv % kNLd) * T::kSlot, db = ld_base + (gd % kNLd) * T::kSlot;
-                float o[32];
+            };
+            auto issue = [&](int n) {
+                const uint32_t gv = g + per * n, gd = gv + 1;
+                const uint32_t vb = ld_base + rslot(gv) * S::kRSlot, db = ld_base + rslot(gd) * S::kRSlot;
                 wg_fence();
 #pragma unroll
-                for (int ks = 0; ks < kNC / 16; ++ks) {
+                for (int ks = 0; ks < kCh / 16; ++ks) {
                     wgmma_ss<LK>(dp, desc_kmaj<LK, BF>(db, 64 * wg, ks, false), desc_kmaj<LK, BF>(vb, 0, ks, false), n > 0 || ks > 0, 0, 0);
                     if constexpr (TERMS == 3) {
                         wgmma_ss<LK>(dp, desc_kmaj<LK, BF>(db, 64 * wg, ks, false), desc_kmaj<LK, BF>(vb, 0, ks, true), 1, 0, 0);
@@ -242,26 +266,38 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
 #pragma unroll
                 for (int ks = 0; ks < KP; ++ks) {
                     const uint32_t pa = pb + 8 * wg * T::kPlane + ks * 256;      // P^T: rows = key pixels [64 wg, +64), k = query rows
-                    wgmma_ss_n64(o, smem_desc(pa, 128, T::kPlane), desc_mnmaj<LK, BF>(db, ks, false), ks > 0, 1, 1);
-                    if constexpr (TERMS == 3) {
-                        wgmma_ss_n64(o, smem_desc(pa, 128, T::kPlane), desc_mnmaj<LK, BF>(db, ks, true), 1, 1, 1);
-                        wgmma_ss_n64(o, smem_desc(pa + LOP, 128, T::kPlane), desc_mnmaj<LK, BF>(db, ks, false), 1, 1, 1);
+                    if constexpr (BF) {
+                        wgmma_ss_n64(o, smem_desc(pa, 128, T::kPlane), desc_mnmaj<LK, BF>(db, ks, false), ks > 0, 1, 1);
+                    } else {
+                        wgmma_ss_n32<1, 1>(o, smem_desc(pa, 128, T::kPlane), desc_mnmaj<LK, BF>(db, ks, false), ks > 0);
+                        wgmma_ss_n32<1, 1>(o, smem_desc(pa, 128, T::kPlane), desc_mnmaj<LK, BF>(db, ks, true), 1);
+                        wgmma_ss_n32<1, 1>(o, smem_desc(pa + LOP, 128, T::kPlane), desc_mnmaj<LK, BF>(db, ks, false), 1);
                     }
                 }
                 wg_commit();
-                wg_wait<0>();
-                wg_acc_fence<LK / 2>(dp);
-                wg_acc_fence<32>(o);
-                mbar_arrive(&empty[gv % kNLd]);
-                mbar_arrive(&empty[gd % kNLd]);
+            };
+            auto retire = [&](int n) {                             // chunk n's MMAs are complete
+                const uint32_t gv = g + per * n, gd = gv + 1;
+                wg_acc_fence<kCh / 2>(o);
+                mbar_arrive(&empty[rslot(gv)]);
+                mbar_arrive(&empty[rslot(gd)]);
 #pragma unroll
                 for (int h = 0; h < 2; ++h)
                     if (kok[h]) {
-                        E *row = dv + kpix[h] * p.C + n * kNC + cq;
+                        E *row = dv + kpix[h] * p.C + n * kCh + cq;
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) put2(row + 8 * j, o[4 * j + 2 * h], o[4 * j + 2 * h + 1], !prod);
+                        for (int j = 0; j < kCh / 8; ++j) put2(row + 8 * j, o[4 * j + 2 * h], o[4 * j + 2 * h + 1], !prod);
                     }
+            };
+            convert_chunk(0);
+            for (int n = 0; n < NCH; ++n) {
+                issue(n);
+                if (n + 1 < NCH) convert_chunk(n + 1);
+                wg_wait<0>();
+                retire(n);
             }
+            wg_acc_fence<LK / 2>(dp);
+            g += per * NCH;
             // ---------------- delta of the query rows
             float dl[2] = {0.f, 0.f};
             if (calc) {
@@ -313,6 +349,7 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
             fence_proxy_async();
             consumers_sync();
             // ---------------- dQ = dS K (rows = query pixels), dK = dS^T Q (rows = key pixels)
+            // Two groups: dQ's rows are written while the dK MMAs run (one accumulator set of 32 live at a time).
             {
                 float aq[32], ak[32];
                 wg_fence();
@@ -324,6 +361,13 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                         wgmma_ss_n64(aq, smem_desc(a, T::kPlane, 128), desc_mnmaj<LK, BF>(kb, ks, true), 1, 0, 1);
                         wgmma_ss_n64(aq, smem_desc(a + LOP, T::kPlane, 128), desc_mnmaj<LK, BF>(kb, ks, false), 1, 0, 1);
                     }
+                }
+                wg_commit();
+                wg_wait<0>();
+                wg_acc_fence<32>(aq);
+                wg_fence();
+#pragma unroll
+                for (int ks = 0; ks < KP; ++ks) {
                     const uint32_t at = pb + 8 * wg * T::kPlane + ks * 256;         // dS^T, MN-major (k = query pixels)
                     wgmma_ss_n64(ak, smem_desc(at, 128, T::kPlane), desc_mnmaj<LK, BF>(qb, ks, false), ks > 0, 1, 1);
                     if constexpr (TERMS == 3) {
@@ -332,21 +376,27 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                     }
                 }
                 wg_commit();
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    if (qok[h]) {
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            const int c = 8 * j + cq;
+                            if (c < p.Cq) put2(dq + qpix[h] * p.Cq + c, aq[4 * j + 2 * h], aq[4 * j + 2 * h + 1], !prod);
+                        }
+                    }
                 wg_wait<0>();
-                wg_acc_fence<32>(aq);
                 wg_acc_fence<32>(ak);
                 mbar_arrive(qk_empty);
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
+                for (int h = 0; h < 2; ++h)
+                    if (kok[h]) {
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const int c = 8 * j + cq;
-                        if (c < p.Cq) {
-                            if (qok[h]) put2(dq + qpix[h] * p.Cq + c, aq[4 * j + 2 * h], aq[4 * j + 2 * h + 1], !prod);
-                            if (kok[h]) put2(dk + kpix[h] * p.Cq + c, ak[4 * j + 2 * h], ak[4 * j + 2 * h + 1], !prod);
+                        for (int j = 0; j < 8; ++j) {
+                            const int c = 8 * j + cq;
+                            if (c < p.Cq) put2(dk + kpix[h] * p.Cq + c, ak[4 * j + 2 * h], ak[4 * j + 2 * h + 1], !prod);
                         }
                     }
-                }
             }
             if (prod) __threadfence();
             consumers_sync();                                      // (also: the planes and dsum are free for the next item)

@@ -9,7 +9,8 @@ namespace cca {
 namespace tc {
 using namespace sm90;
 
-constexpr int kNC = 64;   // channels per chunk (one ring slot = [LK px][64 ch] fp32 = two swizzled TMA tiles)
+constexpr int kNC = 64;   // channels per chunk (forward ring slot = [LK px][64 ch] fp32 = two swizzled TMA tiles; the backward's
+                          // ring slots are one tile, cca_tc_bwd.cu)
 
 // Thread layout of the attention kernels (three warpgroups):
 //   warpgroup 0           : TMA producer (one elected lane of warp 0), the rest idle
@@ -19,6 +20,11 @@ constexpr int kThreads = 384;
 constexpr int kConsumers = 256;
 constexpr int kBarConsumers = 1;   // named barrier of the 256 consumer threads
 constexpr int kBarConvert = 2;     // named barrier inside a conversion
+// Register split (setmaxnreg): the producer warpgroup only runs one TMA lane, so it gives its registers to the consumers.  The
+// kernels are launched with 168 registers per thread (384 threads, one CTA per SM); the split must fit that same pool.
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
+static_assert(128 * kProducerRegs + kConsumers * kConsumerRegs <= kThreads * 168, "register split exceeds the launch allocation");
 
 // BF = false: fp32 I/O, every operand split into bf16 hi + lo (3 MMAs per product).
 // BF = true : bf16 I/O, operands used as they are (1 MMA per product); a 64-channel chunk is ONE 128-byte-wide TMA tile.
@@ -63,13 +69,13 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads)
 }
 __device__ __forceinline__ void consumers_sync() { named_bar_sync(kBarConsumers, kConsumers); }
 
-// Conversion of one staged slot ([LK px][64 ch] fp32 as two swizzled 32-channel TMA boxes) into bf16 hi/lo operand planes
-// [8-channel chunk][pixel][16 B], IN PLACE, by the 256 consumer threads (thread t: pixel row t & 127, 32-channel half t >> 7 of
-// the slot, i.e. 16 channels of each box).  Every thread reads its 2 x 64 B, the consumers meet, then overwrite; the planes are
-// made visible to wgmma (async proxy) and every consumer has passed the closing barrier on return.
+// Conversion of one staged slot (NB swizzled 32-channel fp32 TMA boxes: [LK px][64 ch] for NB = 2, [LK px][32 ch] for NB = 1)
+// into bf16 hi/lo operand planes [8-channel chunk][pixel][16 B], IN PLACE, by the 256 consumer threads (thread t: pixel row
+// t & 127, 16-channel half t >> 7 of each box).  Every thread reads its NB x 64 B, the consumers meet, then overwrite; the
+// planes are made visible to wgmma (async proxy) and every consumer has passed the closing barrier on return.
 // With `dot` (the O tile of the same pixels, same layout): returns this thread's part of sum_c slot[r][c] * dot[r][c].
-// bf16 slots need no conversion; only the dot product is computed.
-template <int LK, bool BF>
+// bf16 slots (one 64-channel box) need no conversion; only the dot product is computed.
+template <int LK, bool BF, int NB = 2>
 __device__ __forceinline__ float convert_slot(uint8_t *slot, int t, const uint8_t *dot = nullptr)
 {
     using T = Tiles<LK, BF>;
@@ -90,15 +96,16 @@ __device__ __forceinline__ float convert_slot(uint8_t *slot, int t, const uint8_
         }
         return r < LK ? acc : 0.f;
     } else {
-        float4 raw[8];
+        static_assert(NB == 1 || NB == 2, "boxes per slot");
+        float4 raw[4 * NB];
 #pragma unroll
-        for (int bx = 0; bx < 2; ++bx)
+        for (int bx = 0; bx < NB; ++bx)
 #pragma unroll
             for (int j = 0; j < 4; ++j)
                 raw[4 * bx + j] = *reinterpret_cast<const float4 *>(slot + bx * T::kTile + rr * 128 + (((hq * 4 + j) ^ sw) * 16));
         if (dot) {
 #pragma unroll
-            for (int bx = 0; bx < 2; ++bx)
+            for (int bx = 0; bx < NB; ++bx)
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     const float4 o = *reinterpret_cast<const float4 *>(dot + bx * T::kTile + rr * 128 + (((hq * 4 + j) ^ sw) * 16));
@@ -109,7 +116,7 @@ __device__ __forceinline__ float convert_slot(uint8_t *slot, int t, const uint8_
         named_bar_sync(kBarConvert, kConsumers);
         if (r < LK) {
 #pragma unroll
-            for (int bx = 0; bx < 2; ++bx) {
+            for (int bx = 0; bx < NB; ++bx) {
                 uint8_t *d = slot + bx * T::kTile + r * 16 + hq * 2 * T::kPStride;
 #pragma unroll
                 for (int j = 0; j < 2; ++j) {
@@ -128,7 +135,9 @@ __device__ __forceinline__ float convert_slot(uint8_t *slot, int t, const uint8_
     }
 }
 
-// Operand descriptors of a [LK px][64 ch] slot (bf16 tile or fp32 planes; `lo`: the lo planes), 16-element k-step ks:
+// Operand descriptors of a [LK px][64 ch] slot (bf16 tile or fp32 planes; `lo`: the lo planes), 16-element k-step ks.  A
+// one-box fp32 slot ([LK px][32 ch], converted with NB = 1) has the layout of the first half of a two-box slot: the same
+// descriptors serve it with ks < 2 (K-major) or N = 32 (MN-major).
 //   channels as the contraction (K-major, rows = pixels starting at row0)
 template <int LK, bool BF> __device__ __forceinline__ uint64_t desc_kmaj(uint32_t slot, int row0, int ks, bool lo)
 {

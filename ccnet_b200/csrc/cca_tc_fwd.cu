@@ -89,9 +89,10 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
     }
     __syncthreads();
 
-    if (warp == 0) {
+    if (tid < 128) {
         // =============================== TMA producer ===============================
-        if (lane == 0) {
+        setmaxnreg_dec<kProducerRegs>();
+        if (warp == 0 && lane == 0) {
             const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
             auto load = [&](uint8_t *dst, uint64_t *bar, const CUtensorMap *m, int c0, const Item &it, int start) {
                 const int cw = it.col ? it.line : start, ch = it.col ? start : it.line;
@@ -119,8 +120,9 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 }
             }
         }
-    } else if (tid >= 128) {
+    } else {
         // =============================== consumers (warpgroup wg = query rows [64 wg, 64 wg + 64)) ===============================
+        setmaxnreg_inc<kConsumerRegs>();
         const int t = tid - 128, wg = t >> 7, wq = (t >> 5) & 3;
         const int rbase = 64 * wg + 16 * wq + (lane >> 2);         // rows rbase, rbase + 8 of the accumulators
         const uint32_t qb = smem_u32(smem + S::off_qk), kb = qb + T::kSlot, ld_base = smem_u32(smem + S::off_ld);
