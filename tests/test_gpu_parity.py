@@ -1,13 +1,16 @@
 """GPU parity tests (H100: ``pytest -m gpu``).  Every call goes through the C ABI
 (ccnet_b200.functional -> ctypes -> libcca_b200.so); the oracle is only the checker.
 
-Tolerances (BASELINE.json north_star): fp32 max-abs <= 1e-3 on identical Q/K/V; bf16 <= 1e-2
-against the fp32 oracle evaluated on the bf16-rounded Q/K/V (SURVEY.md 8c)."""
+Tolerances: fp32 results of the tensor-core kernels are held to the bf16x3 error budget derived in tests/tc_budget.py (about
+1e-4 relative), fp32 results of the generic kernels to plain fp32 accuracy (2e-5); bf16 <= 1e-2 against the oracle evaluated on
+the bf16-rounded Q/K/V (SURVEY.md 8c).  FP32_TOL (BASELINE.json north_star) remains for the module's parameter gradients."""
 import ctypes
 
 import numpy as np
 import pytest
 import torch
+
+import tc_budget as tb
 
 pytestmark = pytest.mark.gpu
 
@@ -25,6 +28,12 @@ def _dev():
 def _oracle():
     from oracle import cca_oracle
     return cca_oracle
+
+
+def _fp32_budget(shape, impl="auto"):
+    """the budget of whichever kernels run an fp32 problem of this shape (q, k of scale <= 1)"""
+    from ccnet_b200.functional import tc_eligible
+    return tb.FP32_BUDGET if impl != "simt" and tc_eligible(*shape, torch.float32) else tb.FP32_SIMT
 
 
 def _rand_qkv(B, Cq, C, H, W, seed, scale=1.0, dtype=torch.float32):
@@ -46,7 +55,8 @@ def test_forward_vs_golden_reference_outputs(golden, impl):
     assert torch.isfinite(out).all() and torch.isfinite(lse).all()
     err = (out.double() - ref).abs().max().item()
     assert err <= FP32_TOL, (golden["name"], err)
-    assert err <= 1e-4 * max(1.0, ref.abs().max().item()), (golden["name"], err)   # SIMT / 3xbf16 are ~fp32 exact
+    tol = tb.FP32_SIMT["out"] if impl == "simt" else 1e-4                           # plain fp32 / within the bf16x3 budget
+    assert err <= tol * max(1.0, ref.abs().max().item()), (golden["name"], err)
 
 
 SHAPES = [
@@ -67,7 +77,7 @@ def test_forward_fp32_vs_oracle(shape, impl):
     out, lse = cca_forward(q.to(dev), k.to(dev), v.to(dev), impl=impl)
     ro, rl = O.cca_forward(q.double(), k.double(), v.double())
     assert (out.cpu().double() - ro).abs().max().item() <= FP32_TOL
-    assert (lse.cpu().double() - rl).abs().max().item() <= FP32_TOL
+    tb.check(dict(out=out, lse=lse), dict(out=ro, lse=rl), _fp32_budget(shape, impl), (shape, impl))
 
 
 TC_SHAPES = [
@@ -90,10 +100,12 @@ def test_forward_tensor_core_vs_oracle_and_simt(shape):
     assert out.shape == v.shape and out.is_contiguous(memory_format=torch.channels_last)
     so, sl = cca_forward(qd, kd, vd, impl="simt")
     assert (out - so).abs().max().item() <= 5e-4 and (lse - sl).abs().max().item() <= 5e-4
+    tb.check(dict(out=out, lse=lse), dict(out=so.cpu().double(), lse=sl.cpu().double()), tb.FP32_BUDGET, (shape, "simt"))
     if shape[0] * shape[3] * shape[4] <= 4 * 97 * 97 or shape[0] == 1:
         ro, rl = O.cca_forward(q.double(), k.double(), v.double())
         assert (out.cpu().double() - ro).abs().max().item() <= 5e-4
         assert (lse.cpu().double() - rl).abs().max().item() <= 5e-4
+        tb.check(dict(out=out, lse=lse), dict(out=ro, lse=rl), tb.FP32_BUDGET, shape)
     # channels-last inputs give the same result (no hidden layout dependence): bit-identical with one tile per line (one
     # store + one add per element); with tiled lines an element is the sum of 2*nt-1 adds whose order is not fixed
     out2, _ = cca_forward(qd.contiguous(memory_format=torch.channels_last), kd, vd.contiguous(memory_format=torch.channels_last), impl="tc")
@@ -118,14 +130,17 @@ def test_backward_tensor_core_vs_oracle(shape):
     dq, dk, dv = cca_backward(dd, qd, kd, vd, out, lse, impl="tc")
     assert dv.shape == v.shape and dv.is_contiguous(memory_format=torch.channels_last)
     rq, rk, rv = O.cca_backward(dout.double(), q.double(), k.double(), v.double())
-    for got, ref, name in ((dq, rq, "dq"), (dk, rk, "dk"), (dv, rv, "dv")):
-        tol = FP32_TOL * max(1.0, ref.abs().max().item())
-        err = (got.cpu().double() - ref).abs().max().item()
-        assert err <= tol, (name, err, tol)
+    budget = tb.FP32_BUDGET
+    if shape[3] == shape[4] == 1:
+        # a 1x1 map: dq and dk are exactly 0 and what the kernels return is the rounding residue of dP - delta, two C-long dot
+        # products (1.5e-4 here).  The fp64 emulation of the kernel arithmetic leaves the same residue: hold them to 3x that.
+        emu = tb.emulate(q, k, v, dout)
+        budget = dict(budget, dq=3 * tb.error("dq", emu["dq"], rq), dk=3 * tb.error("dk", emu["dk"], rk))
+    tb.check(dict(dq=dq, dk=dk, dv=dv), dict(dq=rq, dk=rk, dv=rv), budget, shape)
     # and against the generic kernels
     sq, sk, sv = cca_backward(dd, qd, kd, vd, out, lse, impl="simt")
-    for got, ref in ((dq, sq), (dk, sk), (dv, sv)):
-        assert (got - ref).abs().max().item() <= FP32_TOL * max(1.0, ref.abs().max().item())
+    tb.check(dict(dq=dq, dk=dk, dv=dv), dict(dq=sq.cpu().double(), dk=sk.cpu().double(), dv=sv.cpu().double()), budget,
+             (shape, "simt"))
 
 
 @pytest.mark.parametrize("shape", [(2, 32, 256, 20, 97), (1, 64, 64, 112, 80), (3, 16, 64, 1, 5), (2, 64, 512, 33, 47), (2, 64, 512, 97, 97),
@@ -207,7 +222,7 @@ def test_launch_knobs_are_bit_identical(dtype):
 def test_backward_full_batch_c2_vs_oracle(dtype, tol):
     """BASELINE config 2 (B=8, C=512, 97x97): forward AND backward of the persistent single-launch schedule (776 lines per
     direction over one persistent CTA per SM, delta hand-off between CTAs) against the fp64 oracle on the first, a middle and
-    the last sample."""
+    the last sample (fp32: at the bf16x3 budget)."""
     from ccnet_b200 import cca_backward, cca_forward
     O = _oracle()
     dev = _dev()
@@ -222,6 +237,10 @@ def test_backward_full_batch_c2_vs_oracle(dtype, tol):
         sl = slice(b, b + 1)
         ro, rl = O.cca_forward(q[sl].double(), k[sl].double(), v[sl].double())
         rq, rk, rv = O.cca_backward(dout[sl].double(), q[sl].double(), k[sl].double(), v[sl].double())
+        if dtype == "fp32":
+            tb.check(dict(out=out[sl], lse=lse[sl], dq=dq[sl], dk=dk[sl], dv=dv[sl]), dict(out=ro, lse=rl, dq=rq, dk=rk, dv=rv),
+                     tb.FP32_BUDGET, b)
+            continue
         assert (out[sl].cpu().double() - ro).abs().max().item() <= tol * max(1.0, ro.abs().max().item()), b
         assert (lse[sl].cpu().double() - rl).abs().max().item() <= tol, b
         for got, ref, name in ((dq, rq, "dq"), (dk, rk, "dk"), (dv, rv, "dv")):
@@ -230,7 +249,7 @@ def test_backward_full_batch_c2_vs_oracle(dtype, tol):
 
 
 def test_tensor_core_peaky_softmax_stress():
-    """q,k ~ N(0,1)*1.5: logits std ~18, near one-hot attention; error budget still 1e-3."""
+    """q,k ~ N(0,1)*1.5: logits std ~18, near one-hot attention; the peaked-softmax budget of tests/tc_budget.py."""
     from ccnet_b200 import cca_forward
     O = _oracle()
     dev = _dev()
@@ -238,7 +257,7 @@ def test_tensor_core_peaky_softmax_stress():
     out, lse = cca_forward(q.to(dev), k.to(dev), v.to(dev), impl="tc")
     ro, rl = O.cca_forward(q.double(), k.double(), v.double())
     assert (out.cpu().double() - ro).abs().max().item() <= FP32_TOL
-    assert (lse.cpu().double() - rl).abs().max().item() <= FP32_TOL
+    tb.check(dict(out=out, lse=lse), dict(out=ro, lse=rl), tb.FP32_PEAKED_BUDGET)
 
 
 @pytest.mark.parametrize("impl", IMPLS)
@@ -268,9 +287,7 @@ def test_backward_fp32_vs_oracle(shape):
     out, lse = cca_forward(q.to(dev), k.to(dev), v.to(dev))
     dq, dk, dv = cca_backward(dout.to(dev), q.to(dev), k.to(dev), v.to(dev), out, lse)
     rq, rk, rv = O.cca_backward(dout.double(), q.double(), k.double(), v.double())
-    for got, ref, name in ((dq, rq, "dq"), (dk, rk, "dk"), (dv, rv, "dv")):
-        tol = FP32_TOL * max(1.0, ref.abs().max().item())
-        assert (got.cpu().double() - ref).abs().max().item() <= tol, name
+    tb.check(dict(dq=dq, dk=dk, dv=dv), dict(dq=rq, dk=rk, dv=rv), _fp32_budget(shape), shape)
 
 
 def test_backward_bf16_vs_oracle():
@@ -299,7 +316,9 @@ def test_module_vs_golden_fwd_bwd(golden):
     for _ in range(int(golden["R"])):
         y = m(y)
     (y * torch.from_numpy(golden["g"]).to(dev)).sum().backward()
-    assert (y.detach().cpu() - torch.from_numpy(golden["y"])).abs().max().item() <= FP32_TOL
+    yref = torch.from_numpy(golden["y"])
+    assert (y.detach().cpu() - yref).abs().max().item() <= FP32_TOL
+    assert (y.detach().cpu() - yref).abs().max().item() <= tb.FP32_BUDGET["out"] * max(1.0, yref.abs().max().item())
     assert (x.grad.cpu() - torch.from_numpy(golden["dx"])).abs().max().item() <= FP32_TOL * max(
         1.0, float(np.abs(golden["dx"]).max()))
     for n, p in m.named_parameters():
@@ -333,7 +352,7 @@ def test_full_size_properties_and_oracle_c2():
     for b in (0, 7):
         ro, rl = O.cca_forward(q[b:b + 1].cpu().double(), k[b:b + 1].cpu().double(), v1[b:b + 1].cpu().double())
         assert (o1[b:b + 1].cpu().double() - ro).abs().max().item() <= FP32_TOL
-        assert (lse[b:b + 1].cpu().double() - rl).abs().max().item() <= FP32_TOL
+        tb.check(dict(out=o1[b:b + 1], lse=lse[b:b + 1]), dict(out=ro, lse=rl), tb.FP32_BUDGET, b)
     # per-sample independence: permuting the batch permutes the output
     perm = torch.tensor([3, 0, 7, 1, 2, 6, 5, 4], device=dev)
     op, _ = cca_forward(q[perm], k[perm], v1[perm])
@@ -341,7 +360,7 @@ def test_full_size_properties_and_oracle_c2():
 
 
 def test_host_buffer_entry_point():
-    """cca_b200_forward_host / backward_host: plain host pointers through the C ABI."""
+    """cca_b200_forward_host / backward_host: plain host pointers through the C ABI (NCHW: the generic kernels, fp32 exact)."""
     from ccnet_b200 import capi
     O = _oracle()
     _dev()
@@ -355,15 +374,14 @@ def test_host_buffer_entry_point():
     rc = lib.cca_b200_forward_host(p(qn), p(kn), p(vn), p(out), p(lse), B, Cq, C, H, W, capi.CCA_F32, 0)
     capi.check(rc, "forward_host")
     ro, rl = O.cca_forward(q.double(), k.double(), v.double())
-    assert np.abs(out - ro.numpy()).max() <= FP32_TOL and np.abs(lse - rl.numpy()).max() <= FP32_TOL
+    tb.check(dict(out=torch.from_numpy(out), lse=torch.from_numpy(lse)), dict(out=ro, lse=rl), tb.FP32_SIMT)
     dout = np.random.default_rng(0).standard_normal((B, C, H, W)).astype(np.float32)
     dq, dk, dv = np.empty_like(qn), np.empty_like(kn), np.empty_like(vn)
     rc = lib.cca_b200_backward_host(p(dout), p(qn), p(kn), p(vn), p(out), p(lse), p(dq), p(dk), p(dv),
                                     B, Cq, C, H, W, capi.CCA_F32, 0)
     capi.check(rc, "backward_host")
     rq, rk, rv = O.cca_backward(torch.from_numpy(dout).double(), q.double(), k.double(), v.double())
-    for got, ref in ((dq, rq), (dk, rk), (dv, rv)):
-        assert np.abs(got - ref.numpy()).max() <= FP32_TOL * max(1.0, ref.abs().max().item())
+    tb.check(dict(dq=torch.from_numpy(dq), dk=torch.from_numpy(dk), dv=torch.from_numpy(dv)), dict(dq=rq, dk=rk, dv=rv), tb.FP32_SIMT)
 
 
 def test_error_behaviour_on_gpu():
@@ -388,7 +406,7 @@ def test_noncontiguous_inputs_and_fresh_output():
     vd = v.to(dev).to(memory_format=torch.channels_last)
     out, _ = cca_forward(qd, k.to(dev), vd)
     ro, _ = O.cca_forward(q.double(), k.double(), v.double())
-    assert (out.cpu().double() - ro).abs().max().item() <= FP32_TOL
+    tb.check(dict(out=out), dict(out=ro), tb.FP32_SIMT)                     # Cq = 4: the generic kernels
     assert out.data_ptr() != vd.data_ptr()
 
 
@@ -464,6 +482,7 @@ def test_fused_module_step_c512_vs_oracle_module():
     yr = ref(ref(xr))
     (yr * g).sum().backward()
     assert (y.detach().cpu() - yr.detach()).abs().max().item() <= FP32_TOL
+    assert (y.detach().cpu() - yr.detach()).abs().max().item() <= tb.FP32_BUDGET["out"] * max(1.0, yr.abs().max().item())
     assert (xd.grad.cpu() - xr.grad).abs().max().item() <= FP32_TOL * max(1.0, xr.grad.abs().max().item())
     rp = dict(ref.named_parameters())
     for n, p in m.named_parameters():
