@@ -114,6 +114,43 @@ __device__ __forceinline__ void tma_load_4d(void *dst, const CUtensorMap *m, uin
         ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(pol)
         : "memory");
 }
+// 4-D tensor stores shared -> global (bulk groups): plain store, and reduce-add performed at L2 (element type of the tensor
+// map).  The shared tile is written by the generic proxy, so the writers run fence_proxy_async() before the issuing thread
+// is released to issue.  Box elements past the tensor's extent are not written.
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap *m, const void *src, int c0, int c1, int c2, int c3)
+{
+    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap *m, const void *src, int c0, int c1, int c2, int c3, uint64_t pol)
+{
+    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3, %4, %5}], [%1], %6;"
+                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap *m, const void *src, int c0, int c1, int c2, int c3)
+{
+    asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+__device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap *m, const void *src, int c0, int c1, int c2, int c3, uint64_t pol)
+{
+    asm volatile("cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group.L2::cache_hint [%0, {%2, %3, %4, %5}], [%1], %6;"
+                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(pol) : "memory");
+}
+// bulk groups of the issuing thread: commit the stores issued since the last commit; wait until at most N groups are
+// pending (wait: their writes are complete; wait_read: they have finished reading shared memory, which may then be reused)
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// orders this thread's generic-proxy accesses of global memory (e.g. an acquire of a counter) with its async-proxy ones
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+// publish a counter: everything this thread's completed bulk stores wrote (bulk_wait<0> first) happens-before the bump
+__device__ __forceinline__ void publish_count(unsigned int *cnt)
+{
+    fence_proxy_async_global();
+    __threadfence();
+    atomicAdd(cnt, 1u);
+}
 
 // ---------------------------------------------------------------- wgmma
 // Shared-memory matrix descriptor of wgmma (start >> 4 [0,14), lbo >> 4 [16,30), sbo >> 4 [32,46), layout [62,64)).

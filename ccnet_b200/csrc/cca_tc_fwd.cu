@@ -13,7 +13,7 @@
 // sample finds q,k,v in L2 and adds onto output lines that are still L2-resident.
 //
 // Two touches per output element, ordered: the "producer" items of a sample (column lines, first key block) STORE their
-// rows, every other item of the sample ADDS onto them (vector reductions at L2) once the per-sample counter cdone[b] says all
+// rows, every other item of the sample ADDS onto them (TMA reduce-add at L2) once the per-sample counter cdone[b] says all
 // producers have completed their stores.  Items are walked in the lagged order of cca_items.cuh -- P(0) | P(1) C(0) | ... --
 // so a consumer practically never waits; only items with a LOWER index are ever waited for and each persistent CTA walks its
 // items in increasing order, so the wait cannot cycle.  With one tile per line every output element is one store plus one
@@ -24,9 +24,12 @@
 //                         SWIZZLE_128B, pixels past the line zero-filled.
 //   consumer warpgroups : fp32 only: tiles -> bf16 hi + lo planes in place (x = hi + lo to ~2^-17).  S = Q K^T (wgmma, both
 //                         operands in shared memory), P = exp2(S log2e - lse2) in registers, re-packed as the bf16 A operand of
-//                         O = P V (wgmma with A from registers, 3 MMAs per k-step for fp32 I/O), O rows stored / added
-//                         straight from the accumulators.
-#include <type_traits>
+//                         O = P V (wgmma with A from registers, 3 MMAs per k-step for fp32 I/O).
+//   chunk pipeline      : two O accumulators.  While chunk n's wgmma group runs, chunk n - 1's O is written into chunk n - 1's
+//                         own V slot (its MMAs have retired) in the swizzled layout of the output's TMA box and chunk n + 1's
+//                         slot is converted; then chunk n is waited for, one thread stores / reduce-adds chunk n - 1 with TMA,
+//                         and chunk n + 1 is issued.  A slot goes back to the producer once its bulk copy has read it,
+//                         checked one chunk later.
 
 #include "cca_items.cuh"
 #include "cca_tc_common.cuh"
@@ -41,10 +44,9 @@ struct FwdParams {
     long npix;
     const float *parts;    // [nparts][B*H*W] partial log2-sum-exp2 (statistics pre-pass)
     float *lse;            // [B,H,W] natural-log lse (saved for backward)
-    void *out;             // [B,H,W,C] fp32 or bf16
     unsigned int *cdone;   // [B] producer items of sample b whose stores have completed (cleared by the statistics kernel)
     int lag;               // item order: 1 = consumers trail the producers by one block, 0 = sample after sample
-    int hints;             // L2 eviction hints on the loads
+    int hints;             // L2 eviction hints on the loads and the output stores
 };
 
 template <int LK, bool BF> struct FwdSmem {
@@ -56,7 +58,7 @@ template <int LK, bool BF> struct FwdSmem {
                                                                    // (128 - LK) rows past a tile; they only feed discarded rows
     static constexpr int off_bar = off_tail + (128 - LK) * 128 + 1024;
     static constexpr int kBytes = off_bar + 8 * (2 + 2 * kNLd);
-    static_assert(kNLd >= 2, "ring depth");
+    static_assert(kNLd >= 4, "ring depth: chunks n - 2 (store reading), n - 1 (staged), n (MMAs), n + 1 (converting)");
     static_assert(kBytes <= 232448, "shared memory budget");
 };
 
@@ -64,11 +66,11 @@ template <int LK, bool BF>
 __global__ void __launch_bounds__(kThreads, 1)
 cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant__ CUtensorMap mqr,
                   const __grid_constant__ CUtensorMap mkc, const __grid_constant__ CUtensorMap mkr,
-                  const __grid_constant__ CUtensorMap mvc, const __grid_constant__ CUtensorMap mvr, FwdParams p)
+                  const __grid_constant__ CUtensorMap mvc, const __grid_constant__ CUtensorMap mvr,
+                  const __grid_constant__ CUtensorMap moc, const __grid_constant__ CUtensorMap mor, FwdParams p)
 {
     using T = Tiles<LK, BF>;
     using S = FwdSmem<LK, BF>;
-    using E = typename std::conditional<BF, __nv_bfloat16, float>::type;
     constexpr int kNLd = S::kNLd;
     constexpr int TERMS = BF ? 1 : 3;
     constexpr int KP = LK / 16;               // k-steps of O = P V
@@ -83,9 +85,10 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
 
     if (tid == 0) {
         mbar_init(qk_full, 1); mbar_init(qk_empty, kConsumers);
-        for (int i = 0; i < kNLd; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kConsumers); }
+        for (int i = 0; i < kNLd; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }   // empty: the store-issuing thread
         fence_mbar_init();
         prefetch_tmap(&mqc); prefetch_tmap(&mqr); prefetch_tmap(&mkc); prefetch_tmap(&mkr); prefetch_tmap(&mvc); prefetch_tmap(&mvr);
+        prefetch_tmap(&moc); prefetch_tmap(&mor);
     }
     __syncthreads();
 
@@ -126,12 +129,52 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
         const int t = tid - 128, wg = t >> 7, wq = (t >> 5) & 3;
         const int rbase = 64 * wg + 16 * wq + (lane >> 2);         // rows rbase, rbase + 8 of the accumulators
         const uint32_t qb = smem_u32(smem + S::off_qk), kb = qb + T::kSlot, ld_base = smem_u32(smem + S::off_ld);
-        E *const out = reinterpret_cast<E *>(p.out);
+        const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
+        // chunk n's O (this thread's rows rbase, rbase + 8; 64 channels) -> its V slot, laid out as the output's swizzled TMA
+        // box(es) [tile px][128 B]; accumulator rows past LK are padding and would land in the next slot, so they are skipped
+        auto stage = [&](const float (&o)[32], uint8_t *slot) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = rbase + 8 * h;
+                if (r >= LK) continue;
+                uint8_t *row = slot + r * 128;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const int c = 8 * j + 2 * (lane & 3);
+                    const int bx = BF ? 0 : c >> 5, byte = BF ? 2 * c : 4 * (c & 31);
+                    uint8_t *dst = row + bx * T::kTile + ((((byte >> 4) ^ r) & 7) << 4) + (byte & 15);
+                    if constexpr (BF) *reinterpret_cast<uint32_t *>(dst) = pack_bf16(o[4 * j + 2 * h], o[4 * j + 2 * h + 1]);
+                    else *reinterpret_cast<float2 *>(dst) = make_float2(o[4 * j + 2 * h], o[4 * j + 2 * h + 1]);
+                }
+            }
+        };
         pdl_wait();                                                // parts and the counters come from the statistics kernel
         uint32_t g = 0;
+        int pending = -1;                                          // (thread 0) slot whose bulk store may still be reading it
         for (int k = 0; k < nk; ++k) {
             const Item it = item_of(k);
             const bool prod = is_producer(it);
+            // ---- final lse2 of rows rbase (h = 0), rbase + 8 (h = 1); independent of S, so loaded before S is waited for
+            float nlse[2];
+            int self[2];
+            bool rok[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = rbase + 8 * h;
+                rok[h] = r < it.lq;
+                const long pix = item_pixel(p.sp, it, rok[h] ? r : 0);
+                self[h] = it.col ? it.q0 + r - it.k0 : -1;
+                float lse2 = 0.f;
+                if (rok[h]) {
+                    float m = -INFINITY;
+                    for (int i = 0; i < p.sp.nparts; ++i) m = fmaxf(m, __ldcg(p.parts + (long)i * p.npix + pix));
+                    float sum = 0.f;
+                    for (int i = 0; i < p.sp.nparts; ++i) sum += exp2f(__ldcg(p.parts + (long)i * p.npix + pix) - m);
+                    lse2 = m + log2f(sum);
+                    if (!it.col && it.ik == 0 && (lane & 3) == 0) p.lse[pix] = lse2 * kLn2;
+                }
+                nlse[h] = -lse2;
+            }
             // ---- S = Q K^T
             mbar_wait(qk_full, k & 1);
             if constexpr (!BF) {
@@ -151,28 +194,7 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
             wg_wait<0>();
             wg_acc_fence<LK / 2>(acc);
             mbar_arrive(qk_empty);
-            // ---- P = exp2(S log2e - lse2) for rows rbase (h = 0), rbase + 8 (h = 1), as bf16 A fragments (hi, lo)
-            long pix[2];
-            float nlse[2];
-            int self[2];
-            bool rok[2];
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int r = rbase + 8 * h;
-                rok[h] = r < it.lq;
-                pix[h] = item_pixel(p.sp, it, rok[h] ? r : 0);
-                self[h] = it.col ? it.q0 + r - it.k0 : -1;
-                float lse2 = 0.f;
-                if (rok[h]) {
-                    float m = -INFINITY;
-                    for (int i = 0; i < p.sp.nparts; ++i) m = fmaxf(m, __ldcg(p.parts + (long)i * p.npix + pix[h]));
-                    float sum = 0.f;
-                    for (int i = 0; i < p.sp.nparts; ++i) sum += exp2f(__ldcg(p.parts + (long)i * p.npix + pix[h]) - m);
-                    lse2 = m + log2f(sum);
-                    if (!it.col && it.ik == 0 && (lane & 3) == 0) p.lse[pix[h]] = lse2 * kLn2;
-                }
-                nlse[h] = -lse2;
-            }
+            // ---- P = exp2(S log2e - lse2) as bf16 A fragments (hi, lo)
             uint32_t ph[KP][4], pl[KP][4];
 #pragma unroll
             for (int j = 0; j < LK / 8; ++j)
@@ -192,14 +214,21 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                         split2(p0, p1, ph[j / 2][reg], pl[j / 2][reg]);
                     }
                 }
-            if (!prod) wait_count(p.cdone + it.b, (unsigned)p.sp.seg0);   // every producer of this sample has stored its rows
-            // ---- O = P V, 64 channels at a time
-            for (int n = 0; n < NCH; ++n, ++g) {
-                const int slot = g % kNLd;
-                mbar_wait(&full[slot], (g / kNLd) & 1);
-                if constexpr (!BF) convert_slot<LK, BF>(smem + S::off_ld + slot * T::kSlot, t);
-                const uint32_t vb = ld_base + slot * T::kSlot;
-                float o[32];
+            // ---- O = P V, 64 channels at a time.  Chunk n's wgmma group runs while chunk n - 1's O (the other accumulator)
+            // is staged and chunk n + 1 is converted; only then is chunk n waited for and chunk n + 1 issued.  One group is in
+            // flight at a time: with chunk n + 1 issued before chunk n is waited for, the accumulator that chunk n + 1 later
+            // overwrites is read inside chunk n's pipeline stage and ptxas serialises every wgmma (C7514).
+            const uint32_t g0 = g;
+            g += NCH;
+            const CUtensorMap *const mo = it.col ? &moc : &mor;
+            const int ow = it.col ? it.line : it.q0, oh = it.col ? it.q0 : it.line;
+            auto slot_of = [&](int n) { return (int)((g0 + n) % kNLd); };
+            auto prep = [&](int n) {                               // chunk n's V has landed; fp32: split into planes
+                mbar_wait(&full[slot_of(n)], ((g0 + n) / kNLd) & 1);
+                if constexpr (!BF) convert_slot<LK, BF>(smem + S::off_ld + slot_of(n) * T::kSlot, t);
+            };
+            auto mma = [&](float (&o)[32], int n) {
+                const uint32_t vb = ld_base + slot_of(n) * T::kSlot;
                 wg_fence();
 #pragma unroll
                 for (int ks = 0; ks < KP; ++ks) {
@@ -210,23 +239,66 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                     }
                 }
                 wg_commit();
-                wg_wait<0>();
+            };
+            auto write = [&](float (&o)[32], int n) {              // chunk n has retired in both warpgroups after the barrier
                 wg_acc_fence<32>(o);
-                mbar_arrive(&empty[slot]);
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    if (rok[h]) {
-                        E *row = out + pix[h] * p.C + n * kNC + 2 * (lane & 3);
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) put2(row + 8 * j, o[4 * j + 2 * h], o[4 * j + 2 * h + 1], !prod);
-                    }
-            }
-            if (prod) {                                            // publish: all stores of this item are visible
-                __threadfence();
                 consumers_sync();
-                if (t == 0) atomicAdd(p.cdone + it.b, 1u);
+                stage(o, smem + S::off_ld + slot_of(n) * T::kSlot);
+                fence_proxy_async();
+                consumers_sync();
+            };
+            auto store = [&](int n) {                              // chunk n is staged
+                if (t != 0) return;
+                if (n == 0 && !prod) fence_proxy_async_global();  // the counter's acquire (below) before the reduce-adds
+                const uint8_t *sl = smem + S::off_ld + slot_of(n) * T::kSlot;
+#pragma unroll
+                for (int bx = 0; bx < (BF ? 1 : 2); ++bx) {
+                    const int c0 = n * kNC + 32 * bx;
+                    const uint8_t *src = sl + bx * T::kTile;
+                    if (p.hints == 1) {                            // producers' rows are added onto by the sample's consumers
+                        if (prod) tma_store_4d(mo, src, c0, ow, oh, it.b, pol_keep);
+                        else tma_reduce_add_4d(mo, src, c0, ow, oh, it.b, pol_stream);
+                    } else {
+                        if (prod) tma_store_4d(mo, src, c0, ow, oh, it.b);
+                        else tma_reduce_add_4d(mo, src, c0, ow, oh, it.b);
+                    }
+                }
+                bulk_commit();
+                bulk_wait_read<1>();                               // the previous chunk's store has read its slot
+                if (pending >= 0) mbar_arrive(&empty[pending]);
+                pending = slot_of(n);
+            };
+            // chunk n in flight in oc, chunk n - 1 retired in op
+            auto step = [&](float (&oc)[32], float (&op)[32], int n) {
+                if (n > 0) write(op, n - 1);
+                const bool more = n + 1 < NCH;
+                if (more) prep(n + 1);
+                wg_wait<0>();
+                if (n > 0) store(n - 1);
+                if (more) mma(op, n + 1);
+            };
+            // every producer of this sample has stored its rows (all threads wait: a spin in thread 0 alone, while a wgmma
+            // group is in flight, makes ptxas serialise the wgmmas)
+            if (!prod) wait_count(p.cdone + it.b, (unsigned)p.sp.seg0);
+            float o0[32], o1[32];
+            prep(0);
+            mma(o0, 0);
+            for (int n = 0; n < NCH; n += 2) {
+                step(o0, o1, n);
+                if (n + 1 < NCH) step(o1, o0, n + 1);
+            }
+            wg_wait<0>();                                          // (nothing is pending; ptxas cannot tell which step ran last)
+            if (NCH & 1) write(o0, NCH - 1);
+            else write(o1, NCH - 1);
+            store(NCH - 1);
+            if (prod && t == 0) {                                  // publish: all stores of this item are complete
+                bulk_wait<0>();
+                mbar_arrive(&empty[pending]);
+                pending = -1;
+                publish_count(p.cdone + it.b);
             }
         }
+        if (t == 0) bulk_wait<0>();                                // shared memory must outlive the last bulk reads
     }
 }
 
@@ -234,21 +306,24 @@ template <int LK, bool BF>
 cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, float *lse, const float *parts, unsigned int *cdone,
                        Dims d, cudaStream_t st, const char **why)
 {
-    CUtensorMap m[6];
-    const void *base[3] = {q, k, v};
-    const int ch[3] = {d.Cq, d.Cq, d.C};
+    CUtensorMap m[8];
+    const void *base[4] = {q, k, v, out};
+    const int ch[4] = {d.Cq, d.Cq, d.C, d.C};
     FwdParams p;
     p.sp = make_space(d.B, d.H, d.W);
-    for (int t = 0; t < 3; ++t)
-        for (int r = 0; r < 2; ++r)
-            // LK-pixel boxes: pixels past the line are zero-filled
-            if (!get_map(&m[2 * t + r], base[t], d.B, d.H, d.W, ch[t], LK, r == 0, BF)) {
+    for (int t = 0; t < 4; ++t)
+        for (int r = 0; r < 2; ++r) {
+            // loads: LK-pixel boxes, pixels past the line are zero-filled; output: boxes of one tile of the direction, so a
+            // store never reaches into the next tile of a line (pixels past the line are not written)
+            const int box = t < 3 ? LK : (r == 0 ? p.sp.col.tl : p.sp.row.tl);
+            if (!get_map(&m[2 * t + r], base[t], d.B, d.H, d.W, ch[t], box, r == 0, BF)) {
                 if (why) *why = "cuTensorMapEncodeTiled failed";
                 return cudaErrorInvalidValue;
             }
+        }
     p.C = d.C; p.Cq = d.Cq;
     p.npix = (long)d.B * d.H * d.W;
-    p.parts = parts; p.lse = lse; p.cdone = cdone; p.out = out;
+    p.parts = parts; p.lse = lse; p.cdone = cdone;
     p.lag = tc_lag() != 0 ? 1 : 0;                 // default (-1): lagged
     p.hints = tc_l2_hints();
     auto kern = cca_tc_fwd_kernel<LK, BF>;
@@ -263,7 +338,7 @@ cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, f
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = tc_pdl() ? 1 : 0;     // may start ahead of the statistics kernel's completion (griddepcontrol.wait inside)
-    e = cudaLaunchKernelEx(&cfg, kern, m[0], m[1], m[2], m[3], m[4], m[5], p);
+    e = cudaLaunchKernelEx(&cfg, kern, m[0], m[1], m[2], m[3], m[4], m[5], m[6], m[7], p);
     count_launch();
     return e != cudaSuccess ? e : cudaGetLastError();
 }
