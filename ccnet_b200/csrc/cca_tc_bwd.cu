@@ -20,12 +20,12 @@
 // Output path (dq, dk, dv need no initialisation by the caller).  One tile per line (H, W <= 112): as in the forward the
 // column items STORE their rows, the row items ADD onto them once the per-sample counter cdone[b] says every column item of the
 // sample has completed its stores.  Tiled lines: several items contribute to the same dk / dv rows, so a prologue clears the
-// outputs and every item adds.
+// outputs and every item adds.  Every output tile is staged in shared memory in the swizzled layout of the output's TMA box and
+// written by one thread with a TMA store or a TMA reduce-add at L2: a dV chunk in the dO slot of its chunk, dQ in the K slot,
+// dK in the P / dS planes, each once the MMAs that read that memory have retired in both warpgroups.
 //
 // All GEMMs run as bf16x3 split MMAs (hi*hi + hi*lo + lo*hi) with fp32 accumulation in registers (single bf16 MMAs for bf16
 // I/O), two consumer warpgroups of 64 rows each (cca_tc_common.cuh).
-#include <type_traits>
-
 #include "cca_items.cuh"
 #include "cca_tc_common.cuh"
 
@@ -44,13 +44,13 @@ struct BwdParams {
     int out_mode;              // 1: producers store, consumers add after cdone (one tile per line); 0: cleared outputs, everything adds
     unsigned int *cdone;       // [B] producer items of sample b whose stores have completed (out_mode 1)
     int lag;                   // item order (cca_items.cuh): 1 = consumers trail the producers by one block
-    int hints;                 // L2 eviction hints on the loads
-    void *dq, *dk, *dv;
+    int hints;                 // L2 eviction hints on the loads and the output stores
 };
 
 // The V / dO / O ring holds chunks of ONE 128-byte TMA box each: 32 channels for fp32 (converted in place to hi/lo planes),
 // 64 for bf16.  Small slots buy depth: at LK = 112 fp32 the ring has 8 slots (2 2/3 chunks of V, dO, O), so chunk n + 1 lands
-// and is converted while chunk n's MMAs run and chunk n + 2 is on its way.
+// and is converted while chunk n's MMAs run.  A dV chunk has the footprint of a slot and is staged in its chunk's dO slot,
+// which goes back to the producer once the bulk copy has read it.
 template <int LK, bool BF> struct BwdSmem {
     using T = Tiles<LK, BF>;
     static constexpr int kCh = BF ? kNC : kNC / 2;                  // channels per ring slot / per chunk
@@ -68,10 +68,13 @@ template <int LK, bool BF> struct BwdSmem {
     static constexpr int off_dsum = off_tail + kTail;
     static constexpr int off_bar = off_dsum + kDsum;
     static constexpr int kBytes = off_bar + 8 * (2 + 2 * kNLd);
-    // The chunk loop holds chunk n's V, dO (its MMAs are in flight) while it waits for chunk n + 1's V, dO, O: the ring must hold
-    // two full chunks, or the producer could not issue chunk n + 1 before chunk n is released and the pipeline would stall
-    // (or, below 5 slots, deadlock).
-    static_assert(kNLd >= 6, "ring depth: two chunks of V, dO, O");
+    // The ring is filled in order, so what counts is the span from the oldest slot still held to the newest one waited for.
+    // While chunk n's MMAs run, the conversion of chunk n + 1 waits for chunk n + 1's V, dO, O; chunk n - 1's dO slot holds its
+    // staged dV until the conversion has ended (the bulk copy is checked then), chunk n's V and dO are in the MMAs.  From
+    // chunk n - 1's dO to chunk n + 1's O that is 8 slots; with fewer the producer could not load chunk n + 1: deadlock.
+    static_assert(kNLd >= 8, "ring depth: chunk n - 1's dO (staged dV) up to chunk n + 1's O");
+    // dK is staged in the P / dS planes: two (fp32) or one (bf16) swizzled [LK px][128 B] boxes, 1024-byte aligned
+    static_assert(off_p % 1024 == 0 && T::kP >= T::kSlot, "dK staging in the P / dS planes");
     static_assert(kBytes <= kBudget, "shared memory budget");
 };
 
@@ -84,11 +87,13 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                   const __grid_constant__ CUtensorMap mkc, const __grid_constant__ CUtensorMap mkr,
                   const __grid_constant__ CUtensorMap mvc, const __grid_constant__ CUtensorMap mvr,
                   const __grid_constant__ CUtensorMap mdoc, const __grid_constant__ CUtensorMap mdor,
-                  const __grid_constant__ CUtensorMap moc, const __grid_constant__ CUtensorMap mor, BwdParams p)
+                  const __grid_constant__ CUtensorMap moc, const __grid_constant__ CUtensorMap mor,
+                  const __grid_constant__ CUtensorMap mdqc, const __grid_constant__ CUtensorMap mdqr,
+                  const __grid_constant__ CUtensorMap mdkc, const __grid_constant__ CUtensorMap mdkr,
+                  const __grid_constant__ CUtensorMap mdvc, const __grid_constant__ CUtensorMap mdvr, BwdParams p)
 {
     using T = Tiles<LK, BF>;
     using S = BwdSmem<LK, BF>;
-    using E = typename std::conditional<BF, __nv_bfloat16, float>::type;
     constexpr int TERMS = BF ? 1 : 3;
     constexpr int kNLd = S::kNLd;
     constexpr int kCh = S::kCh;
@@ -105,11 +110,13 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
     auto item_of = [&](int k) { return decode_item_order(p.sp, (int)blockIdx.x + k * (int)gridDim.x, p.lag); };
 
     if (tid == 0) {
-        mbar_init(qk_full, 1); mbar_init(qk_empty, kConsumers);
-        for (int i = 0; i < kNLd; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kConsumers); }
+        // empty barriers: one arrival per use of a slot (consumer thread 0, after the barrier or bulk read that ends the use)
+        mbar_init(qk_full, 1); mbar_init(qk_empty, 1);
+        for (int i = 0; i < kNLd; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
         fence_mbar_init();
         prefetch_tmap(&mqc); prefetch_tmap(&mqr); prefetch_tmap(&mkc); prefetch_tmap(&mkr); prefetch_tmap(&mvc); prefetch_tmap(&mvr);
         prefetch_tmap(&mdoc); prefetch_tmap(&mdor); prefetch_tmap(&moc); prefetch_tmap(&mor);
+        prefetch_tmap(&mdqc); prefetch_tmap(&mdqr); prefetch_tmap(&mdkc); prefetch_tmap(&mdkr); prefetch_tmap(&mdvc); prefetch_tmap(&mdvr);
     }
     __syncthreads();
 
@@ -159,25 +166,59 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
         const uint32_t qb = smem_u32(smem + S::off_qk), kb = qb + T::kSlot, ld_base = smem_u32(smem + S::off_ld);
         const uint32_t pb = smem_u32(smem + S::off_p);
         uint8_t *pgen = smem + S::off_p;
-        E *const dq = reinterpret_cast<E *>(p.dq), *const dk = reinterpret_cast<E *>(p.dk), *const dv = reinterpret_cast<E *>(p.dv);
+        const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
+        // this thread's accumulator rows rbase, rbase + 8 (nc channels from 0) -> `tile`, laid out as the output's swizzled TMA
+        // box(es) [tile px][128 B] (fp32: 32-channel boxes T::kTile apart); rows past LK are padding and are skipped
+        auto stage = [&](const float *acc, int nc, uint8_t *tile) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = rbase + 8 * h;
+                if (r >= LK) continue;
+                uint8_t *row = tile + r * 128;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    if (8 * j >= nc) break;
+                    const int c = 8 * j + cq;
+                    const int bx = BF ? 0 : c >> 5, byte = BF ? 2 * c : 4 * (c & 31);
+                    uint8_t *dst = row + bx * T::kTile + ((((byte >> 4) ^ r) & 7) << 4) + (byte & 15);
+                    if constexpr (BF) *reinterpret_cast<uint32_t *>(dst) = pack_bf16(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                    else *reinterpret_cast<float2 *>(dst) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                }
+            }
+        };
+        // (thread 0) the staged boxes -> global: producers store, everybody else reduce-adds; L2 hints as for the loads
+        auto put = [&](const CUtensorMap *m, const uint8_t *tile, int boxes, int c0, int px0, const Item &it, bool prod) {
+            const int cw = it.col ? it.line : px0, ch = it.col ? px0 : it.line;
+            for (int bx = 0; bx < boxes; ++bx) {
+                const uint8_t *src = tile + bx * T::kTile;
+                if (p.hints == 1) {
+                    if (prod) tma_store_4d(m, src, c0 + 32 * bx, cw, ch, it.b, pol_keep);
+                    else tma_reduce_add_4d(m, src, c0 + 32 * bx, cw, ch, it.b, pol_stream);
+                } else {
+                    if (prod) tma_store_4d(m, src, c0 + 32 * bx, cw, ch, it.b);
+                    else tma_reduce_add_4d(m, src, c0 + 32 * bx, cw, ch, it.b);
+                }
+            }
+            bulk_commit();
+        };
+        // dQ / dK boxes: 64 channels (fp32: two boxes; a box wholly past Cq is not issued, TMA clips the rest)
+        const int qboxes = BF ? 1 : (p.Cq > 32 ? 2 : 1);
         pdl_wait();                                                // prep kernel complete: counters (and the outputs) cleared
         uint32_t g = 0;
+        int pending = -1;                                          // (thread 0) ring slot whose bulk copy may still be reading it
         for (int k = 0; k < nk; ++k) {
             const Item it = item_of(k);
             const bool calc = calc_delta(p, it);
             const bool prod = p.out_mode == 1 && is_producer(it);
-            Item kit = it;                                         // key pixels of the item as "query rows" (pixel addressing)
-            kit.q0 = it.k0;
-            long qpix[2], kpix[2];
-            bool qok[2], kok[2];
+            long qpix[2];
+            bool qok[2];
             float nlse[2];
             int self[2];
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int r = rbase + 8 * h;
-                qok[h] = r < it.lq; kok[h] = r < it.lk;
+                qok[h] = r < it.lq;
                 qpix[h] = item_pixel(p.sp, it, qok[h] ? r : 0);
-                kpix[h] = item_pixel(p.sp, kit, kok[h] ? r : 0);
                 nlse[h] = qok[h] ? -p.lse[qpix[h]] * kLog2e : 0.f;
                 self[h] = it.col ? it.q0 + r - it.k0 : -1;
             }
@@ -200,6 +241,8 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 wg_commit();
                 wg_wait<0>();
                 wg_acc_fence<LK / 2>(acc);
+                if (t == 0) bulk_wait_read<0>();                   // the previous item's dK copy has read the P / dS planes
+                consumers_sync();
 #pragma unroll
                 for (int j = 0; j < LK / 8; ++j)
 #pragma unroll
@@ -225,12 +268,15 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
             fence_proxy_async();
             consumers_sync();
             if (!prod && p.out_mode == 1) wait_count(p.cdone + it.b, (unsigned)p.sp.seg0);   // producers of the sample have stored
+            // the counter's acquire (or the prep kernel's clear, tiled lines) before this item's reduce-adds
+            if (!prod && t == 0) fence_proxy_async_global();
             // ---------------- per chunk: dP += dO V^T, dV = P^T dO
-            // Pipelined over the chunks: issue chunk n's MMAs, convert chunk n + 1 (and accumulate its delta dot) while they run,
-            // wait, release chunk n's slots and write its dV.  One group in flight at a time: with a second one (wg_wait<1>
-            // and a second dV accumulator, so that the dV writes also overlap the MMAs) ptxas treats the groups chained
-            // through dP as one pipeline stage, sees the other dV accumulator read inside it and serialises every wgmma of
-            // the kernel (C7514); at LK = 112 fp32 the second accumulator also spills.
+            // Pipelined over the chunks: chunk n's MMAs run while chunk n + 1 is converted (and its delta dot accumulated); then
+            // chunk n is waited for, its V slot released, its dV staged in its dO slot and stored by one thread with TMA, and
+            // chunk n + 1 is issued.  The dO slot goes back to the producer at the end of the next conversion, when the copy
+            // has long read it.  One group in flight at a time: with a second one (wg_wait<1> and a second dV accumulator)
+            // ptxas treats the groups chained through dP as one pipeline stage, sees the other dV accumulator read inside it and
+            // serialises every wgmma of the kernel (C7514); at LK = 112 fp32 the second accumulator also spills.
             float dp[LK / 2];
             float o[kCh / 2];                                      // dV of the chunk
             float dacc = 0.f;
@@ -246,7 +292,7 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 if (calc) {
                     dacc += convert_slot<LK, BF, 1>(ds, t, smem + S::off_ld + rslot(go) * S::kRSlot);
                     if constexpr (BF) consumers_sync();            // (fp32: the conversion ends on a consumer barrier)
-                    mbar_arrive(&empty[rslot(go)]);
+                    if (t == 0) mbar_arrive(&empty[rslot(go)]);
                 } else if constexpr (!BF) {
                     convert_slot<LK, BF, 1>(ds, t);
                 }
@@ -276,26 +322,37 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 }
                 wg_commit();
             };
-            auto retire = [&](int n) {                             // chunk n's MMAs are complete
+            auto release = [&]() {                                 // (thread 0) the previous chunk's dV copy has read its slot
+                if (t == 0 && pending >= 0) {
+                    bulk_wait_read<0>();
+                    mbar_arrive(&empty[pending]);
+                    pending = -1;
+                }
+            };
+            auto retire = [&](int n) {                             // chunk n's MMAs are complete in this warpgroup
                 const uint32_t gv = g + per * n, gd = gv + 1;
                 wg_acc_fence<kCh / 2>(o);
-                mbar_arrive(&empty[rslot(gv)]);
-                mbar_arrive(&empty[rslot(gd)]);
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    if (kok[h]) {
-                        E *row = dv + kpix[h] * p.C + n * kCh + cq;
-#pragma unroll
-                        for (int j = 0; j < kCh / 8; ++j) put2(row + 8 * j, o[4 * j + 2 * h], o[4 * j + 2 * h + 1], !prod);
-                    }
+                consumers_sync();                                  // ... and in the other: V and dO are free
+                if (t == 0) mbar_arrive(&empty[rslot(gv)]);
+                uint8_t *ds = smem + S::off_ld + rslot(gd) * S::kRSlot;
+                stage(o, kCh, ds);
+                fence_proxy_async();
+                consumers_sync();
+                if (t == 0) {
+                    put(it.col ? &mdvc : &mdvr, ds, 1, n * kCh, it.k0, it, prod);
+                    pending = (int)rslot(gd);
+                }
             };
             convert_chunk(0);
+            issue(0);
             for (int n = 0; n < NCH; ++n) {
-                issue(n);
                 if (n + 1 < NCH) convert_chunk(n + 1);
+                release();
                 wg_wait<0>();
                 retire(n);
+                if (n + 1 < NCH) issue(n + 1);
             }
+            wg_wait<0>();                                          // (nothing is pending; ptxas cannot tell which step ran last)
             wg_acc_fence<LK / 2>(dp);
             g += per * NCH;
             // ---------------- delta of the query rows
@@ -349,7 +406,8 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
             fence_proxy_async();
             consumers_sync();
             // ---------------- dQ = dS K (rows = query pixels), dK = dS^T Q (rows = key pixels)
-            // Two groups: dQ's rows are written while the dK MMAs run (one accumulator set of 32 live at a time).
+            // Two groups (one accumulator set of 32 live at a time): dQ is staged in the K slot (dK reads dS and Q) and its bulk
+            // copy runs with the dK MMAs; dK is staged in the P / dS planes once its MMAs have retired.
             {
                 float aq[32], ak[32];
                 wg_fence();
@@ -365,6 +423,11 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 wg_commit();
                 wg_wait<0>();
                 wg_acc_fence<32>(aq);
+                consumers_sync();                                  // both warpgroups' dQ MMAs have read the K slot
+                stage(aq, 64, smem + S::off_qk + T::kSlot);
+                fence_proxy_async();
+                consumers_sync();
+                if (t == 0) put(it.col ? &mdqc : &mdqr, smem + S::off_qk + T::kSlot, qboxes, 0, it.q0, it, prod);
                 wg_fence();
 #pragma unroll
                 for (int ks = 0; ks < KP; ++ks) {
@@ -376,32 +439,26 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                     }
                 }
                 wg_commit();
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    if (qok[h]) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const int c = 8 * j + cq;
-                            if (c < p.Cq) put2(dq + qpix[h] * p.Cq + c, aq[4 * j + 2 * h], aq[4 * j + 2 * h + 1], !prod);
-                        }
-                    }
                 wg_wait<0>();
                 wg_acc_fence<32>(ak);
-                mbar_arrive(qk_empty);
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    if (kok[h]) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const int c = 8 * j + cq;
-                            if (c < p.Cq) put2(dk + kpix[h] * p.Cq + c, ak[4 * j + 2 * h], ak[4 * j + 2 * h + 1], !prod);
-                        }
+                consumers_sync();                                  // both warpgroups' dK MMAs have read dS and Q
+                stage(ak, 64, pgen);
+                fence_proxy_async();
+                consumers_sync();                                  // (also: the planes and dsum are free for the next item)
+                if (t == 0) {
+                    put(it.col ? &mdkc : &mdkr, pgen, qboxes, 0, it.k0, it, prod);
+                    bulk_wait_read<1>();                           // the last dV copy and the dQ copy have read their slots
+                    if (pending >= 0) mbar_arrive(&empty[pending]);
+                    pending = -1;
+                    mbar_arrive(qk_empty);
+                    if (prod) {                                    // publish: all stores of this item are complete
+                        bulk_wait<0>();
+                        publish_count(p.cdone + it.b);
                     }
+                }
             }
-            if (prod) __threadfence();
-            consumers_sync();                                      // (also: the planes and dsum are free for the next item)
-            if (prod && t == 0) atomicAdd(p.cdone + it.b, 1u);     // publish: all stores of this item are visible
         }
+        if (t == 0) bulk_wait<0>();                                // shared memory must outlive the last bulk reads
     }
 }
 
@@ -422,18 +479,21 @@ cudaError_t launch_bwd(const void *dout, const void *q, const void *k, const voi
                        unsigned int *counters, void *dq, void *dk, void *dv, Dims d, int delta_mode, cudaStream_t st,
                        const char **why)
 {
-    CUtensorMap m[10];
-    const void *base[5] = {q, k, v, dout, out};
-    const int ch[5] = {d.Cq, d.Cq, d.C, d.C, d.C};
+    CUtensorMap m[16];
+    const void *base[8] = {q, k, v, dout, out, dq, dk, dv};
+    const int ch[8] = {d.Cq, d.Cq, d.C, d.C, d.C, d.Cq, d.Cq, d.C};
     BwdParams p;
     p.sp = make_space(d.B, d.H, d.W);
-    for (int t = 0; t < 5; ++t)
-        for (int r = 0; r < 2; ++r)
-            // LK-pixel boxes, zero-filled past the line
-            if (!get_map(&m[2 * t + r], base[t], d.B, d.H, d.W, ch[t], LK, r == 0, BF)) {
+    for (int t = 0; t < 8; ++t)
+        for (int r = 0; r < 2; ++r) {
+            // loads: LK-pixel boxes, zero-filled past the line; outputs: boxes of one tile of the direction, so a store never
+            // reaches into the next tile of a line (pixels past the line are not written)
+            const int box = t < 5 ? LK : (r == 0 ? p.sp.col.tl : p.sp.row.tl);
+            if (!get_map(&m[2 * t + r], base[t], d.B, d.H, d.W, ch[t], box, r == 0, BF)) {
                 if (why) *why = "cuTensorMapEncodeTiled failed";
                 return cudaErrorInvalidValue;
             }
+        }
     p.C = d.C; p.Cq = d.Cq;
     p.npix = (long)d.B * d.H * d.W;
     p.lse = lse; p.delta = delta;
@@ -443,7 +503,6 @@ cudaError_t launch_bwd(const void *dout, const void *q, const void *k, const voi
     p.out_mode = one_tile ? 1 : 0;
     p.lag = tc_lag() != 0 ? 1 : 0;
     p.hints = tc_l2_hints();
-    p.dq = dq; p.dk = dk; p.dv = dv;
     const long es = BF ? 2 : 4;
     const long nq = p.out_mode == 1 ? 0 : p.npix * d.Cq * es, nv = p.out_mode == 1 ? 0 : p.npix * d.C * es;
     cca_bwd_prep_kernel<<<p.out_mode == 1 ? 1 : sm_count(), 256, 0, st>>>(
@@ -463,7 +522,8 @@ cudaError_t launch_bwd(const void *dout, const void *q, const void *k, const voi
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = tc_pdl() ? 1 : 0;
-    e = cudaLaunchKernelEx(&cfg, kern, m[0], m[1], m[2], m[3], m[4], m[5], m[6], m[7], m[8], m[9], p);
+    e = cudaLaunchKernelEx(&cfg, kern, m[0], m[1], m[2], m[3], m[4], m[5], m[6], m[7], m[8], m[9], m[10], m[11], m[12], m[13],
+                           m[14], m[15], p);
     count_launch();
     return e != cudaSuccess ? e : cudaGetLastError();
 }

@@ -153,19 +153,6 @@ template <int LK, bool BF> __device__ __forceinline__ uint64_t desc_mnmaj(uint32
     else return smem_desc(slot + ks * 256 + (lo ? T::kLoOff : 0), 128, T::kPStride);
 }
 
-// global row stores of the accumulator layout: two consecutive channels per thread
-__device__ __forceinline__ void put2(float *p, float a, float b, bool add)
-{
-    if (add) atomicAdd(reinterpret_cast<float2 *>(p), make_float2(a, b));
-    else *reinterpret_cast<float2 *>(p) = make_float2(a, b);
-}
-__device__ __forceinline__ void put2(__nv_bfloat16 *p, float a, float b, bool add)
-{
-    const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-    if (add) atomicAdd(reinterpret_cast<__nv_bfloat162 *>(p), v);
-    else *reinterpret_cast<__nv_bfloat162 *>(p) = v;
-}
-
 // ---- host: TMA tensor maps over channels-last fp32 tensors -------------------------------------
 typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                              const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
