@@ -69,7 +69,8 @@ void count_launch(int n = 1);
 //   CCA_B200_PDL = 0/1        programmatic dependent launch between the launches of one op (default 1)
 //   CCA_B200_ZERO_AHEAD = n   the items of sample b clear the outputs of sample b+n (default 1)
 //   CCA_B200_DELTA = -1/0/1   backward: -1 automatic, 0 every item computes delta, 1 column items produce it for the sample
-//   CCA_B200_LAG = 0/1        item order: consumers of a sample trail its producers by one block (default 1)
+//   CCA_B200_LAG = 0/1        item order: consumers of a sample trail its producers by one block (default: 1 in the
+//                             backward; picked from the shape in the forward values kernel, cca_tc_fwd.cu)
 //   CCA_B200_L2HINT = 0/1     L2 eviction hints on the bulk copies (default 1)
 int tc_pdl();
 int tc_zero_ahead();

@@ -14,10 +14,12 @@
 //
 // Two touches per output element, ordered: the "producer" items of a sample (column lines, first key block) STORE their
 // rows, every other item of the sample ADDS onto them (TMA reduce-add at L2) once the per-sample counter cdone[b] says all
-// producers have completed their stores.  Items are walked in the lagged order of cca_items.cuh -- P(0) | P(1) C(0) | ... --
-// so a consumer practically never waits; only items with a LOWER index are ever waited for and each persistent CTA walks its
-// items in increasing order, so the wait cannot cycle.  With one tile per line every output element is one store plus one
-// add: the result is bit-reproducible; with key-block tiling a pixel gets 2*nt-1 adds whose order is not fixed.
+// producers have completed their stores.  Items are walked in one of the two orders of cca_items.cuh (launch_fwd picks it):
+// the lagged one -- P(0) | P(1) C(0) | ... -- in which a consumer practically never waits, or sample after sample, which
+// keeps one sample's v and out in the L2 instead of two.  Only items with a LOWER index are ever waited for and each
+// persistent CTA walks its items in increasing order, so the wait cannot cycle.  With one tile per line every output element
+// is one store plus one add: the result is bit-reproducible; with key-block tiling a pixel gets 2*nt-1 adds whose order is
+// not fixed.
 //
 // Roles (cca_tc_common.cuh):
 //   producer lane       : Q, K of an item into their own stage; the item's 64-channel V chunks into a ring.  4-D tiled loads,
@@ -268,18 +270,24 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 if (pending >= 0) mbar_arrive(&empty[pending]);
                 pending = slot_of(n);
             };
+            // before a consumer's first reduce-add: every producer of this sample has stored its rows.  Only the adds need it,
+            // so S, P and the first chunks' MMAs overlap the wait.  It sits where no wgmma group is in flight, and all threads
+            // wait: a spin in thread 0 alone, while a group is in flight, makes ptxas serialise the wgmmas.
+            auto acquire = [&](int n) {
+                if (n == 0 && !prod) wait_count(p.cdone + it.b, (unsigned)p.sp.seg0);
+            };
             // chunk n in flight in oc, chunk n - 1 retired in op
             auto step = [&](float (&oc)[32], float (&op)[32], int n) {
                 if (n > 0) write(op, n - 1);
                 const bool more = n + 1 < NCH;
                 if (more) prep(n + 1);
                 wg_wait<0>();
-                if (n > 0) store(n - 1);
+                if (n > 0) {
+                    acquire(n - 1);
+                    store(n - 1);
+                }
                 if (more) mma(op, n + 1);
             };
-            // every producer of this sample has stored its rows (all threads wait: a spin in thread 0 alone, while a wgmma
-            // group is in flight, makes ptxas serialise the wgmmas)
-            if (!prod) wait_count(p.cdone + it.b, (unsigned)p.sp.seg0);
             float o0[32], o1[32];
             prep(0);
             mma(o0, 0);
@@ -290,6 +298,7 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
             wg_wait<0>();                                          // (nothing is pending; ptxas cannot tell which step ran last)
             if (NCH & 1) write(o0, NCH - 1);
             else write(o1, NCH - 1);
+            acquire(NCH - 1);
             store(NCH - 1);
             if (prod && t == 0) {                                  // publish: all stores of this item are complete
                 bulk_wait<0>();
@@ -324,13 +333,19 @@ cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, f
     p.C = d.C; p.Cq = d.Cq;
     p.npix = (long)d.B * d.H * d.W;
     p.parts = parts; p.lse = lse; p.cdone = cdone;
-    p.lag = tc_lag() != 0 ? 1 : 0;                 // default (-1): lagged
     p.hints = tc_l2_hints();
+    const int sms = sm_count();
+    const int grid = p.sp.total < sms ? p.sp.total : sms;
+    // Item order (default; DESIGN.md 4).  Sample after sample, the first consumers of each sample wait for its last producers,
+    // up to about one item per CTA and sample; in the lagged order two samples' v and out are in play in the L2 instead of one.
+    // The wait weighs less the more items a sample has per CTA.  Measured on an H100 (132 SMs): sample after sample is faster
+    // from 4/3 items per CTA (lines of 89 pixels and more) with 4 samples or more, and slower with fewer items per CTA (lines
+    // of 73 and 81) or 2 samples.
+    const int lag = tc_lag();
+    p.lag = lag >= 0 ? lag : (d.B >= 4 && 3 * p.sp.per_sample >= 4 * grid ? 0 : 1);
     auto kern = cca_tc_fwd_kernel<LK, BF>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem<LK, BF>::kBytes);
     if (e != cudaSuccess) return e;
-    const int sms = sm_count();
-    const int grid = p.sp.total < sms ? p.sp.total : sms;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = FwdSmem<LK, BF>::kBytes; cfg.stream = st;
     cudaLaunchAttribute attr[1];
