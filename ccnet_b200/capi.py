@@ -12,7 +12,7 @@ import threading
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("CCA_B200_LIB") or os.path.join(_HERE, "lib", "libcca_b200.so")   # (override: another build flavour)
 
-CCA_F32, CCA_BF16 = 0, 1
+CCA_F32, CCA_BF16, CCA_F16 = 0, 1, 2
 CCA_FLAG_AUTO, CCA_FLAG_FORCE_SIMT, CCA_FLAG_FORCE_TC, CCA_FLAG_NHWC = 0, 1, 2, 4
 CCA_WS_FORWARD, CCA_WS_BACKWARD = 0, 1
 

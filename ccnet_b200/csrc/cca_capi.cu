@@ -28,11 +28,12 @@ int check_dims(int B, int Cq, int C, int H, int W, int dtype)
 {
     if (B <= 0 || Cq <= 0 || C <= 0 || H <= 0 || W <= 0)
         return fail(CCA_ERR_INVALID, "non-positive dimension%s%s");
-    if (dtype != CCA_F32 && dtype != CCA_BF16) return fail(CCA_ERR_INVALID, "dtype must be CCA_F32 or CCA_BF16%s%s");
+    if (dtype != CCA_F32 && dtype != CCA_BF16 && dtype != CCA_F16)
+        return fail(CCA_ERR_INVALID, "dtype must be CCA_F32, CCA_BF16 or CCA_F16%s%s");
     if ((long long)B * C * H * W >= (1ll << 40)) return fail(CCA_ERR_UNSUPPORTED, "tensor too large%s%s");
     return CCA_OK;
 }
-size_t esize(int dtype) { return dtype == CCA_F32 ? 4 : 2; }
+size_t esize(int dtype) { return dtype == CCA_F32 ? 4 : 2; }    // (CCA_BF16, CCA_F16: 2)
 }  // namespace
 
 void count_launch(int n) { g_launches.fetch_add((unsigned long long)n, std::memory_order_relaxed); }

@@ -1,6 +1,7 @@
 // Shared declarations for the criss-cross attention kernels (sm_90a).
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -24,9 +25,11 @@ struct Line {
 template <typename T> __device__ __forceinline__ float to_f(T x);
 template <> __device__ __forceinline__ float to_f<float>(float x) { return x; }
 template <> __device__ __forceinline__ float to_f<__nv_bfloat16>(__nv_bfloat16 x) { return __bfloat162float(x); }
+template <> __device__ __forceinline__ float to_f<__half>(__half x) { return __half2float(x); }
 template <typename T> __device__ __forceinline__ T from_f(float x);
 template <> __device__ __forceinline__ float from_f<float>(float x) { return x; }
 template <> __device__ __forceinline__ __nv_bfloat16 from_f<__nv_bfloat16>(float x) { return __float2bfloat16_rn(x); }
+template <> __device__ __forceinline__ __half from_f<__half>(float x) { return __float2half_rn(x); }
 
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
@@ -70,7 +73,7 @@ void count_launch(int n = 1);
 //   CCA_B200_ZERO_AHEAD = n   the items of sample b clear the outputs of sample b+n (default 1)
 //   CCA_B200_DELTA = -1/0/1   backward: -1 automatic, 0 every item computes delta, 1 column items produce it for the sample
 //   CCA_B200_LAG = 0/1        item order: consumers of a sample trail its producers by one block (default: 1 in the
-//                             backward; picked from the shape in the forward values kernel, cca_tc_fwd.cu)
+//                             backward; picked from the shape in the forward values kernel, cca_tc_fwd.cuh)
 //   CCA_B200_L2HINT = 0/1     L2 eviction hints on the bulk copies (default 1)
 int tc_pdl();
 int tc_zero_ahead();

@@ -1,6 +1,6 @@
 // Generic CUDA-core (FFMA) criss-cross attention kernels for sm_90a: any dtype/shape within
 // the shared-memory limits.  They are the shape-general companion of the wgmma kernels
-// (cca_tc_fwd.cu) and the first correct CUDA path of the operator.
+// (cca_tc_fwd.cuh) and the first correct CUDA path of the operator.
 //
 // Decomposition (replaces cc_attention/functions.py:30-47 without materialising any
 // [B,H,W,H+W] tensor in HBM): the criss-cross softmax of a pixel couples one image column and
@@ -435,6 +435,7 @@ cudaError_t simt_forward(const void *q, const void *k, const void *v, void *out,
                          Dims d, int dtype, cudaStream_t st, const char **why)
 {
     (void)why;
+    if (dtype == CCA_F16) return fwd_typed<__half>(q, k, v, out, lse, ws, d, st);
     return dtype == CCA_F32 ? fwd_typed<float>(q, k, v, out, lse, ws, d, st)
                             : fwd_typed<__nv_bfloat16>(q, k, v, out, lse, ws, d, st);
 }
@@ -444,6 +445,7 @@ cudaError_t simt_backward(const void *dout, const void *q, const void *k, const 
                           cudaStream_t st, const char **why)
 {
     (void)why;
+    if (dtype == CCA_F16) return bwd_typed<__half>(dout, q, k, v, out, lse, dq, dk, dv, ws, d, st);
     return dtype == CCA_F32 ? bwd_typed<float>(dout, q, k, v, out, lse, dq, dk, dv, ws, d, st)
                             : bwd_typed<__nv_bfloat16>(dout, q, k, v, out, lse, dq, dk, dv, ws, d, st);
 }

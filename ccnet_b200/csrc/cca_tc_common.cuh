@@ -1,6 +1,8 @@
-// Pieces shared by the wgmma statistics, forward and backward kernels (channels-last, fp32 I/O as a bf16x3 split, or bf16 I/O).
+// Pieces shared by the wgmma statistics, forward and backward kernels (channels-last; fp32 I/O as a bf16x3 split, or bf16 or
+// f16 I/O).
 #pragma once
 #include <mutex>
+#include <type_traits>
 
 #include "cca_common.cuh"
 #include "cca_sm90.cuh"
@@ -10,7 +12,7 @@ namespace tc {
 using namespace sm90;
 
 constexpr int kNC = 64;   // channels per chunk (forward ring slot = [LK px][64 ch] fp32 = two swizzled TMA tiles; the backward's
-                          // ring slots are one tile, cca_tc_bwd.cu)
+                          // ring slots are one tile, cca_tc_bwd.cuh)
 
 // Thread layout of the attention kernels (three warpgroups):
 //   warpgroup 0           : TMA producer (one elected lane of warp 0), the rest idle
@@ -26,17 +28,23 @@ constexpr int kProducerRegs = 40;
 constexpr int kConsumerRegs = 232;
 static_assert(128 * kProducerRegs + kConsumers * kConsumerRegs <= kThreads * 168, "register split exceeds the launch allocation");
 
-// BF = false: fp32 I/O, every operand split into bf16 hi + lo (3 MMAs per product).
-// BF = true : bf16 I/O, operands used as they are (1 MMA per product); a 64-channel chunk is ONE 128-byte-wide TMA tile.
-template <int LK, bool BF = false> struct Tiles {
-    static constexpr int kTile = LK * 128;             // [LK px][128 B] = 32 fp32 or 64 bf16 channels, SWIZZLE_128B
-    static constexpr int kSlot = BF ? kTile : 2 * kTile; // 64 channels
+// I/O element type E of the kernels:
+//   float        : fp32 I/O, every operand split into bf16 hi + lo (3 bf16 MMAs per product).
+//   __nv_bfloat16: bf16 I/O, operands used as they are (1 MMA per product); a 64-channel chunk is ONE 128-byte-wide TMA tile.
+//   __half       : f16 I/O, the layout of bf16 I/O with f16 MMAs and f16 packing of P, dS and the staged outputs.
+template <typename E> constexpr bool kH16 = sizeof(E) == 2;                      // 16-bit I/O (bf16 or f16)
+template <typename E> constexpr bool kF16 = std::is_same<E, __half>::value;
+template <typename E> constexpr int kDtype = kF16<E> ? CCA_F16 : (kH16<E> ? CCA_BF16 : CCA_F32);
+template <int LK, typename E> struct Tiles {
+    static constexpr bool H16 = kH16<E>;
+    static constexpr int kTile = LK * 128;             // [LK px][128 B] = 32 fp32 or 64 bf16 / f16 channels, SWIZZLE_128B
+    static constexpr int kSlot = H16 ? kTile : 2 * kTile;  // 64 channels
     static constexpr int kPlane = LK * 16;             // operand plane: LK rows x 16 B (8 bf16)
     // fp32 I/O: a converted slot holds its 8-channel planes as  hi0 lo0 hi1 lo1 ... hi7 lo7  (each 32-channel TMA box is rewritten
     // inside its own bytes, so the two boxes of a slot are converted by two independent thread groups)
     static constexpr int kPStride = 2 * kPlane;        // hi plane p -> hi plane p+1 (and lo -> lo)
     static constexpr int kLoOff = kPlane;              // hi plane p -> lo plane p
-    static constexpr int kTerms = BF ? 1 : 2;          // operand copies kept: hi (+ lo)
+    static constexpr int kTerms = H16 ? 1 : 2;         // operand copies kept: hi (+ lo)
     static constexpr int kOp = kTerms * 8 * kPlane;    // 8 planes = 64 channels, per copy
     static constexpr int kPP = LK / 8;                 // planes of a [LK x LK] pixel-pixel matrix (P, dS)
     static constexpr int kP = kTerms * kPP * kPlane;
@@ -62,6 +70,27 @@ __device__ __forceinline__ void split8(const float *v, uint4 &hi, uint4 &lo)
 }
 __device__ __forceinline__ float bf_lo(uint32_t w) { return __uint_as_float(w << 16); }
 __device__ __forceinline__ float bf_hi(uint32_t w) { return __uint_as_float(w & 0xFFFF0000u); }
+// the same for a 16-bit operand type (F16: f16, else bf16): (a, b) -> packed pair (low half = a), and the halves back
+template <bool F16> __device__ __forceinline__ uint32_t pack2(float a, float b)
+{
+    if constexpr (F16) {
+        uint32_t r;
+        asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
+        return r;
+    } else {
+        return pack_bf16(a, b);
+    }
+}
+template <bool F16> __device__ __forceinline__ float lo2(uint32_t w)
+{
+    if constexpr (F16) return __half2float(__ushort_as_half((unsigned short)(w & 0xFFFFu)));
+    else return bf_lo(w);
+}
+template <bool F16> __device__ __forceinline__ float hi2(uint32_t w)
+{
+    if constexpr (F16) return __half2float(__ushort_as_half((unsigned short)(w >> 16)));
+    else return bf_hi(w);
+}
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads)
 {
@@ -74,15 +103,16 @@ __device__ __forceinline__ void consumers_sync() { named_bar_sync(kBarConsumers,
 // t & 127, 16-channel half t >> 7 of each box).  Every thread reads its NB x 64 B, the consumers meet, then overwrite; the
 // planes are made visible to wgmma (async proxy) and every consumer has passed the closing barrier on return.
 // With `dot` (the O tile of the same pixels, same layout): returns this thread's part of sum_c slot[r][c] * dot[r][c].
-// bf16 slots (one 64-channel box) need no conversion; only the dot product is computed.
-template <int LK, bool BF, int NB = 2>
+// 16-bit slots (one 64-channel box) need no conversion; only the dot product is computed.
+template <int LK, typename E, int NB = 2>
 __device__ __forceinline__ float convert_slot(uint8_t *slot, int t, const uint8_t *dot = nullptr)
 {
-    using T = Tiles<LK, BF>;
+    using T = Tiles<LK, E>;
+    constexpr bool H16 = T::H16, F16 = kF16<E>;
     const int r = t & 127, hq = t >> 7;
     const int rr = r < LK ? r : LK - 1, sw = rr & 7;
     float acc = 0.f;
-    if constexpr (BF) {
+    if constexpr (H16) {
         if (dot) {
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
@@ -91,7 +121,7 @@ __device__ __forceinline__ float convert_slot(uint8_t *slot, int t, const uint8_
                 const uint4 y = *reinterpret_cast<const uint4 *>(dot + rr * 128 + c * 16);
                 const uint32_t xw[4] = {x.x, x.y, x.z, x.w}, yw[4] = {y.x, y.y, y.z, y.w};
 #pragma unroll
-                for (int e = 0; e < 4; ++e) acc += bf_lo(xw[e]) * bf_lo(yw[e]) + bf_hi(xw[e]) * bf_hi(yw[e]);
+                for (int e = 0; e < 4; ++e) acc += lo2<F16>(xw[e]) * lo2<F16>(yw[e]) + hi2<F16>(xw[e]) * hi2<F16>(yw[e]);
             }
         }
         return r < LK ? acc : 0.f;
@@ -135,25 +165,25 @@ __device__ __forceinline__ float convert_slot(uint8_t *slot, int t, const uint8_
     }
 }
 
-// Operand descriptors of a [LK px][64 ch] slot (bf16 tile or fp32 planes; `lo`: the lo planes), 16-element k-step ks.  A
+// Operand descriptors of a [LK px][64 ch] slot (16-bit tile or fp32 planes; `lo`: the lo planes), 16-element k-step ks.  A
 // one-box fp32 slot ([LK px][32 ch], converted with NB = 1) has the layout of the first half of a two-box slot: the same
 // descriptors serve it with ks < 2 (K-major) or N = 32 (MN-major).
 //   channels as the contraction (K-major, rows = pixels starting at row0)
-template <int LK, bool BF> __device__ __forceinline__ uint64_t desc_kmaj(uint32_t slot, int row0, int ks, bool lo)
+template <int LK, typename E> __device__ __forceinline__ uint64_t desc_kmaj(uint32_t slot, int row0, int ks, bool lo)
 {
-    using T = Tiles<LK, BF>;
-    if constexpr (BF) return smem_desc(slot + row0 * 128 + ks * 32, 16, 1024, kSw128);
+    using T = Tiles<LK, E>;
+    if constexpr (T::H16) return smem_desc(slot + row0 * 128 + ks * 32, 16, 1024, kSw128);
     else return smem_desc(slot + row0 * 16 + ks * 2 * T::kPStride + (lo ? T::kLoOff : 0), T::kPStride, 128);
 }
 //   pixels as the contraction (MN-major: the 64 channels are the N dimension)
-template <int LK, bool BF> __device__ __forceinline__ uint64_t desc_mnmaj(uint32_t slot, int ks, bool lo)
+template <int LK, typename E> __device__ __forceinline__ uint64_t desc_mnmaj(uint32_t slot, int ks, bool lo)
 {
-    using T = Tiles<LK, BF>;
-    if constexpr (BF) return smem_desc(slot + ks * 2048, 16, 1024, kSw128);
+    using T = Tiles<LK, E>;
+    if constexpr (T::H16) return smem_desc(slot + ks * 2048, 16, 1024, kSw128);
     else return smem_desc(slot + ks * 256 + (lo ? T::kLoOff : 0), 128, T::kPStride);
 }
 
-// ---- host: TMA tensor maps over channels-last fp32 tensors -------------------------------------
+// ---- host: TMA tensor maps over channels-last tensors -------------------------------------
 typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                              const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
                              CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -170,17 +200,22 @@ inline EncodeFn get_encode()
     });
     return fn;
 }
-// NHWC tensor [B,H,W,C] (fp32 or bf16); box = [128 bytes of channels] x [LK pixels along W (row pass) or H (column pass)]
-inline bool make_map(CUtensorMap *m, const void *base, int B, int H, int W, int C, int LK, bool col, bool bf16 = false)
+// NHWC tensor [B,H,W,C] of cca_dtype `dtype`; box = [128 bytes of channels] x [LK pixels along W (row pass) or H (column
+// pass)].  The map's element type is also the arithmetic type of the TMA reduce-adds through it.
+inline bool make_map(CUtensorMap *m, const void *base, int B, int H, int W, int C, int LK, bool col, int dtype)
 {
     EncodeFn enc = get_encode();
     if (!enc) return false;
-    const cuuint64_t es_bytes = bf16 ? 2 : 4;
+    const bool h16 = dtype != CCA_F32;
+    const cuuint64_t es_bytes = h16 ? 2 : 4;
     cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
     cuuint64_t strides[3] = {(cuuint64_t)C * es_bytes, (cuuint64_t)W * C * es_bytes, (cuuint64_t)H * W * C * es_bytes};
-    cuuint32_t box[4] = {bf16 ? 64u : 32u, col ? 1u : (cuuint32_t)LK, col ? (cuuint32_t)LK : 1u, 1};
+    cuuint32_t box[4] = {h16 ? 64u : 32u, col ? 1u : (cuuint32_t)LK, col ? (cuuint32_t)LK : 1u, 1};
     cuuint32_t es[4] = {1, 1, 1, 1};
-    return enc(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<void *>(base), dims, strides, box, es,
+    const CUtensorMapDataType et = dtype == CCA_F16    ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                   : dtype == CCA_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                       : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+    return enc(m, et, 4, const_cast<void *>(base), dims, strides, box, es,
                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
@@ -188,12 +223,12 @@ inline bool make_map(CUtensorMap *m, const void *base, int B, int H, int W, int 
 inline int lk_for(int tile) { return tile <= 80 ? 80 : (tile <= 112 ? 112 : 0); }
 // Cached tensor maps (cca_tc_host.cu): encoding costs ~1 us of driver time per map and an op call needs 8-15 of them;
 // a map only depends on (base, shape, box, dtype), so it stays valid for as long as that address holds such a tensor.
-bool get_map(CUtensorMap *m, const void *base, int B, int H, int W, int C, int LK, bool col, bool bf16);
+bool get_map(CUtensorMap *m, const void *base, int B, int H, int W, int C, int LK, bool col, int dtype);
 // SM count of the CURRENT device (cached per device id)
 int sm_count();
 inline bool shape_supported(Dims d, int dtype)
 {
-    if (dtype != CCA_F32 && dtype != CCA_BF16) return false;
+    if (dtype != CCA_F32 && dtype != CCA_BF16 && dtype != CCA_F16) return false;
     if (d.Cq % 16 != 0 || d.Cq > 64 || d.Cq < 16 || d.C % kNC != 0) return false;
     if (d.H > 112 * 8 || d.W > 112 * 8) return false;        // cca_items.cuh: at most kMaxNT tiles of kMaxTile pixels per line
     return get_encode() != nullptr;

@@ -32,17 +32,19 @@ std::mutex g_sm_mu;
 int g_sm_count[64] = {};
 }  // namespace
 
-bool get_map(CUtensorMap *m, const void *base, int B, int H, int W, int C, int LK, bool col, bool bf16)
+bool get_map(CUtensorMap *m, const void *base, int B, int H, int W, int C, int LK, bool col, int dtype)
 {
     int dev = 0;
     cudaGetDevice(&dev);                       // the same virtual address may be a different tensor on another device
-    const MapKey key{base, B, H, W, C, LK, (col ? 1 : 0) | (bf16 ? 2 : 0) | (dev << 2)};
+    // the dtype is part of the key: a map of another element type over the same bytes would load, store and reduce-add in
+    // the wrong format
+    const MapKey key{base, B, H, W, C, LK, (col ? 1 : 0) | (dtype << 1) | (dev << 3)};
     {
         std::lock_guard<std::mutex> lk(g_map_mu);
         auto it = g_maps.find(key);
         if (it != g_maps.end()) { *m = it->second; return true; }
     }
-    if (!make_map(m, base, B, H, W, C, LK, col, bf16)) return false;
+    if (!make_map(m, base, B, H, W, C, LK, col, dtype)) return false;
     std::lock_guard<std::mutex> lk(g_map_mu);
     if (g_maps.size() >= kMaxCachedMaps) g_maps.clear();
     g_maps.emplace(key, *m);

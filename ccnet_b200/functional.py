@@ -10,7 +10,7 @@ import torch
 
 from . import capi
 
-_DTYPES = {torch.float32: capi.CCA_F32, torch.bfloat16: capi.CCA_BF16}
+_DTYPES = {torch.float32: capi.CCA_F32, torch.bfloat16: capi.CCA_BF16, torch.float16: capi.CCA_F16}
 _IMPL_FLAGS = {"auto": capi.CCA_FLAG_AUTO, "simt": capi.CCA_FLAG_FORCE_SIMT, "tc": capi.CCA_FLAG_FORCE_TC}
 
 
@@ -19,7 +19,7 @@ def _check_inputs(q, k, v):
         raise RuntimeError("ccnet_b200: criss-cross attention needs CUDA tensors on an H100 (sm_90) "
                            "(there is no CPU path in this package)")
     if q.dtype not in _DTYPES or k.dtype != q.dtype or v.dtype != q.dtype:
-        raise RuntimeError(f"ccnet_b200: q,k,v must share dtype float32 or bfloat16, got "
+        raise RuntimeError(f"ccnet_b200: q,k,v must share dtype float32, bfloat16 or float16, got "
                            f"{q.dtype},{k.dtype},{v.dtype}")
     if q.dim() != 4 or k.shape != q.shape or v.dim() != 4 or v.shape[0] != q.shape[0] or v.shape[2:] != q.shape[2:]:
         raise RuntimeError(f"ccnet_b200: expected q,k [B,Cq,H,W] and v [B,C,H,W], got "
@@ -28,13 +28,15 @@ def _check_inputs(q, k, v):
         raise RuntimeError("ccnet_b200: q,k,v must be on the same device")
 
 
-def _bf16_long_lines(dtype, H: int, W: int) -> bool:
-    """bf16 I/O with lines longer than one 112-pixel tile: every output element of the tensor-core kernels is then the sum of
-    up to 2*ceil(L/112) TMA reduce-adds, each rounded to bf16 in memory, in no fixed order -- measured at the 1e-2 budget
-    (profiles/r02_parity_report.jsonl).  Such calls run on the fp32 kernels (bf16 values are exact in the bf16x3 split) and the
-    result is rounded to bf16 ONCE.  CCA_B200_BF16_NATIVE=1 keeps the native bf16 kernels (the C ABI always does)."""
+def _half_long_lines(dtype, H: int, W: int) -> bool:
+    """bf16 or fp16 I/O with lines longer than one 112-pixel tile: every output element of the tensor-core kernels is then the
+    sum of up to 2*ceil(L/112) TMA reduce-adds, each rounded to the 16-bit type in memory, in no fixed order -- measured at the
+    1e-2 budget for bf16 (profiles/r02_parity_report.jsonl).  Such calls run on the fp32 kernels (bf16 and fp16 values are
+    exact in the bf16x3 split) and the result is rounded to the 16-bit type ONCE.  CCA_B200_BF16_NATIVE=1 keeps the native
+    bf16 and fp16 kernels for both types (the C ABI always does)."""
     import os
-    return dtype == torch.bfloat16 and (H > 112 or W > 112) and not os.environ.get("CCA_B200_BF16_NATIVE")
+    return (dtype in (torch.bfloat16, torch.float16) and (H > 112 or W > 112)
+            and not os.environ.get("CCA_B200_BF16_NATIVE"))
 
 
 def _stream_ptr(device) -> int:
@@ -67,9 +69,9 @@ def cca_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "
     use_tc = impl in ("auto", "tc") and lib.cca_b200_tc_supported(capi.CCA_WS_FORWARD, B, Cq, C, H, W, dt) == 1
     if impl == "tc" and not use_tc:
         raise RuntimeError(f"ccnet_b200: tensor-core kernels do not cover q{tuple(q.shape)} v{tuple(v.shape)} {q.dtype}")
-    if use_tc and _bf16_long_lines(q.dtype, H, W):
+    if use_tc and _half_long_lines(q.dtype, H, W):
         out32, lse = cca_forward(q.float(), k.float(), v.float(), impl)
-        return out32.to(torch.bfloat16), lse
+        return out32.to(q.dtype), lse
     if use_tc:
         fmt = torch.channels_last
         q, k, v = (t.contiguous(memory_format=fmt) for t in (q, k, v))
@@ -112,9 +114,9 @@ def cca_backward(dout, q, k, v, out, lse, impl: str = "auto", want_delta: bool =
     use_tc = impl in ("auto", "tc") and lib.cca_b200_tc_supported(capi.CCA_WS_BACKWARD, B, Cq, C, H, W, dt) == 1
     if impl == "tc" and not use_tc:
         raise RuntimeError(f"ccnet_b200: tensor-core kernels do not cover q{tuple(q.shape)} v{tuple(v.shape)} {q.dtype}")
-    if use_tc and _bf16_long_lines(q.dtype, H, W):
+    if use_tc and _half_long_lines(q.dtype, H, W):
         res = cca_backward(dout.float(), q.float(), k.float(), v.float(), out.float(), lse, impl, want_delta)
-        return tuple(g.to(torch.bfloat16) for g in res[:3]) + tuple(res[3:])
+        return tuple(g.to(q.dtype) for g in res[:3]) + tuple(res[3:])
     if use_tc:
         fmt = torch.channels_last
         dout, q, k, v, out = (t.contiguous(memory_format=fmt) for t in (dout, q, k, v, out))

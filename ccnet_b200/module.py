@@ -29,6 +29,7 @@ class _QKVProject(torch.autograd.Function):
         ws = [w.view(w.shape[0], C) for w in (wq, wk, wv)]
         outs = [torch.addmm(b, xm, w.t()) for w, b in zip(ws, (bq, bk, bv))]
         ctx.save_for_backward(xm, *ws)
+        ctx.gemm_dtype = outs[0].dtype                                      # fp16 / bf16 under autocast, else x's dtype
         ctx.shape = (B, H, W)
         ctx.wshapes = (wq.shape, wk.shape, wv.shape)
         return tuple(y.view(B, H, W, y.shape[1]).permute(0, 3, 1, 2) for y in outs)   # logical NCHW, channels-last strides
@@ -36,8 +37,10 @@ class _QKVProject(torch.autograd.Function):
     @staticmethod
     @torch.amp.custom_bwd(device_type="cuda")
     def backward(ctx, dq, dk, dv):
-        xm, wq, wk, wv = ctx.saved_tensors
-        dq, dk, dv = (g.to(xm.dtype) for g in (dq, dk, dv))                # autocast may hand back reduced-precision grads
+        # the backward GEMMs run in the dtype of the forward's (under autocast: the autocast dtype, as the reference's convs do);
+        # in-place addmm_ is not autocast, so every operand is brought to that dtype here (no-ops without autocast)
+        xm, wq, wk, wv = (t.to(ctx.gemm_dtype) for t in ctx.saved_tensors)
+        dq, dk, dv = (g.to(ctx.gemm_dtype) for g in (dq, dk, dv))
         B, H, W = ctx.shape
         C = xm.shape[1]
         gs = [g.permute(0, 2, 3, 1).reshape(B * H * W, g.shape[1]) for g in (dq, dk, dv)]   # views of channels-last grads

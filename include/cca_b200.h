@@ -13,7 +13,7 @@
  * Conventions
  *   - plain pointers and sizes only; no torch / C++ types.
  *   - tensors are NCHW-contiguous (default) or channels-last (CCA_FLAG_NHWC), same dtype
- *     for q,k,v,out (CCA_F32 or CCA_BF16); lse / stats / delta are always fp32 [B,H,W].
+ *     for q,k,v,out (CCA_F32, CCA_BF16 or CCA_F16); lse / stats / delta are always fp32 [B,H,W].
  *   - q,k: [B,Cq,H,W]   v,out,dout,dv: [B,C,H,W]   lse: [B,H,W].
  *   - "device" entry points take device pointers valid on the current CUDA device and a
  *     cudaStream_t (as void*); they enqueue work and return without synchronising.
@@ -45,10 +45,16 @@ extern "C" {
 
 typedef enum cca_dtype {
     CCA_F32 = 0,  /* float32 I/O, fp32 accumulate                                       */
-    CCA_BF16 = 1  /* bfloat16 I/O, fp32 accumulate, fp32 lse.  Lines longer than 112 pixels: an */
+    CCA_BF16 = 1, /* bfloat16 I/O, fp32 accumulate, fp32 lse.  Lines longer than 112 pixels: an */
                   /* output element is the sum of up to 2*ceil(L/112) bf16-rounded partial      */
                   /* results (TMA reduce-add, no fixed order): gradients at the 1e-2 budget --  */
                   /* call CCA_F32 on upcast tensors for fp32-grade accumulation (INTEGRATION.md) */
+    CCA_F16 = 2   /* float16 I/O (what torch.autocast uses by default), fp32 accumulate, fp32    */
+                  /* lse / delta; P and dS enter the f16 MMAs rounded to f16.  Both kernel      */
+                  /* families, the same shapes as CCA_BF16 (cca_b200_tc_supported(.., CCA_F16)  */
+                  /* says whether the tensor-core kernels cover a problem); long lines as for   */
+                  /* CCA_BF16 (partial results rounded to f16).  Values beyond the f16 range    */
+                  /* overflow to inf, as in any f16 computation.                                */
 } cca_dtype;
 
 typedef enum cca_status {
