@@ -47,31 +47,34 @@ struct BwdParams {
     int hints;                 // L2 eviction hints on the loads and the output stores
 };
 
-// The V / dO / O ring holds chunks of ONE 128-byte TMA box each: 32 channels for fp32 (converted in place to hi/lo planes),
-// 64 for 16-bit I/O.  Small slots buy depth: at LK = 112 fp32 the ring has 8 slots (2 2/3 chunks of V, dO, O), so chunk n + 1 lands
-// and is converted while chunk n's MMAs run.  A dV chunk has the footprint of a slot and is staged in its chunk's dO slot,
-// which goes back to the producer once the bulk copy has read it.
+// The load ring holds ONE 128-byte TMA box per slot: 32 channels for fp32 (converted in place to hi/lo planes), 64 for 16-bit
+// I/O.  Per item it carries Q's boxes, K's boxes, then the V, dO (, O) chunks.  Small slots buy depth: at LK = 112 fp32 the ring
+// has 8 slots (2 2/3 chunks of V, dO, O), so chunk n + 1 lands and is converted while chunk n's MMAs run, and the next item's
+// Q, K and first chunks land while this item runs its dS, dQ, dK epilogue.  A dV chunk has the footprint of a slot and is
+// staged in its chunk's dO slot, which goes back to the producer once the bulk copy has read it.
 template <int LK, typename E> struct BwdSmem {
     using T = Tiles<LK, E>;
     static constexpr int kCh = T::H16 ? kNC : kNC / 2;               // channels per ring slot / per chunk
     static constexpr int kRSlot = T::kTile;                         // ring slot bytes: [LK px][128 B]
-    static constexpr int off_qk = 0;                                // Q slot, K slot (held for the whole item: dQ, dK read them)
+    static constexpr int off_qk = 0;                                // Q, K of the item, moved here from the ring (dQ, dK read them)
     static constexpr int off_p = off_qk + 2 * T::kSlot;             // P / dS planes (hi block, lo block)
     // (pad: 64-row P^T operands read up to 16 planes; TMA destinations with SWIZZLE_128B must be 1024-byte aligned)
     static constexpr int off_ld = (off_p + T::kP + (16 - LK / 8) * T::kPlane + 1023) / 1024 * 1024;
     static constexpr int kTail = (128 - LK) * 128 + 256;            // over-read of the last slot by the second warpgroup
     static constexpr int kDsum = 1024;                              // float [2][128]: delta halves per pixel row
     static constexpr int kBudget = 232448;                          // 227 KB: the opt-in maximum per block on sm_90
-    // every slot also needs its full / empty barriers (8 B each); qk_full, qk_empty take the rest
-    static constexpr int kNLd = (kBudget - off_ld - kTail - kDsum - 16) / (kRSlot + 16);
+    // every slot also needs its full / empty barriers (8 B each)
+    static constexpr int kNLd = (kBudget - off_ld - kTail - kDsum) / (kRSlot + 16);
     static constexpr int off_tail = off_ld + kNLd * kRSlot;
     static constexpr int off_dsum = off_tail + kTail;
     static constexpr int off_bar = off_dsum + kDsum;
-    static constexpr int kBytes = off_bar + 8 * (2 + 2 * kNLd);
+    static constexpr int kBytes = off_bar + 8 * 2 * kNLd;
     // The ring is filled in order, so what counts is the span from the oldest slot still held to the newest one waited for.
     // While chunk n's MMAs run, the conversion of chunk n + 1 waits for chunk n + 1's V, dO, O; chunk n - 1's dO slot holds its
     // staged dV until the conversion has ended (the bulk copy is checked then), chunk n's V and dO are in the MMAs.  From
     // chunk n - 1's dO to chunk n + 1's O that is 8 slots; with fewer the producer could not load chunk n + 1: deadlock.
+    // An item's Q / K entries are moved out and released before its chunk 0 is converted, and nothing is held across items
+    // (the last dV slot goes back at the end of the item), so they add nothing to this span.
     static_assert(kNLd >= 8, "ring depth: chunk n - 1's dO (staged dV) up to chunk n + 1's O");
     // dK is staged in the P / dS planes: two (fp32) or one (16-bit) swizzled [LK px][128 B] boxes, 1024-byte aligned
     static_assert(off_p % 1024 == 0 && T::kP >= T::kSlot, "dK staging in the P / dS planes");
@@ -99,10 +102,11 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
     constexpr int kNLd = S::kNLd;
     constexpr int kCh = S::kCh;
     constexpr int KP = LK / 16;
+    constexpr int kQKBoxes = H16 ? 1 : 2;          // ring entries per Q or K operand (64 channels)
     constexpr uint32_t LOP = T::kPP * T::kPlane;   // P / dS planes: hi block -> lo block
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + S::off_bar);
-    uint64_t *qk_full = bars, *qk_empty = bars + 1, *full = bars + 2, *empty = bars + 2 + kNLd;
+    uint64_t *full = bars, *empty = bars + kNLd;
     float *dsum = reinterpret_cast<float *>(smem + S::off_dsum);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int NCH = p.C / kCh;
@@ -112,7 +116,6 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
 
     if (tid == 0) {
         // empty barriers: one arrival per use of a slot (consumer thread 0, after the barrier or bulk read that ends the use)
-        mbar_init(qk_full, 1); mbar_init(qk_empty, 1);
         for (int i = 0; i < kNLd; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
         fence_mbar_init();
         prefetch_tmap(&mqc); prefetch_tmap(&mqr); prefetch_tmap(&mkc); prefetch_tmap(&mkr); prefetch_tmap(&mvc); prefetch_tmap(&mvr);
@@ -126,31 +129,28 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
         setmaxnreg_dec<kProducerRegs>();
         if (warp == 0 && lane == 0) {
             const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
-            // boxes: 128-byte TMA boxes from channel c0 on (Q / K: the 64 channels of a fp32 slot are two boxes)
-            auto load = [&](uint8_t *dst, uint64_t *bar, const CUtensorMap *m, int c0, const Item &it, int start, bool last_use, int boxes) {
-                const int cw = it.col ? it.line : start, ch = it.col ? start : it.line;
-                if (p.hints == 1) {     // what the sample's consumers read again stays; O and the consumers' own operands stream
-                    const uint64_t pol = (is_producer(it) && !last_use) ? pol_keep : pol_stream;
-                    for (int bx = 0; bx < boxes; ++bx) tma_load_4d(dst + bx * T::kTile, m, bar, c0 + 32 * bx, cw, ch, it.b, pol);
-                } else {
-                    for (int bx = 0; bx < boxes; ++bx) tma_load_4d(dst + bx * T::kTile, m, bar, c0 + 32 * bx, cw, ch, it.b);
-                }
-            };
+            // the next ring slot <- the 128-byte TMA box from channel c0 on.  The producer waits for nothing but free slots, so it
+            // runs ahead into the next item (its Q, K and first chunks) while the consumers finish this one.
             uint32_t g = 0;
             auto ring = [&](const CUtensorMap *m, int c0, const Item &it, int start, bool last_use) {
                 const int slot = g % kNLd;
                 mbar_wait(&empty[slot], ((g / kNLd) & 1) ^ 1);
                 mbar_expect_tx(&full[slot], S::kRSlot);
-                load(smem + S::off_ld + slot * S::kRSlot, &full[slot], m, c0, it, start, last_use, 1);
+                uint8_t *dst = smem + S::off_ld + slot * S::kRSlot;
+                const int cw = it.col ? it.line : start, ch = it.col ? start : it.line;
+                if (p.hints == 1) {     // what the sample's consumers read again stays; O and the consumers' own operands stream
+                    const uint64_t pol = (is_producer(it) && !last_use) ? pol_keep : pol_stream;
+                    tma_load_4d(dst, m, &full[slot], c0, cw, ch, it.b, pol);
+                } else {
+                    tma_load_4d(dst, m, &full[slot], c0, cw, ch, it.b);
+                }
                 ++g;
             };
             for (int k = 0; k < nk; ++k) {
                 const Item it = item_of(k);
                 const bool calc = calc_delta(p, it);
-                mbar_wait(qk_empty, (k & 1) ^ 1);
-                mbar_expect_tx(qk_full, 2 * T::kSlot);
-                load(smem + S::off_qk, qk_full, it.col ? &mqc : &mqr, 0, it, it.q0, false, H16 ? 1 : 2);
-                load(smem + S::off_qk + T::kSlot, qk_full, it.col ? &mkc : &mkr, 0, it, it.k0, false, H16 ? 1 : 2);
+                for (int bx = 0; bx < kQKBoxes; ++bx) ring(it.col ? &mqc : &mqr, 32 * bx, it, it.q0, false);
+                for (int bx = 0; bx < kQKBoxes; ++bx) ring(it.col ? &mkc : &mkr, 32 * bx, it, it.k0, false);
                 for (int n = 0; n < NCH; ++n) {
                     ring(it.col ? &mvc : &mvr, n * kCh, it, it.k0, false);
                     ring(it.col ? &mdoc : &mdor, n * kCh, it, it.q0, false);
@@ -207,6 +207,7 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
         pdl_wait();                                                // prep kernel complete: counters (and the outputs) cleared
         uint32_t g = 0;
         int pending = -1;                                          // (thread 0) ring slot whose bulk copy may still be reading it
+        int unpublished = -1;                                      // (thread 0) sample of the last producer item, not yet published
         for (int k = 0; k < nk; ++k) {
             const Item it = item_of(k);
             const bool calc = calc_delta(p, it);
@@ -223,12 +224,41 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 nlse[h] = qok[h] ? -p.lse[qpix[h]] * kLog2e : 0.f;
                 self[h] = it.col ? it.q0 + r - it.k0 : -1;
             }
-            // ---------------- S = Q K^T, P = exp(S - lse) -> planes
-            mbar_wait(qk_full, k & 1);
-            if constexpr (!H16) {
-                convert_slot<LK, E>(smem + S::off_qk, t);
-                convert_slot<LK, E>(smem + S::off_qk + T::kSlot, t);
+            // ---------------- Q, K: the item's first ring entries -> the Q / K region
+            // Every thread reads its part, the consumers meet, then write: the previous item's dK MMAs (both warpgroups) and
+            // its dQ copy out of the K region (thread 0's wait_group.read at the end of that item) precede that barrier.
+            {
+                const uint8_t *src[2 * kQKBoxes];
+#pragma unroll
+                for (int i = 0; i < 2 * kQKBoxes; ++i) {
+                    const uint32_t gi = g + i;
+                    mbar_wait(&full[gi % kNLd], (gi / kNLd) & 1);
+                    src[i] = smem + S::off_ld + (gi % kNLd) * S::kRSlot;
+                }
+                if constexpr (H16) {                               // a plain copy: both sides are 1024-byte aligned, so the
+                    constexpr int kV = T::kTile / 16, kPer = (kV + kConsumers - 1) / kConsumers;     // swizzle carries over
+                    uint4 v[2][kPer];
+#pragma unroll
+                    for (int i = 0; i < 2; ++i)
+#pragma unroll
+                        for (int j = 0; j < kPer; ++j)
+                            if (t + kConsumers * j < kV) v[i][j] = reinterpret_cast<const uint4 *>(src[i])[t + kConsumers * j];
+                    consumers_sync();
+#pragma unroll
+                    for (int i = 0; i < 2; ++i)
+#pragma unroll
+                        for (int j = 0; j < kPer; ++j)
+                            if (t + kConsumers * j < kV) reinterpret_cast<uint4 *>(smem + S::off_qk + i * T::kSlot)[t + kConsumers * j] = v[i][j];
+                    fence_proxy_async();
+                    consumers_sync();
+                } else {
+                    convert_slot<LK, E, 4>(smem + S::off_qk, t, nullptr, src);      // Q0 Q1 K0 K1 -> hi/lo planes of Q, K
+                }
+                if (t == 0)
+                    for (int i = 0; i < 2 * kQKBoxes; ++i) mbar_arrive(&empty[(g + i) % kNLd]);
+                g += 2 * kQKBoxes;
             }
+            // ---------------- S = Q K^T, P = exp(S - lse) -> planes
             {
                 float acc[LK / 2];
                 wg_fence();
@@ -242,7 +272,18 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 wg_commit();
                 wg_wait<0>();
                 wg_acc_fence<LK / 2>(acc);
-                if (t == 0) bulk_wait_read<0>();                   // the previous item's dK copy has read the P / dS planes
+                if (t == 0) {                                      // the previous item's dK copy has read the P / dS planes
+                    // Deferred publish of the previous item (a producer): its stores have long completed by now.  It must come
+                    // before this item's first counter wait (cdone before chunk 0's dV add, ddone before dS): in the lagged
+                    // order an item can consume the very sample the CTA's previous item produced, and would wait for itself.
+                    if (unpublished >= 0) {
+                        bulk_wait<0>();
+                        publish_count(p.cdone + unpublished);
+                        unpublished = -1;
+                    } else {
+                        bulk_wait_read<0>();
+                    }
+                }
                 consumers_sync();
 #pragma unroll
                 for (int j = 0; j < LK / 8; ++j)
@@ -268,37 +309,77 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
             }
             fence_proxy_async();
             consumers_sync();
-            if (!prod && p.out_mode == 1) wait_count(p.cdone + it.b, (unsigned)p.sp.seg0);   // producers of the sample have stored
-            // the counter's acquire (or the prep kernel's clear, tiled lines) before this item's reduce-adds
-            if (!prod && t == 0) fence_proxy_async_global();
             // ---------------- per chunk: dP += dO V^T, dV = P^T dO
             // Pipelined over the chunks: chunk n's MMAs run while chunk n + 1 is converted (and its delta dot accumulated); then
-            // chunk n is waited for, its V slot released, its dV staged in its dO slot and stored by one thread with TMA, and
-            // chunk n + 1 is issued.  The dO slot goes back to the producer at the end of the next conversion, when the copy
-            // has long read it.  One group in flight at a time: with a second one (wg_wait<1> and a second dV accumulator)
-            // ptxas treats the groups chained through dP as one pipeline stage, sees the other dV accumulator read inside it and
-            // serialises every wgmma of the kernel (C7514); at LK = 112 fp32 the second accumulator also spills.
+            // chunk n is waited for and its V slot released, chunk n + 1's dP is issued, chunk n's dV is staged in its dO slot
+            // and stored by one thread with TMA while that dP runs, and chunk n + 1's dV is issued.  The dO slot goes back to
+            // the producer at the end of the next conversion, when the copy has long read it.  dP and dV are two commit groups
+            // so that the staging (which reads the dV accumulator) overlaps the dP group; the one wait per chunk waits for
+            // both.  A second dV accumulator (so that a dV group could stay in flight across the wait) makes ptxas treat the
+            // groups chained through dP as one pipeline stage, see the other dV accumulator read inside it and serialise every
+            // wgmma of the kernel (C7514); at LK = 112 fp32 it also spills.
             float dp[LK / 2];
             float o[kCh / 2];                                      // dV of the chunk
             float dacc = 0.f;
             const uint32_t per = calc ? 3 : 2;                     // ring slots per chunk: V, dO (, O)
             auto rslot = [&](uint32_t gi) { return gi % kNLd; };
+            // fp32: chunk n's V and dO boxes -> hi/lo planes in place, in one pass (the layout of convert_slot with one box each).
+            // Every thread reads its part of both (and accumulates the delta dot with O), the consumers meet once, then write.
+            // There is no closing barrier: the barrier that follows the previous chunk's wait (or the one after chunk 0's
+            // conversion) orders these writes before this chunk's MMAs are issued.
             auto convert_chunk = [&](int n) {
                 const uint32_t gv = g + per * n, gd = gv + 1, go = gv + 2;
                 mbar_wait(&full[rslot(gv)], (gv / kNLd) & 1);
                 mbar_wait(&full[rslot(gd)], (gd / kNLd) & 1);
                 if (calc) mbar_wait(&full[rslot(go)], (go / kNLd) & 1);
                 uint8_t *vs = smem + S::off_ld + rslot(gv) * S::kRSlot, *ds = smem + S::off_ld + rslot(gd) * S::kRSlot;
-                if constexpr (!H16) convert_slot<LK, E, 1>(vs, t);
-                if (calc) {
-                    dacc += convert_slot<LK, E, 1>(ds, t, smem + S::off_ld + rslot(go) * S::kRSlot);
-                    if constexpr (H16) consumers_sync();            // (fp32: the conversion ends on a consumer barrier)
-                    if (t == 0) mbar_arrive(&empty[rslot(go)]);
-                } else if constexpr (!H16) {
-                    convert_slot<LK, E, 1>(ds, t);
+                const uint8_t *os = smem + S::off_ld + rslot(go) * S::kRSlot;
+                if constexpr (H16) {
+                    if (calc) {
+                        dacc += convert_slot<LK, E, 1>(ds, t, os);
+                        consumers_sync();
+                        if (t == 0) mbar_arrive(&empty[rslot(go)]);
+                    }
+                } else {
+                    const int r = t & 127, hq = t >> 7;
+                    const int rr = r < LK ? r : LK - 1, sw = rr & 7;
+                    float4 raw[2][4];
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        raw[0][j] = *reinterpret_cast<const float4 *>(vs + rr * 128 + (((hq * 4 + j) ^ sw) * 16));
+                        raw[1][j] = *reinterpret_cast<const float4 *>(ds + rr * 128 + (((hq * 4 + j) ^ sw) * 16));
+                    }
+                    if (calc) {
+                        float acc = 0.f;
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) {
+                            const float4 o = *reinterpret_cast<const float4 *>(os + rr * 128 + (((hq * 4 + j) ^ sw) * 16));
+                            const float4 x = raw[1][j];
+                            acc += x.x * o.x + x.y * o.y + x.z * o.z + x.w * o.w;
+                        }
+                        dacc += r < LK ? acc : 0.f;
+                    }
+                    named_bar_sync(kBarConvert, kConsumers);
+                    if (calc && t == 0) mbar_arrive(&empty[rslot(go)]);
+                    if (r < LK) {
+#pragma unroll
+                        for (int b = 0; b < 2; ++b) {
+                            uint8_t *d = (b ? ds : vs) + r * 16 + hq * 2 * T::kPStride;
+#pragma unroll
+                            for (int j = 0; j < 2; ++j) {
+                                const float4 a = raw[b][2 * j], c = raw[b][2 * j + 1];
+                                const float v[8] = {a.x, a.y, a.z, a.w, c.x, c.y, c.z, c.w};
+                                uint4 hi, lo;
+                                split8(v, hi, lo);
+                                *reinterpret_cast<uint4 *>(d + j * T::kPStride) = hi;
+                                *reinterpret_cast<uint4 *>(d + j * T::kPStride + T::kLoOff) = lo;
+                            }
+                        }
+                    }
+                    fence_proxy_async();
                 }
             };
-            auto issue = [&](int n) {
+            auto issue_dp = [&](int n) {
                 const uint32_t gv = g + per * n, gd = gv + 1;
                 const uint32_t vb = ld_base + rslot(gv) * S::kRSlot, db = ld_base + rslot(gd) * S::kRSlot;
                 wg_fence();
@@ -310,6 +391,11 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                         wgmma_ss<LK, F16>(dp, desc_kmaj<LK, E>(db, 64 * wg, ks, true), desc_kmaj<LK, E>(vb, 0, ks, false), 1, 0, 0);
                     }
                 }
+                wg_commit();
+            };
+            auto issue_dv = [&](int n) {
+                const uint32_t db = ld_base + rslot(g + per * n + 1) * S::kRSlot;
+                wg_fence();
 #pragma unroll
                 for (int ks = 0; ks < KP; ++ks) {
                     const uint32_t pa = pb + 8 * wg * T::kPlane + ks * 256;      // P^T: rows = key pixels [64 wg, +64), k = query rows
@@ -330,28 +416,32 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                     pending = -1;
                 }
             };
-            auto retire = [&](int n) {                             // chunk n's MMAs are complete in this warpgroup
-                const uint32_t gv = g + per * n, gd = gv + 1;
+            convert_chunk(0);
+            if constexpr (!H16) consumers_sync();
+            issue_dp(0);
+            issue_dv(0);
+            for (int n = 0; n < NCH; ++n) {
+                if (n + 1 < NCH) convert_chunk(n + 1);
+                release();
+                wg_wait<0>();                                      // chunk n's MMAs are complete in this warpgroup
                 wg_acc_fence<kCh / 2>(o);
+                if (n == 0 && !prod) {                             // before this item's first reduce-add, no group in flight:
+                    if (p.out_mode == 1) wait_count(p.cdone + it.b, (unsigned)p.sp.seg0);   // producers of the sample have stored
+                    // the counter's acquire (or the prep kernel's clear, tiled lines) before the reduce-adds
+                    if (t == 0) fence_proxy_async_global();
+                }
                 consumers_sync();                                  // ... and in the other: V and dO are free
-                if (t == 0) mbar_arrive(&empty[rslot(gv)]);
-                uint8_t *ds = smem + S::off_ld + rslot(gd) * S::kRSlot;
+                if (t == 0) mbar_arrive(&empty[rslot(g + per * n)]);
+                if (n + 1 < NCH) issue_dp(n + 1);
+                uint8_t *ds = smem + S::off_ld + rslot(g + per * n + 1) * S::kRSlot;
                 stage(o, kCh, ds);
                 fence_proxy_async();
                 consumers_sync();
                 if (t == 0) {
                     put(it.col ? &mdvc : &mdvr, ds, 1, n * kCh, it.k0, it, prod);
-                    pending = (int)rslot(gd);
+                    pending = (int)rslot(g + per * n + 1);
                 }
-            };
-            convert_chunk(0);
-            issue(0);
-            for (int n = 0; n < NCH; ++n) {
-                if (n + 1 < NCH) convert_chunk(n + 1);
-                release();
-                wg_wait<0>();
-                retire(n);
-                if (n + 1 < NCH) issue(n + 1);
+                if (n + 1 < NCH) issue_dv(n + 1);
             }
             wg_wait<0>();                                          // (nothing is pending; ptxas cannot tell which step ran last)
             wg_acc_fence<LK / 2>(dp);
@@ -451,15 +541,14 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                     bulk_wait_read<1>();                           // the last dV copy and the dQ copy have read their slots
                     if (pending >= 0) mbar_arrive(&empty[pending]);
                     pending = -1;
-                    mbar_arrive(qk_empty);
-                    if (prod) {                                    // publish: all stores of this item are complete
-                        bulk_wait<0>();
-                        publish_count(p.cdone + it.b);
-                    }
+                    if (prod) unpublished = it.b;                  // published once its stores are complete, in the next item
                 }
             }
         }
-        if (t == 0) bulk_wait<0>();                                // shared memory must outlive the last bulk reads
+        if (t == 0) {
+            bulk_wait<0>();                                        // shared memory must outlive the last bulk reads
+            if (unpublished >= 0) publish_count(p.cdone + unpublished);
+        }
     }
 }
 

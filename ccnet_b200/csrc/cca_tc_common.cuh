@@ -103,9 +103,11 @@ __device__ __forceinline__ void consumers_sync() { named_bar_sync(kBarConsumers,
 // t & 127, 16-channel half t >> 7 of each box).  Every thread reads its NB x 64 B, the consumers meet, then overwrite; the
 // planes are made visible to wgmma (async proxy) and every consumer has passed the closing barrier on return.
 // With `dot` (the O tile of the same pixels, same layout): returns this thread's part of sum_c slot[r][c] * dot[r][c].
+// With `src` (fp32): box bx is read from src[bx] instead, and `slot` is only the destination of the NB converted boxes (NB = 4:
+// two [LK px][64 ch] slots back to back).
 // 16-bit slots (one 64-channel box) need no conversion; only the dot product is computed.
 template <int LK, typename E, int NB = 2>
-__device__ __forceinline__ float convert_slot(uint8_t *slot, int t, const uint8_t *dot = nullptr)
+__device__ __forceinline__ float convert_slot(uint8_t *slot, int t, const uint8_t *dot = nullptr, const uint8_t *const *src = nullptr)
 {
     using T = Tiles<LK, E>;
     constexpr bool H16 = T::H16, F16 = kF16<E>;
@@ -126,13 +128,13 @@ __device__ __forceinline__ float convert_slot(uint8_t *slot, int t, const uint8_
         }
         return r < LK ? acc : 0.f;
     } else {
-        static_assert(NB == 1 || NB == 2, "boxes per slot");
+        static_assert(NB == 1 || NB == 2 || NB == 4, "boxes per slot");
         float4 raw[4 * NB];
 #pragma unroll
         for (int bx = 0; bx < NB; ++bx)
 #pragma unroll
             for (int j = 0; j < 4; ++j)
-                raw[4 * bx + j] = *reinterpret_cast<const float4 *>(slot + bx * T::kTile + rr * 128 + (((hq * 4 + j) ^ sw) * 16));
+                raw[4 * bx + j] = *reinterpret_cast<const float4 *>((src ? src[bx] : slot + bx * T::kTile) + rr * 128 + (((hq * 4 + j) ^ sw) * 16));
         if (dot) {
 #pragma unroll
             for (int bx = 0; bx < NB; ++bx)

@@ -1,4 +1,6 @@
-"""Discrete model of the mbarrier protocol of tools/experiments/cca_tc_fwdt.cu (roles as coroutines, random interleavings).
+"""Discrete models of mbarrier protocols (roles as coroutines, random interleavings): the channel-major forward kernel
+explored for an earlier tensor-core design (tools/experiments/cca_tc_fwdt.cu, not adopted), and the backward kernel's load
+ring, bulk copies and per-sample counters (ccnet_b200/csrc/cca_tc_bwd.cuh; build_bwd / run_bwd).
 
 Not a performance model: it only answers "can this hand-shake deadlock, and does every arrive / wait hit the barrier
 phase it was meant for?" before GPU minutes are spent on it.  Every wait and arrive carries the use index the code
@@ -229,6 +231,204 @@ def run(NCH, kNLd, nk, seed):
             idle += 1
         if idle > 20000:
             raise AssertionError(f"deadlock: still running {sorted(live)}")
+    return True
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# Backward kernel (ccnet_b200/csrc/cca_tc_bwd.cuh): the load ring, the bulk copies and the per-sample counters, over several CTAs.
+#
+# Per CTA two roles: the producer lane (it waits only on ring slots) and the consumers (the 256 threads move together through
+# their barriers, so one agent; thread 0's arrivals are its events).  A third agent per CTA plays the bulk-copy engine: it
+# reads the committed groups in order and completes their writes some time later.  Items are those of cca_items.cuh with one
+# tile per line (column items store and publish, row items add after the counter), in the real item orders.
+
+def bwd_items(B, H, W, lag):
+    """[(b, producer)] in the order of decode_item / decode_item_lagged (one tile per line: seg1 is empty)."""
+    seg0, per_sample = W, W + H
+    def in_sample(b, j):
+        return (b, j < seg0)
+    out = []
+    for idx in range(B * per_sample):
+        if not lag:
+            out.append(in_sample(idx // per_sample, idx % per_sample))
+            continue
+        if idx < seg0:
+            out.append(in_sample(0, idx))
+            continue
+        x = idx - seg0
+        grp, rem = divmod(x, per_sample)
+        if grp < B - 1:
+            out.append(in_sample(grp + 1, rem) if rem < seg0 else in_sample(grp, rem))
+        else:
+            out.append(in_sample(B - 1, seg0 + rem))
+    return out, seg0
+
+
+def build_bwd(kNLd, NCH, B, H, W, ncta, lag, nqk=4, publish="before_waits"):
+    """nqk: ring entries of an item's Q and K (4 in fp32, 2 for 16-bit I/O).  publish: where a producer item's count is
+    published -- "before_waits" (the kernel: in the next item, after S, before its first counter wait) or "after_wait" (after
+    the next item's first counter wait: must deadlock when a CTA consumes the sample it just produced)."""
+    items, seg0 = bwd_items(B, H, W, lag)
+    cdone, ddone = [0] * B, [0] * B
+    agents = {}
+
+    def count_wait(cnt, b):
+        while cnt[b] < seg0:
+            yield
+
+    def bump(cnt, b):
+        PROGRESS[0] += 1
+        cnt[b] += 1
+
+    for c in range(ncta):
+        mine = items[c::ncta]
+        full = [Bar(f"c{c}.full{i}", 1) for i in range(kNLd)]
+        empty = [Bar(f"c{c}.empty{i}", 1) for i in range(kNLd)]
+        bulk = {"groups": [], "read": 0, "written": 0}     # committed groups (kind), how many read / written so far
+        region = {"dq_group": -1}                           # the group of the last dQ copy out of the K region
+
+        def producer(mine=mine, full=full, empty=empty):
+            g = 0
+            for b, prod in mine:
+                for _ in range(nqk + (3 if prod else 2) * NCH):   # Q, K boxes; per chunk V, dO (, O: delta producers)
+                    slot = g % kNLd
+                    yield from wait(empty[slot], ((g // kNLd) & 1) ^ 1, g // kNLd)
+                    yield                                          # (the TMA lands some time later)
+                    full[slot].arrive(use=g // kNLd)
+                    g += 1
+
+        def engine(bulk=bulk, rng=random.Random(c)):
+            while not bulk.get("done"):                      # reads in commit order; a group's writes complete after its read
+                yield
+                can_read, can_write = bulk["read"] < len(bulk["groups"]), bulk["written"] < bulk["read"]
+                if can_read and (not can_write or rng.random() < 0.5):
+                    bulk["read"] += 1
+                    PROGRESS[0] += 1
+                elif can_write:
+                    bulk["written"] += 1
+                    PROGRESS[0] += 1
+
+        def consumer(mine=mine, full=full, empty=empty, bulk=bulk, region=region):
+            g = 0
+            pending = -1
+            unpublished = -1
+
+            def commit(kind):
+                bulk["groups"].append(kind)
+                return len(bulk["groups"]) - 1
+
+            def wait_read(n):                                    # cp.async.bulk.wait_group.read n
+                while len(bulk["groups"]) - bulk["read"] > n:
+                    yield
+
+            def wait_written():                                  # cp.async.bulk.wait_group 0
+                while bulk["written"] < len(bulk["groups"]):
+                    yield
+
+            def wfull(gi):
+                yield from wait(full[gi % kNLd], (gi // kNLd) & 1, gi // kNLd + 1)
+
+            def publish_if_due():
+                nonlocal unpublished
+                if unpublished >= 0:
+                    yield from wait_written()
+                    bump(cdone, unpublished)
+                    unpublished = -1
+
+            for b, prod in mine:
+                calc = prod                                      # delta mode 1: the column items of the first key block
+                per = 3 if calc else 2
+                # Q, K entries -> the Q / K region (after the barrier that follows the previous item's dQ wait_group.read)
+                for i in range(nqk):
+                    yield from wfull(g + i)
+                if region["dq_group"] >= 0 and bulk["read"] <= region["dq_group"]:
+                    raise AssertionError("Q / K region written while the previous dQ copy may still read it")
+                yield
+                for i in range(nqk):
+                    empty[(g + i) % kNLd].arrive(use=(g + i) // kNLd)
+                g += nqk
+                # S; then the deferred publish (or the wait for the dK copy's read of the P planes)
+                yield
+                if publish == "before_waits":
+                    yield from publish_if_due()
+                yield from wait_read(0)
+
+                def convert(n):
+                    gv = g + per * n
+                    yield from wfull(gv)
+                    yield from wfull(gv + 1)
+                    if calc:
+                        yield from wfull(gv + 2)
+                        yield
+                        empty[(gv + 2) % kNLd].arrive(use=(gv + 2) // kNLd)
+
+                yield from convert(0)
+                for n in range(NCH):
+                    if n + 1 < NCH:
+                        yield from convert(n + 1)
+                    if pending >= 0:                             # release(): the previous dV copy has read its dO slot
+                        yield from wait_read(0)
+                        empty[pending % kNLd].arrive(use=pending // kNLd)
+                        pending = -1
+                    yield                                        # wg_wait<0>
+                    if n == 0 and not prod:
+                        yield from count_wait(cdone, b)
+                        if publish == "after_wait":
+                            yield from publish_if_due()
+                    gv = g + per * n
+                    empty[gv % kNLd].arrive(use=gv // kNLd)      # V free
+                    yield                                        # dP(n + 1) issued, dV(n) staged in the dO slot
+                    commit("dv")
+                    pending = gv + 1
+                g += per * NCH
+                if calc:
+                    bump(ddone, b)
+                else:
+                    yield from count_wait(ddone, b)
+                    if publish == "after_wait":
+                        yield from publish_if_due()
+                yield                                            # dS, dQ MMAs
+                region["dq_group"] = commit("dq")
+                yield                                            # dK MMAs
+                commit("dk")
+                yield from wait_read(1)
+                if pending >= 0:
+                    empty[pending % kNLd].arrive(use=pending // kNLd)
+                    pending = -1
+                if prod:
+                    unpublished = b
+            yield from wait_written()
+            yield from publish_if_due()
+            bulk["done"] = True
+
+        agents[f"prod{c}"] = producer()
+        agents[f"cons{c}"] = consumer()
+        agents[f"bulk{c}"] = engine()
+    return agents, cdone, ddone, seg0
+
+
+def run_bwd(kNLd, NCH, B, H, W, ncta, lag, seed, nqk=4, publish="before_waits"):
+    rng = random.Random(seed)
+    agents, cdone, ddone, seg0 = build_bwd(kNLd, NCH, B, H, W, ncta, lag, nqk, publish)
+    live = dict(agents)
+    names = list(live)
+    weights = {n: rng.choice((1, 1, 1, 5, 25)) for n in names}
+    idle, last = 0, PROGRESS[0]
+    while live:
+        name = rng.choices(names, [weights[n] for n in names])[0]
+        try:
+            next(live[name])
+        except StopIteration:
+            del live[name]
+            names.remove(name)
+        if PROGRESS[0] != last:
+            last, idle = PROGRESS[0], 0
+        else:
+            idle += 1
+        if idle > 20000:
+            raise AssertionError(f"deadlock: still running {sorted(live)}")
+    if cdone != [seg0] * B or ddone != [seg0] * B:
+        raise AssertionError(f"counters {cdone} {ddone}, expected {seg0} each")
     return True
 
 
