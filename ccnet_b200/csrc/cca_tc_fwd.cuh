@@ -157,26 +157,22 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
         for (int k = 0; k < nk; ++k) {
             const Item it = item_of(k);
             const bool prod = is_producer(it);
-            // ---- final lse2 of rows rbase (h = 0), rbase + 8 (h = 1); independent of S, so loaded before S is waited for
-            float nlse[2];
+            // ---- partial lse planes of rows rbase (h = 0), rbase + 8 (h = 1): the first kPre are loaded here, all at once, and
+            // only used once S is in flight, so their L2 latency overlaps the Q / K wait, the conversion and S
+            constexpr int kPre = 4;                                // (one tile per line: 2 planes)
+            float pv[2][kPre];
+            long pix[2];
             int self[2];
             bool rok[2];
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int r = rbase + 8 * h;
                 rok[h] = r < it.lq;
-                const long pix = item_pixel(p.sp, it, rok[h] ? r : 0);
+                pix[h] = item_pixel(p.sp, it, rok[h] ? r : 0);
                 self[h] = it.col ? it.q0 + r - it.k0 : -1;
-                float lse2 = 0.f;
-                if (rok[h]) {
-                    float m = -INFINITY;
-                    for (int i = 0; i < p.sp.nparts; ++i) m = fmaxf(m, __ldcg(p.parts + (long)i * p.npix + pix));
-                    float sum = 0.f;
-                    for (int i = 0; i < p.sp.nparts; ++i) sum += exp2f(__ldcg(p.parts + (long)i * p.npix + pix) - m);
-                    lse2 = m + log2f(sum);
-                    if (!it.col && it.ik == 0 && (lane & 3) == 0) p.lse[pix] = lse2 * kLn2;
-                }
-                nlse[h] = -lse2;
+#pragma unroll
+                for (int i = 0; i < kPre; ++i)
+                    pv[h][i] = rok[h] && i < p.sp.nparts ? __ldcg(p.parts + (long)i * p.npix + pix[h]) : 0.f;
             }
             // ---- S = Q K^T
             mbar_wait(qk_full, k & 1);
@@ -194,6 +190,27 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 }
             }
             wg_commit();
+            // ---- final lse2 of the two rows while S runs (planes past kPre, if any, are read here)
+            float nlse[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float lse2 = 0.f;
+                if (rok[h]) {
+                    float m = -INFINITY;
+#pragma unroll
+                    for (int i = 0; i < kPre; ++i)
+                        if (i < p.sp.nparts) m = fmaxf(m, pv[h][i]);
+                    for (int i = kPre; i < p.sp.nparts; ++i) m = fmaxf(m, __ldcg(p.parts + (long)i * p.npix + pix[h]));
+                    float sum = 0.f;
+#pragma unroll
+                    for (int i = 0; i < kPre; ++i)
+                        if (i < p.sp.nparts) sum += exp2f(pv[h][i] - m);
+                    for (int i = kPre; i < p.sp.nparts; ++i) sum += exp2f(__ldcg(p.parts + (long)i * p.npix + pix[h]) - m);
+                    lse2 = m + log2f(sum);
+                    if (!it.col && it.ik == 0 && (lane & 3) == 0) p.lse[pix[h]] = lse2 * kLn2;
+                }
+                nlse[h] = -lse2;
+            }
             wg_wait<0>();
             wg_acc_fence<LK / 2>(acc);
             mbar_arrive(qk_empty);
