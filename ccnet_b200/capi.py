@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("CCA_B200_LIB") or os.path.join(_HERE, "lib", "libcca_b200.so")   # (override: another build flavour)
 
 CCA_F32, CCA_BF16, CCA_F16 = 0, 1, 2
-CCA_FLAG_AUTO, CCA_FLAG_FORCE_SIMT, CCA_FLAG_FORCE_TC, CCA_FLAG_NHWC = 0, 1, 2, 4
+CCA_FLAG_AUTO, CCA_FLAG_FORCE_SIMT, CCA_FLAG_FORCE_TC, CCA_FLAG_NHWC, CCA_FLAG_DETERMINISTIC = 0, 1, 2, 4, 8
 CCA_WS_FORWARD, CCA_WS_BACKWARD = 0, 1
 
 # every symbol include/cca_b200.h declares: name -> (restype, argtypes)
@@ -27,13 +27,17 @@ SYMBOLS = {
     "cca_b200_tc_supported": (_i, [_i] * 7),
     "cca_b200_item_space": (None, [_i] * 3 + [ctypes.POINTER(_i)]),
     "cca_b200_decode_item": (None, [_i] * 5 + [ctypes.POINTER(_i)]),
+    "cca_b200_item_planes": (None, [_i] * 5 + [ctypes.POINTER(_i)]),
     "cca_b200_workspace_bytes": (_sz, [_i] * 7),
+    "cca_b200_workspace_bytes_ex": (_sz, [_i] * 7 + [_u]),
     "cca_b200_qkv_supported": (_i, [_i, _i]),
     "cca_b200_qkv_workspace_bytes": (_sz, [_i, _i]),
     "cca_b200_qkv_project": (_i, [_vp] * 11 + [_sz, ctypes.c_longlong, _i, _i, _vp]),
     "cca_b200_qkv_project_dgrad": (_i, [_vp] * 9 + [_sz, ctypes.c_longlong, _i, _i, _i, _vp]),
     "cca_b200_qkv_wgrad_supported": (_i, [_i, _i]),
     "cca_b200_qkv_project_wgrad": (_i, [_vp] * 9 + [ctypes.c_longlong, _i, _i, _vp]),
+    "cca_b200_qkv_wgrad_workspace_bytes": (_sz, [_i, _i]),
+    "cca_b200_qkv_project_wgrad_ex": (_i, [_vp] * 9 + [ctypes.c_longlong, _i, _i, _vp, _sz, _u, _vp]),
     "cca_b200_forward": (_i, [_vp] * 6 + [_sz] + [_i] * 6 + [_u, _vp]),
     "cca_b200_backward": (_i, [_vp] * 10 + [_sz] + [_i] * 6 + [_u, _vp]),
     "cca_b200_forward_host": (_i, [_vp] * 5 + [_i] * 6 + [_u]),

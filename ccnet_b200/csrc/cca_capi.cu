@@ -34,6 +34,8 @@ int check_dims(int B, int Cq, int C, int H, int W, int dtype)
     return CCA_OK;
 }
 size_t esize(int dtype) { return dtype == CCA_F32 ? 4 : 2; }    // (CCA_BF16, CCA_F16: 2)
+constexpr const char *kDetHalfMsg =
+    "CCA_FLAG_DETERMINISTIC with 16-bit I/O on lines longer than 112 pixels: call CCA_F32 on upcast tensors%s%s";
 }  // namespace
 
 void count_launch(int n) { g_launches.fetch_add((unsigned long long)n, std::memory_order_relaxed); }
@@ -145,6 +147,18 @@ int cca_b200_tc_supported(int which, int B, int Cq, int C, int H, int W, int dty
     return (which == CCA_WS_BACKWARD ? tc_backward_supported(d, dtype) : tc_forward_supported(d, dtype)) ? 1 : 0;
 }
 
+// CCA_FLAG_DETERMINISTIC on a tiled fp32 channels-last problem the tensor-core kernels cover: the partial planes follow the
+// tensor-core workspace (tc_forward / tc_backward)
+size_t cca_b200_workspace_bytes_ex(int which, int B, int Cq, int C, int H, int W, int dtype, unsigned flags)
+{
+    const size_t base = cca_b200_workspace_bytes(which, B, Cq, C, H, W, dtype);
+    if (!base || !(flags & CCA_FLAG_DETERMINISTIC) || !(flags & CCA_FLAG_NHWC) || dtype != CCA_F32) return base;
+    const Dims d{B, Cq, C, H, W};
+    if (!tc::shape_fits(d, dtype)) return base;
+    const size_t need = (which == CCA_WS_FORWARD ? tc_forward_workspace(d) : tc_backward_workspace(d)) + tc_planes_bytes(which, d);
+    return need > base ? need : base;
+}
+
 size_t cca_b200_workspace_bytes(int which, int B, int Cq, int C, int H, int W, int dtype)
 {
     (void)dtype;
@@ -172,13 +186,20 @@ void cca_b200_decode_item(int B, int H, int W, int index, int lagged, int *out10
     out10[5] = it.q0; out10[6] = it.lq; out10[7] = it.k0; out10[8] = it.lk; out10[9] = it.j;
 }
 
+void cca_b200_item_planes(int B, int H, int W, int index, int lagged, int *out2)
+{
+    const tc::ItemSpace s = tc::make_space(B, H, W);
+    const tc::Item it = tc::decode_item_order(s, index, lagged);
+    out2[0] = tc::part_index(s, it); out2[1] = tc::qtile_part_index(s, it);
+}
+
 int cca_b200_forward(const void *q, const void *k, const void *v, void *out, float *lse, void *ws, size_t ws_bytes,
                      int B, int Cq, int C, int H, int W, int dtype, unsigned flags, void *stream)
 {
     int rc = check_dims(B, Cq, C, H, W, dtype);
     if (rc) return rc;
     if (!q || !k || !v || !out || !lse || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
-    if (ws_bytes < cca_b200_workspace_bytes(CCA_WS_FORWARD, B, Cq, C, H, W, dtype))
+    if (ws_bytes < cca_b200_workspace_bytes_ex(CCA_WS_FORWARD, B, Cq, C, H, W, dtype, flags))
         return fail(CCA_ERR_WORKSPACE, "forward workspace too small%s%s");
     if ((flags & CCA_FLAG_FORCE_SIMT) && (flags & CCA_FLAG_FORCE_TC))
         return fail(CCA_ERR_INVALID, "FORCE_SIMT and FORCE_TC are exclusive%s%s");
@@ -197,7 +218,9 @@ int cca_b200_forward(const void *q, const void *k, const void *v, void *out, flo
         if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
              reinterpret_cast<uintptr_t>(out)) & 15)
             return fail(CCA_ERR_INVALID, "tensor-core path needs 16-byte aligned tensors%s%s");
-        e = tc_forward(q, k, v, out, lse, ws, d, dtype, st, &why);
+        const bool det = (flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d);
+        if (det && dtype != CCA_F32) return fail(CCA_ERR_UNSUPPORTED, kDetHalfMsg);
+        e = tc_forward(q, k, v, out, lse, ws, d, dtype, st, &why, det);
         if (e != cudaSuccess) return cuda_fail(e, why && *why ? why : "tc_forward");
         return CCA_OK;
     }
@@ -215,7 +238,7 @@ int cca_b200_backward(const void *dout, const void *q, const void *k, const void
     if (rc) return rc;
     if (!dout || !q || !k || !v || !out || !lse || !dq || !dk || !dv || !ws)
         return fail(CCA_ERR_INVALID, "null pointer%s%s");
-    if (ws_bytes < cca_b200_workspace_bytes(CCA_WS_BACKWARD, B, Cq, C, H, W, dtype))
+    if (ws_bytes < cca_b200_workspace_bytes_ex(CCA_WS_BACKWARD, B, Cq, C, H, W, dtype, flags))
         return fail(CCA_ERR_WORKSPACE, "backward workspace too small%s%s");
     if ((flags & CCA_FLAG_FORCE_SIMT) && (flags & CCA_FLAG_FORCE_TC))
         return fail(CCA_ERR_INVALID, "FORCE_SIMT and FORCE_TC are exclusive%s%s");
@@ -233,8 +256,10 @@ int cca_b200_backward(const void *dout, const void *q, const void *k, const void
              reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(dq) |
              reinterpret_cast<uintptr_t>(dk) | reinterpret_cast<uintptr_t>(dv)) & 15)
             return fail(CCA_ERR_INVALID, "tensor-core path needs 16-byte aligned tensors%s%s");
+        const bool det = (flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d);
+        if (det && dtype != CCA_F32) return fail(CCA_ERR_UNSUPPORTED, kDetHalfMsg);
         cudaError_t e = tc_backward(dout, q, k, v, out, lse, dq, dk, dv, ws, d, dtype,
-                                    reinterpret_cast<cudaStream_t>(stream), &why);
+                                    reinterpret_cast<cudaStream_t>(stream), &why, det);
         if (e != cudaSuccess) return cuda_fail(e, why && *why ? why : "tc_backward");
         return CCA_OK;
     }
@@ -312,6 +337,31 @@ int cca_b200_qkv_project_wgrad(const float *x, const float *dq, const float *dk,
     if (e != cudaSuccess) return cuda_fail(e, why && *why ? why : "qkv_project_wgrad");
     return CCA_OK;
 }
+size_t cca_b200_qkv_wgrad_workspace_bytes(int C, int Cq)
+{
+    return C > 0 && Cq > 0 && qkv_wgrad_supported(C, Cq) ? qkv_wgrad_workspace(C, Cq) : 0;
+}
+int cca_b200_qkv_project_wgrad_ex(const float *x, const float *dq, const float *dk, const float *dv, const float *scale, float *dwq,
+                                  float *dwk, float *dwv, float *db, long long pixels, int C, int Cq, void *ws, size_t ws_bytes,
+                                  unsigned flags, void *stream)
+{
+    if (!(flags & CCA_FLAG_DETERMINISTIC))
+        return cca_b200_qkv_project_wgrad(x, dq, dk, dv, scale, dwq, dwk, dwv, db, pixels, C, Cq, stream);
+    if (!x || !dq || !dk || !dv || !dwq || !dwk || !dwv || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
+    if (pixels <= 0 || pixels >= (1ll << 31) || C <= 0 || Cq <= 0) return fail(CCA_ERR_INVALID, "bad dimension%s%s");
+    int rc = check_device();
+    if (rc) return rc;
+    if (!qkv_wgrad_supported(C, Cq)) return fail(CCA_ERR_UNSUPPORTED, "weight-gradient GEMM needs C %% 256 == 0 and Cq %% 64 == 0%s%s");
+    if (ws_bytes < qkv_wgrad_workspace(C, Cq)) return fail(CCA_ERR_WORKSPACE, "weight-gradient workspace too small%s%s");
+    if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dq) | reinterpret_cast<uintptr_t>(dk) | reinterpret_cast<uintptr_t>(dv) |
+         reinterpret_cast<uintptr_t>(ws)) & 15)
+        return fail(CCA_ERR_INVALID, "weight-gradient GEMM needs 16-byte aligned tensors%s%s");
+    const char *why = "";
+    cudaError_t e = qkv_project_wgrad(x, dq, dk, dv, scale, dwq, dwk, dwv, db, (long)pixels, C, Cq, reinterpret_cast<cudaStream_t>(stream),
+                                      &why, ws);
+    if (e != cudaSuccess) return cuda_fail(e, why && *why ? why : "qkv_project_wgrad");
+    return CCA_OK;
+}
 int cca_b200_qkv_wgrad_supported(int C, int Cq)
 {
     if (C <= 0 || Cq <= 0) return 0;
@@ -352,7 +402,7 @@ int cca_b200_forward_host(const void *q, const void *k, const void *v, void *out
     if (!q || !k || !v || !out || !lse) return fail(CCA_ERR_INVALID, "null pointer%s%s");
     const size_t px = (size_t)B * H * W, es = esize(dtype);
     const size_t nq = px * Cq * es, nv = px * C * es, nl = px * sizeof(float);
-    const size_t nws = cca_b200_workspace_bytes(CCA_WS_FORWARD, B, Cq, C, H, W, dtype);
+    const size_t nws = cca_b200_workspace_bytes_ex(CCA_WS_FORWARD, B, Cq, C, H, W, dtype, flags);
     DevBufs d;
     cudaError_t e = cudaStreamCreateWithFlags(&d.st, cudaStreamNonBlocking);
     void *dq = d.alloc(nq, e), *dk = d.alloc(nq, e), *dv = d.alloc(nv, e), *dout = d.alloc(nv, e);
@@ -380,7 +430,7 @@ int cca_b200_backward_host(const void *dout, const void *q, const void *k, const
     if (!dout || !q || !k || !v || !out || !lse || !dq || !dk || !dv) return fail(CCA_ERR_INVALID, "null pointer%s%s");
     const size_t px = (size_t)B * H * W, es = esize(dtype);
     const size_t nq = px * Cq * es, nv = px * C * es, nl = px * sizeof(float);
-    const size_t nws = cca_b200_workspace_bytes(CCA_WS_BACKWARD, B, Cq, C, H, W, dtype);
+    const size_t nws = cca_b200_workspace_bytes_ex(CCA_WS_BACKWARD, B, Cq, C, H, W, dtype, flags);
     DevBufs d;
     cudaError_t e = cudaStreamCreateWithFlags(&d.st, cudaStreamNonBlocking);
     void *g = d.alloc(nv, e), *tq = d.alloc(nq, e), *tk = d.alloc(nq, e), *tv = d.alloc(nv, e), *to = d.alloc(nv, e);

@@ -44,16 +44,27 @@ bool simt_supported(Dims d, bool backward);
 
 bool tc_forward_supported(Dims d, int dtype);
 size_t tc_forward_workspace(Dims d);
+// det: planes mode on tiled lines (fp32 only; the workspace then has tc_planes_bytes more at its end)
 cudaError_t tc_forward(const void *q, const void *k, const void *v, void *out, float *lse, void *ws,
-                       Dims d, int dtype, cudaStream_t st, const char **why);
+                       Dims d, int dtype, cudaStream_t st, const char **why, bool det = false);
 // statistics pre-pass of the tensor-core forward (cca_tc_stats.cu): partial lse planes; also clears a byte range and counters
 cudaError_t tc_stats(const void *q, const void *k, float *parts, void *zero_ptr, long zero_bytes, unsigned int *counters,
                      int n_counters, Dims d, int dtype, cudaStream_t st, const char **why);
 
+// deterministic mode on tiled lines (cca_tc_det.cu): fp32 planes-mode item kernels + the plane sum
+bool tc_tiled(Dims d);                          // a line longer than one tile in either direction
+size_t tc_planes_bytes(int which, Dims d);      // plane workspace (0 on one-tile shapes)
+cudaError_t tc_forward_planes(const void *q, const void *k, const void *v, float *out, float *lse, const float *parts,
+                              unsigned int *cdone, void *planes, Dims d, cudaStream_t st, const char **why);
+cudaError_t tc_backward_planes(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
+                               float *delta, unsigned int *counters, float *dq, float *dk, float *dv, void *planes, Dims d,
+                               int delta_mode, cudaStream_t st, const char **why);
+
 bool tc_backward_supported(Dims d, int dtype);
 size_t tc_backward_workspace(Dims d);
 cudaError_t tc_backward(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
-                        void *dq, void *dk, void *dv, void *ws, Dims d, int dtype, cudaStream_t st, const char **why);
+                        void *dq, void *dk, void *dv, void *ws, Dims d, int dtype, cudaStream_t st, const char **why,
+                        bool det = false);
 
 // wgmma GEMMs of the 1x1 Q/K/V projections (cca_gemm.cu), fp32 channels-last tensors as [pixels, channels] matrices
 bool qkv_gemm_supported(int C, int Cq);
@@ -64,8 +75,11 @@ cudaError_t qkv_project_dgrad(const float *dq, const float *dk, const float *dv,
                               const float *scale, float *dx, void *ws, long P, int C, int Cq, int accumulate, cudaStream_t st,
                               const char **why);
 bool qkv_wgrad_supported(int C, int Cq);
+// ws != nullptr: deterministic variant (per-split partials in ws, qkv_wgrad_workspace bytes, summed in split order)
 cudaError_t qkv_project_wgrad(const float *x, const float *dq, const float *dk, const float *dv, const float *scale, float *dwq,
-                              float *dwk, float *dwv, float *db, long P, int C, int Cq, cudaStream_t st, const char **why);
+                              float *dwk, float *dwv, float *db, long P, int C, int Cq, cudaStream_t st, const char **why,
+                              void *ws = nullptr);
+size_t qkv_wgrad_workspace(int C, int Cq);
 
 void count_launch(int n = 1);
 // Launch knobs of the tensor-core kernels, read once from the environment (std::atomic, safe under DataParallel threads):

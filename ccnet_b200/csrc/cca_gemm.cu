@@ -230,8 +230,12 @@ struct WgradParams {
     const float *x, *dq, *dk, *dv;
     const float *scale;
     float *dwq, *dwk, *dwv, *db;
+    float *part;           // DET: [splits][2Cq + C][C] dW partials, then [splits][16][2Cq + C] db partials (16 loader rows)
 };
 
+// DET (deterministic variant): each split STORES its scaled dW tile and db column sums into its own slice of p.part, and
+// cca_wgrad_sum_kernel adds the splits in split order.  Otherwise the splits atomically add onto the cleared outputs.
+template <bool DET = false>
 __global__ void __launch_bounds__(kGThreads, 1) cca_wgrad_kernel(const __grid_constant__ WgradParams p)
 {
     __shared__ __align__(1024) uint8_t sg[2 * 16 * kWPlane];   // G^T planes: [hi | lo][16 n-chunks][64 px][16 B]
@@ -310,6 +314,25 @@ __global__ void __launch_bounds__(kGThreads, 1) cca_wgrad_kernel(const __grid_co
         first = false;
         __syncthreads();
     }
+    if constexpr (DET) {                                            // every split writes its whole slice, pixels or not
+        const int N = 2 * Cq + C;
+        if (first)
+#pragma unroll
+            for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            float *row = p.part + ((long)split * N + n0 + rbase + 8 * h) * C;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int k = k0 + 8 * j + cq;
+                *reinterpret_cast<float2 *>(row + k) = make_float2(sc * acc[4 * j + 2 * h], sc * acc[4 * j + 2 * h + 1]);
+            }
+        }
+        if (kt == 0)
+#pragma unroll
+            for (int e = 0; e < 8; ++e) p.part[(long)p.splits * N * C + ((long)split * 16 + (t >> 4)) * N + gn + e] = sc * colsum[e];
+        return;
+    }
     if (first) return;                                              // (no pixels in this split)
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -324,6 +347,33 @@ __global__ void __launch_bounds__(kGThreads, 1) cca_wgrad_kernel(const __grid_co
     if (p.db && kt == 0)
 #pragma unroll
         for (int e = 0; e < 8; ++e) atomicAdd(p.db + gn + e, sc * colsum[e]);
+}
+
+// dW, db of the deterministic variant: the splits' partials added in split order
+__global__ void __launch_bounds__(256) cca_wgrad_sum_kernel(const __grid_constant__ WgradParams p)
+{
+    const int C = p.C, Cq = p.Cq, N = 2 * Cq + C;
+    const long nw = (long)N * C, total = nw + (p.db ? N : 0);
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+        const bool w = i < nw;
+        const float *src = w ? p.part + i : p.part + (long)p.splits * nw + (i - nw);
+        const long stride = w ? nw : N;
+        const int terms = w ? p.splits : 16 * p.splits;
+        float s = src[0];
+        for (int k = 1; k < terms; ++k) s += src[k * stride];
+        if (!w) { p.db[i - nw] = s; continue; }
+        const long n = i / C, c = i - n * C;
+        float *dst = n < Cq ? p.dwq + n * C : (n < 2 * Cq ? p.dwk + (n - Cq) * C : p.dwv + (n - 2 * Cq) * C);
+        dst[c] = s;
+    }
+}
+
+// split-K factor of the weight-gradient GEMM: about two CTAs per SM
+int wgrad_splits(int C, int Cq)
+{
+    const int tiles = (2 * Cq + C) / 128 * (C / 64);
+    const int sms = sm_count();
+    return 2 * sms / tiles > 0 ? 2 * sms / tiles : 1;
 }
 
 }  // namespace
@@ -406,26 +456,44 @@ cudaError_t qkv_project_dgrad(const float *dq, const float *dk, const float *dv,
 }
 
 // dWq [Cq,C], dWk [Cq,C], dWv [C,C] = scale * G^T x ; db (packed q | k | v, 2Cq + C floats) = scale * column sums of G.
-// The outputs are cleared here (cudaMemsetAsync) and accumulated by the split-K CTAs.
+// The outputs are cleared here (cudaMemsetAsync) and accumulated by the split-K CTAs; with `ws` (deterministic variant) the
+// splits' partials go to ws and are summed in split order instead.  The split count follows the SM count, so the result is
+// reproducible on one card model.
+size_t qkv_wgrad_workspace(int C, int Cq)
+{
+    const size_t N = (size_t)2 * Cq + C;
+    return (size_t)wgrad_splits(C, Cq) * (N * C + 16 * N) * sizeof(float);
+}
 cudaError_t qkv_project_wgrad(const float *x, const float *dq, const float *dk, const float *dv, const float *scale, float *dwq,
-                              float *dwk, float *dwv, float *db, long P, int C, int Cq, cudaStream_t st, const char **)
+                              float *dwk, float *dwv, float *db, long P, int C, int Cq, cudaStream_t st, const char **, void *ws)
 {
     cudaError_t e;
-    if ((e = cudaMemsetAsync(dwq, 0, sizeof(float) * Cq * C, st)) != cudaSuccess || (e = cudaMemsetAsync(dwk, 0, sizeof(float) * Cq * C, st)) != cudaSuccess ||
-        (e = cudaMemsetAsync(dwv, 0, sizeof(float) * C * C, st)) != cudaSuccess)
+    if (!ws && ((e = cudaMemsetAsync(dwq, 0, sizeof(float) * Cq * C, st)) != cudaSuccess ||
+                (e = cudaMemsetAsync(dwk, 0, sizeof(float) * Cq * C, st)) != cudaSuccess ||
+                (e = cudaMemsetAsync(dwv, 0, sizeof(float) * C * C, st)) != cudaSuccess))
         return e;
-    if (db && (e = cudaMemsetAsync(db, 0, sizeof(float) * (2 * Cq + C), st)) != cudaSuccess) return e;
+    if (!ws && db && (e = cudaMemsetAsync(db, 0, sizeof(float) * (2 * Cq + C), st)) != cudaSuccess) return e;
     WgradParams p = {};
     p.P = (int)P; p.C = C; p.Cq = Cq;
     p.n_row_tiles = (2 * Cq + C) / 128; p.n_col_tiles = C / 64;
     const int tiles = p.n_row_tiles * p.n_col_tiles;
-    const int sms = sm_count();
-    p.splits = 2 * sms / tiles > 0 ? 2 * sms / tiles : 1;
+    p.splits = wgrad_splits(C, Cq);
     const int total_stages = (int)((P + kWPix - 1) / kWPix);
     p.stages_per_split = (total_stages + p.splits - 1) / p.splits;
     p.x = x; p.dq = dq; p.dk = dk; p.dv = dv;
     p.scale = scale; p.dwq = dwq; p.dwk = dwk; p.dwv = dwv; p.db = db;
-    cca_wgrad_kernel<<<tiles * p.splits, kGThreads, 0, st>>>(p);
+    if (!ws) {
+        cca_wgrad_kernel<false><<<tiles * p.splits, kGThreads, 0, st>>>(p);
+        count_launch();
+        return cudaGetLastError();
+    }
+    p.part = reinterpret_cast<float *>(ws);
+    cca_wgrad_kernel<true><<<tiles * p.splits, kGThreads, 0, st>>>(p);
+    count_launch();
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    const long total = (long)(2 * Cq + C) * (C + 1);
+    const long want = (total + 255) / 256;
+    cca_wgrad_sum_kernel<<<(int)(want < 4L * sm_count() ? want : 4L * sm_count()), 256, 0, st>>>(p);
     count_launch();
     return cudaGetLastError();
 }

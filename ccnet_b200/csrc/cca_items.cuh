@@ -141,6 +141,8 @@ CCA_HD long item_pixel(const ItemSpace &s, const Item &it, int r)
 }
 // plane of the partial log-sum-exp this (direction, key block) writes / all items read: rows first, then columns
 CCA_HD int part_index(const ItemSpace &s, const Item &it) { return it.col ? s.row.nt + it.ik : it.ik; }
+// plane of the (direction, query tile) partial dK / dV of the deterministic backward (cca_tc_bwd.cuh, planes mode)
+CCA_HD int qtile_part_index(const ItemSpace &s, const Item &it) { return it.col ? s.row.nt + it.iq : it.iq; }
 
 // Zero-ahead: the items of sample b clear the output of sample b + ahead before anybody adds onto it.  Item j of a sample
 // owns bytes [j*share, min(bytes, (j+1)*share)) of that sample's slice of each output tensor.

@@ -15,7 +15,7 @@ size_t tc_backward_workspace(Dims d)
 
 // all tensors channels-last (NHWC), fp32, bf16 or f16
 cudaError_t tc_backward(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
-                        void *dq, void *dk, void *dv, void *ws, Dims d, int dtype, cudaStream_t st, const char **why)
+                        void *dq, void *dk, void *dv, void *ws, Dims d, int dtype, cudaStream_t st, const char **why, bool det)
 {
     float *delta = reinterpret_cast<float *>(ws);
     const size_t delta_bytes = ((size_t)d.B * d.H * d.W * sizeof(float) + 15) & ~(size_t)15;
@@ -24,6 +24,10 @@ cudaError_t tc_backward(const void *dout, const void *q, const void *k, const vo
     const int lk = lk_for(max_tile(sp));
     int mode = tc_delta_mode();                       // -1: automatic = producers compute delta for their sample (the consumers
     if (mode < 0) mode = 1;                           // only ever wait for lower-indexed items, tiled or not)
+    if (det && tc_tiled(d))                           // (fp32: cca_capi.cu refuses 16-bit I/O here)
+        return tc_backward_planes(dout, q, k, v, out, lse, delta, counters, reinterpret_cast<float *>(dq),
+                                  reinterpret_cast<float *>(dk), reinterpret_cast<float *>(dv),
+                                  reinterpret_cast<uint8_t *>(ws) + tc_backward_workspace(d), d, mode, st, why);
     if (dtype == CCA_F16)
         return lk == 80 ? launch_bwd<80, __half>(dout, q, k, v, out, lse, delta, counters, dq, dk, dv, d, mode, st, why)
                         : launch_bwd<112, __half>(dout, q, k, v, out, lse, delta, counters, dq, dk, dv, d, mode, st, why);

@@ -24,6 +24,12 @@
 // written by one thread with a TMA store or a TMA reduce-add at L2: a dV chunk in the dO slot of its chunk, dQ in the K slot,
 // dK in the P / dS planes, each once the MMAs that read that memory have retired in both warpgroups.
 //
+// Planes mode (PL, fp32 only; torch.use_deterministic_algorithms): on tiled lines the reduce-adds above land in no fixed
+// order.  Instead every item STORES its tiles into partial planes, [nparts*B, H, W, C or Cq] buffers: dQ into plane
+// part_index(item) (direction, key block), dK and dV into plane qtile_part_index(item) (direction, query tile).  Each
+// (pixel, plane) pair is written by exactly one item, so there is no clear and no cdone wait (the delta hand-off stays), and
+// cca_planes_sum_kernel (cca_tc_det.cu) adds the planes in plane order into dq, dk, dv.
+//
 // All GEMMs run as bf16x3 split MMAs (hi*hi + hi*lo + lo*hi) with fp32 accumulation in registers (single bf16 / f16 MMAs for
 // 16-bit I/O), two consumer warpgroups of 64 rows each (cca_tc_common.cuh).
 #pragma once
@@ -32,6 +38,11 @@
 
 namespace cca {
 namespace tc {
+
+template <int LK, typename E, bool PL = false>
+cudaError_t launch_bwd(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse, float *delta,
+                       unsigned int *counters, void *dq, void *dk, void *dv, Dims d, int delta_mode, cudaStream_t st,
+                       const char **why);
 
 struct BwdParams {
     ItemSpace sp;
@@ -84,7 +95,7 @@ template <int LK, typename E> struct BwdSmem {
 // does this item compute delta itself (its ring carries the O chunks)?
 __device__ __forceinline__ bool calc_delta(const BwdParams &p, const Item &it) { return p.delta_mode == 0 || (it.col && it.ik == 0); }
 
-template <int LK, typename E>
+template <int LK, typename E, bool PL = false>
 __global__ void __launch_bounds__(kThreads, 1)
 cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant__ CUtensorMap mqr,
                   const __grid_constant__ CUtensorMap mkc, const __grid_constant__ CUtensorMap mkr,
@@ -188,16 +199,18 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
             }
         };
         // (thread 0) the staged boxes -> global: producers store, everybody else reduce-adds; L2 hints as for the loads
-        auto put = [&](const CUtensorMap *m, const uint8_t *tile, int boxes, int c0, int px0, const Item &it, bool prod) {
+        // (PL: `part` is the plane of the box, sample coordinate part * B + b)
+        auto put = [&](const CUtensorMap *m, const uint8_t *tile, int boxes, int c0, int px0, const Item &it, bool prod, int part) {
             const int cw = it.col ? it.line : px0, ch = it.col ? px0 : it.line;
+            const int ob = PL ? part * p.sp.B + it.b : it.b;
             for (int bx = 0; bx < boxes; ++bx) {
                 const uint8_t *src = tile + bx * T::kTile;
                 if (p.hints == 1) {
-                    if (prod) tma_store_4d(m, src, c0 + 32 * bx, cw, ch, it.b, pol_keep);
-                    else tma_reduce_add_4d(m, src, c0 + 32 * bx, cw, ch, it.b, pol_stream);
+                    if (prod) tma_store_4d(m, src, c0 + 32 * bx, cw, ch, ob, pol_keep);
+                    else tma_reduce_add_4d(m, src, c0 + 32 * bx, cw, ch, ob, pol_stream);
                 } else {
-                    if (prod) tma_store_4d(m, src, c0 + 32 * bx, cw, ch, it.b);
-                    else tma_reduce_add_4d(m, src, c0 + 32 * bx, cw, ch, it.b);
+                    if (prod) tma_store_4d(m, src, c0 + 32 * bx, cw, ch, ob);
+                    else tma_reduce_add_4d(m, src, c0 + 32 * bx, cw, ch, ob);
                 }
             }
             bulk_commit();
@@ -211,7 +224,7 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
         for (int k = 0; k < nk; ++k) {
             const Item it = item_of(k);
             const bool calc = calc_delta(p, it);
-            const bool prod = p.out_mode == 1 && is_producer(it);
+            const bool prod = PL || (p.out_mode == 1 && is_producer(it));
             long qpix[2];
             bool qok[2];
             float nlse[2];
@@ -438,7 +451,7 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 fence_proxy_async();
                 consumers_sync();
                 if (t == 0) {
-                    put(it.col ? &mdvc : &mdvr, ds, 1, n * kCh, it.k0, it, prod);
+                    put(it.col ? &mdvc : &mdvr, ds, 1, n * kCh, it.k0, it, prod, qtile_part_index(p.sp, it));
                     pending = (int)rslot(g + per * n + 1);
                 }
                 if (n + 1 < NCH) issue_dv(n + 1);
@@ -518,7 +531,7 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 stage(aq, 64, smem + S::off_qk + T::kSlot);
                 fence_proxy_async();
                 consumers_sync();
-                if (t == 0) put(it.col ? &mdqc : &mdqr, smem + S::off_qk + T::kSlot, qboxes, 0, it.q0, it, prod);
+                if (t == 0) put(it.col ? &mdqc : &mdqr, smem + S::off_qk + T::kSlot, qboxes, 0, it.q0, it, prod, part_index(p.sp, it));
                 wg_fence();
 #pragma unroll
                 for (int ks = 0; ks < KP; ++ks) {
@@ -537,11 +550,11 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 fence_proxy_async();
                 consumers_sync();                                  // (also: the planes and dsum are free for the next item)
                 if (t == 0) {
-                    put(it.col ? &mdkc : &mdkr, pgen, qboxes, 0, it.k0, it, prod);
+                    put(it.col ? &mdkc : &mdkr, pgen, qboxes, 0, it.k0, it, prod, qtile_part_index(p.sp, it));
                     bulk_wait_read<1>();                           // the last dV copy and the dQ copy have read their slots
                     if (pending >= 0) mbar_arrive(&empty[pending]);
                     pending = -1;
-                    if (prod) unpublished = it.b;                  // published once its stores are complete, in the next item
+                    if (!PL && prod) unpublished = it.b;                  // published once its stores are complete, in the next item
                 }
             }
         }
@@ -567,7 +580,8 @@ __global__ void __launch_bounds__(256) cca_bwd_prep_kernel(uint4 *dq, uint4 *dk,
 }
 }  // namespace
 
-template <int LK, typename E>
+// PL: dq, dk, dv are the [nparts*B, H, W, Cq or C] plane buffers (cca_tc_det.cu sums them into the gradients)
+template <int LK, typename E, bool PL>
 cudaError_t launch_bwd(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse, float *delta,
                        unsigned int *counters, void *dq, void *dk, void *dv, Dims d, int delta_mode, cudaStream_t st,
                        const char **why)
@@ -582,7 +596,8 @@ cudaError_t launch_bwd(const void *dout, const void *q, const void *k, const voi
             // loads: LK-pixel boxes, zero-filled past the line; outputs: boxes of one tile of the direction, so a store never
             // reaches into the next tile of a line (pixels past the line are not written)
             const int box = t < 5 ? LK : (r == 0 ? p.sp.col.tl : p.sp.row.tl);
-            if (!get_map(&m[2 * t + r], base[t], d.B, d.H, d.W, ch[t], box, r == 0, kDtype<E>)) {
+            const int nb = PL && t >= 5 ? p.sp.nparts * d.B : d.B;
+            if (!get_map(&m[2 * t + r], base[t], nb, d.H, d.W, ch[t], box, r == 0, kDtype<E>)) {
                 if (why) *why = "cuTensorMapEncodeTiled failed";
                 return cudaErrorInvalidValue;
             }
@@ -593,7 +608,7 @@ cudaError_t launch_bwd(const void *dout, const void *q, const void *k, const voi
     p.ddone = counters; p.cdone = counters + d.B;
     p.delta_mode = delta_mode;
     const bool one_tile = p.sp.col.nt == 1 && p.sp.row.nt == 1;
-    p.out_mode = one_tile ? 1 : 0;
+    p.out_mode = one_tile || PL ? 1 : 0;          // (PL: every item stores; 1 only skips the clear below)
     p.lag = tc_lag() != 0 ? 1 : 0;
     p.hints = tc_l2_hints();
     const long es = sizeof(E);
@@ -603,7 +618,7 @@ cudaError_t launch_bwd(const void *dout, const void *q, const void *k, const voi
     count_launch();
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
-    auto kern = cca_tc_bwd_kernel<LK, E>;
+    auto kern = cca_tc_bwd_kernel<LK, E, PL>;
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem<LK, E>::kBytes);
     if (e != cudaSuccess) return e;
     const int sms = sm_count();
@@ -629,6 +644,13 @@ extern template cudaError_t launch_bwd<80, __half>(const void *, const void *, c
 extern template cudaError_t launch_bwd<112, __half>(const void *, const void *, const void *, const void *, const void *, const float *,
                                                     float *, unsigned int *, void *, void *, void *, Dims, int, cudaStream_t,
                                                     const char **);
+// The planes-mode instantiations (fp32) live in cca_tc_det.cu.
+extern template cudaError_t launch_bwd<80, float, true>(const void *, const void *, const void *, const void *, const void *,
+                                                        const float *, float *, unsigned int *, void *, void *, void *, Dims, int,
+                                                        cudaStream_t, const char **);
+extern template cudaError_t launch_bwd<112, float, true>(const void *, const void *, const void *, const void *, const void *,
+                                                         const float *, float *, unsigned int *, void *, void *, void *, Dims, int,
+                                                         cudaStream_t, const char **);
 
 }  // namespace tc
 }  // namespace cca

@@ -228,13 +228,14 @@ inline int lk_for(int tile) { return tile <= 80 ? 80 : (tile <= 112 ? 112 : 0); 
 bool get_map(CUtensorMap *m, const void *base, int B, int H, int W, int C, int LK, bool col, int dtype);
 // SM count of the CURRENT device (cached per device id)
 int sm_count();
-inline bool shape_supported(Dims d, int dtype)
+// the shapes the kernels are written for (no device query)
+inline bool shape_fits(Dims d, int dtype)
 {
     if (dtype != CCA_F32 && dtype != CCA_BF16 && dtype != CCA_F16) return false;
     if (d.Cq % 16 != 0 || d.Cq > 64 || d.Cq < 16 || d.C % kNC != 0) return false;
-    if (d.H > 112 * 8 || d.W > 112 * 8) return false;        // cca_items.cuh: at most kMaxNT tiles of kMaxTile pixels per line
-    return get_encode() != nullptr;
+    return d.H <= 112 * 8 && d.W <= 112 * 8;                 // cca_items.cuh: at most kMaxNT tiles of kMaxTile pixels per line
 }
+inline bool shape_supported(Dims d, int dtype) { return shape_fits(d, dtype) && get_encode() != nullptr; }
 
 }  // namespace tc
 }  // namespace cca

@@ -16,7 +16,7 @@ size_t tc_forward_workspace(Dims d)
 
 // q,k,v,out are channels-last (NHWC), fp32, bf16 or f16.  Two launches: statistics pre-pass (q,k only), values.
 cudaError_t tc_forward(const void *q, const void *k, const void *v, void *out, float *lse, void *ws, Dims d, int dtype,
-                       cudaStream_t st, const char **why)
+                       cudaStream_t st, const char **why, bool det)
 {
     const ItemSpace sp = make_space(d.B, d.H, d.W);
     const long npix = (long)d.B * d.H * d.W;
@@ -26,6 +26,9 @@ cudaError_t tc_forward(const void *q, const void *k, const void *v, void *out, f
     // statistics; it also clears the per-sample counters of the values kernel
     cudaError_t e = tc_stats(q, k, parts, nullptr, 0, cdone, d.B, d, dtype, st, why);
     if (e != cudaSuccess) return e;
+    if (det && tc_tiled(d))       // (fp32: cca_capi.cu refuses 16-bit I/O here)
+        return tc_forward_planes(q, k, v, reinterpret_cast<float *>(out), lse, parts, cdone,
+                                 reinterpret_cast<uint8_t *>(ws) + tc_forward_workspace(d), d, st, why);
     const int lk = lk_for(max_tile(sp));
     if (dtype == CCA_F16)
         return lk == 80 ? launch_fwd<80, __half>(q, k, v, out, lse, parts, cdone, d, st, why)

@@ -32,6 +32,11 @@
 //                         slot is converted; then chunk n is waited for, one thread stores / reduce-adds chunk n - 1 with TMA,
 //                         and chunk n + 1 is issued.  A slot goes back to the producer once its bulk copy has read it,
 //                         checked one chunk later.
+//
+// Planes mode (PL, fp32 only; torch.use_deterministic_algorithms): with key-block tiling the reduce-adds above land in no
+// fixed order.  Instead every item STORES its O tile into partial plane part_index(item) -- the (direction, key block)
+// index of the lse planes -- of a [nparts*B, H, W, C] buffer; each (pixel, plane) pair is written by exactly one item, so
+// nothing waits for anything, and cca_planes_sum_kernel (cca_tc_det.cu) adds the planes in plane order into out.
 
 #pragma once
 #include "cca_items.cuh"
@@ -39,6 +44,10 @@
 
 namespace cca {
 namespace tc {
+
+template <int LK, typename E, bool PL = false>
+cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, float *lse, const float *parts, unsigned int *cdone,
+                       Dims d, cudaStream_t st, const char **why);
 
 struct FwdParams {
     ItemSpace sp;
@@ -64,7 +73,7 @@ template <int LK, typename E> struct FwdSmem {
     static_assert(kBytes <= 232448, "shared memory budget");
 };
 
-template <int LK, typename E>
+template <int LK, typename E, bool PL = false>
 __global__ void __launch_bounds__(kThreads, 1)
 cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant__ CUtensorMap mqr,
                   const __grid_constant__ CUtensorMap mkc, const __grid_constant__ CUtensorMap mkr,
@@ -156,7 +165,8 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
         int pending = -1;                                          // (thread 0) slot whose bulk store may still be reading it
         for (int k = 0; k < nk; ++k) {
             const Item it = item_of(k);
-            const bool prod = is_producer(it);
+            bool prod = true;                                      // (PL: every item stores)
+            if constexpr (!PL) prod = is_producer(it);
             // ---- partial lse planes of rows rbase (h = 0), rbase + 8 (h = 1): the first kPre are loaded here, all at once, and
             // only used once S is in flight, so their L2 latency overlaps the Q / K wait, the conversion and S
             constexpr int kPre = 4;                                // (one tile per line: 2 planes)
@@ -271,16 +281,17 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 if (t != 0) return;
                 if (n == 0 && !prod) fence_proxy_async_global();  // the counter's acquire (below) before the reduce-adds
                 const uint8_t *sl = smem + S::off_ld + slot_of(n) * T::kSlot;
+                const int ob = PL ? part_index(p.sp, it) * p.sp.B + it.b : it.b;     // sample coordinate of the output box
 #pragma unroll
                 for (int bx = 0; bx < (H16 ? 1 : 2); ++bx) {
                     const int c0 = n * kNC + 32 * bx;
                     const uint8_t *src = sl + bx * T::kTile;
                     if (p.hints == 1) {                            // producers' rows are added onto by the sample's consumers
-                        if (prod) tma_store_4d(mo, src, c0, ow, oh, it.b, pol_keep);
-                        else tma_reduce_add_4d(mo, src, c0, ow, oh, it.b, pol_stream);
+                        if (prod) tma_store_4d(mo, src, c0, ow, oh, ob, pol_keep);
+                        else tma_reduce_add_4d(mo, src, c0, ow, oh, ob, pol_stream);
                     } else {
-                        if (prod) tma_store_4d(mo, src, c0, ow, oh, it.b);
-                        else tma_reduce_add_4d(mo, src, c0, ow, oh, it.b);
+                        if (prod) tma_store_4d(mo, src, c0, ow, oh, ob);
+                        else tma_reduce_add_4d(mo, src, c0, ow, oh, ob);
                     }
                 }
                 bulk_commit();
@@ -318,18 +329,21 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
             else write(o1, NCH - 1);
             acquire(NCH - 1);
             store(NCH - 1);
-            if (prod && t == 0) {                                  // publish: all stores of this item are complete
-                bulk_wait<0>();
-                mbar_arrive(&empty[pending]);
-                pending = -1;
-                publish_count(p.cdone + it.b);
+            if constexpr (!PL) {
+                if (prod && t == 0) {                              // publish: all stores of this item are complete
+                    bulk_wait<0>();
+                    mbar_arrive(&empty[pending]);
+                    pending = -1;
+                    publish_count(p.cdone + it.b);
+                }
             }
         }
         if (t == 0) bulk_wait<0>();                                // shared memory must outlive the last bulk reads
     }
 }
 
-template <int LK, typename E>
+// PL: `out` is the [nparts*B, H, W, C] plane buffer (cca_tc_det.cu sums it into the output)
+template <int LK, typename E, bool PL>
 cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, float *lse, const float *parts, unsigned int *cdone,
                        Dims d, cudaStream_t st, const char **why)
 {
@@ -343,7 +357,8 @@ cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, f
             // loads: LK-pixel boxes, pixels past the line are zero-filled; output: boxes of one tile of the direction, so a
             // store never reaches into the next tile of a line (pixels past the line are not written)
             const int box = t < 3 ? LK : (r == 0 ? p.sp.col.tl : p.sp.row.tl);
-            if (!get_map(&m[2 * t + r], base[t], d.B, d.H, d.W, ch[t], box, r == 0, kDtype<E>)) {
+            const int nb = PL && t == 3 ? p.sp.nparts * d.B : d.B;
+            if (!get_map(&m[2 * t + r], base[t], nb, d.H, d.W, ch[t], box, r == 0, kDtype<E>)) {
                 if (why) *why = "cuTensorMapEncodeTiled failed";
                 return cudaErrorInvalidValue;
             }
@@ -361,7 +376,7 @@ cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, f
     // of 73 and 81) or 2 samples.
     const int lag = tc_lag();
     p.lag = lag >= 0 ? lag : (d.B >= 4 && 3 * p.sp.per_sample >= 4 * grid ? 0 : 1);
-    auto kern = cca_tc_fwd_kernel<LK, E>;
+    auto kern = cca_tc_fwd_kernel<LK, E, PL>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem<LK, E>::kBytes);
     if (e != cudaSuccess) return e;
     cudaLaunchConfig_t cfg = {};
@@ -382,6 +397,11 @@ extern template cudaError_t launch_fwd<80, __half>(const void *, const void *, c
                                                    unsigned int *, Dims, cudaStream_t, const char **);
 extern template cudaError_t launch_fwd<112, __half>(const void *, const void *, const void *, void *, float *, const float *,
                                                     unsigned int *, Dims, cudaStream_t, const char **);
+// The planes-mode instantiations (fp32) live in cca_tc_det.cu.
+extern template cudaError_t launch_fwd<80, float, true>(const void *, const void *, const void *, void *, float *, const float *,
+                                                        unsigned int *, Dims, cudaStream_t, const char **);
+extern template cudaError_t launch_fwd<112, float, true>(const void *, const void *, const void *, void *, float *, const float *,
+                                                         unsigned int *, Dims, cudaStream_t, const char **);
 
 }  // namespace tc
 }  // namespace cca

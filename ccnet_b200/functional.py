@@ -13,6 +13,26 @@ from . import capi
 _DTYPES = {torch.float32: capi.CCA_F32, torch.bfloat16: capi.CCA_BF16, torch.float16: capi.CCA_F16}
 _IMPL_FLAGS = {"auto": capi.CCA_FLAG_AUTO, "simt": capi.CCA_FLAG_FORCE_SIMT, "tc": capi.CCA_FLAG_FORCE_TC}
 
+#: Bytes of partial-plane workspace one deterministic call may allocate (lines longer than 112 pixels).  A batch that would
+#: need more runs in groups of samples; a sample's result does not depend on the batch it is in, so the bits are the same.
+deterministic_workspace_cap = 1 << 30
+
+
+def _resolve_deterministic(deterministic) -> bool:
+    """``deterministic=None`` follows ``torch.use_deterministic_algorithms``."""
+    return torch.are_deterministic_algorithms_enabled() if deterministic is None else bool(deterministic)
+
+
+def _sample_groups(lib, which, B, Cq, C, H, W, dt, flags):
+    """[(b0, b1)]: batch slices whose plane workspace stays under ``deterministic_workspace_cap`` (one slice unless the
+    call needs planes)"""
+    if not flags & capi.CCA_FLAG_DETERMINISTIC:
+        return [(0, B)]
+    per_sample = (lib.cca_b200_workspace_bytes_ex(which, 1, Cq, C, H, W, dt, flags)
+                  - lib.cca_b200_workspace_bytes(which, 1, Cq, C, H, W, dt))
+    g = max(1, deterministic_workspace_cap // per_sample) if per_sample > 0 else B
+    return [(b0, min(B, b0 + g)) for b0 in range(0, B, g)]
+
 
 def _check_inputs(q, k, v):
     if not (q.is_cuda and k.is_cuda and v.is_cuda):
@@ -28,15 +48,31 @@ def _check_inputs(q, k, v):
         raise RuntimeError("ccnet_b200: q,k,v must be on the same device")
 
 
-def _half_long_lines(dtype, H: int, W: int) -> bool:
+def _workspace(nbytes: int, device) -> torch.Tensor:
+    """Device scratch of the C ABI calls.  The kernels write every byte they read, so torch's deterministic mode need not fill
+    it first (its ``torch.empty`` fill would otherwise touch up to ``deterministic_workspace_cap`` bytes per call).  The fill
+    switch is process-wide: a ``torch.empty`` another thread runs meanwhile may come back unfilled."""
+    if not torch.are_deterministic_algorithms_enabled():
+        return torch.empty((max(nbytes, 16),), dtype=torch.uint8, device=device)
+    import torch.utils.deterministic as td
+    fill = td.fill_uninitialized_memory
+    td.fill_uninitialized_memory = False
+    try:
+        return torch.empty((max(nbytes, 16),), dtype=torch.uint8, device=device)
+    finally:
+        td.fill_uninitialized_memory = fill
+
+
+def _half_long_lines(dtype, H: int, W: int, deterministic: bool = False) -> bool:
     """bf16 or fp16 I/O with lines longer than one 112-pixel tile: every output element of the tensor-core kernels is then the
     sum of up to 2*ceil(L/112) TMA reduce-adds, each rounded to the 16-bit type in memory, in no fixed order -- measured at the
     1e-2 budget for bf16 (profiles/r02_parity_report.jsonl).  Such calls run on the fp32 kernels (bf16 and fp16 values are
     exact in the bf16x3 split) and the result is rounded to the 16-bit type ONCE.  CCA_B200_BF16_NATIVE=1 keeps the native
-    bf16 and fp16 kernels for both types (the C ABI always does)."""
+    bf16 and fp16 kernels for both types (the C ABI always does), except in deterministic mode: only the fp32 kernels have
+    it on such lines."""
     import os
     return (dtype in (torch.bfloat16, torch.float16) and (H > 112 or W > 112)
-            and not os.environ.get("CCA_B200_BF16_NATIVE"))
+            and (deterministic or not os.environ.get("CCA_B200_BF16_NATIVE")))
 
 
 def _stream_ptr(device) -> int:
@@ -52,15 +88,19 @@ def tc_eligible(B: int, Cq: int, C: int, H: int, W: int, dtype: torch.dtype) -> 
             and lib.cca_b200_tc_supported(capi.CCA_WS_BACKWARD, B, Cq, C, H, W, _DTYPES[dtype]) == 1)
 
 
-def cca_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto"):
+def cca_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", deterministic=None):
     """One criss-cross step: returns (out[B,C,H,W], lse[B,H,W] fp32).
 
     ``impl``: "auto" (tensor-core kernels when they cover the shape, else the generic kernels),
     "tc" (tensor-core kernels or error), "simt" (generic kernels).  The tensor-core kernels work on
     channels-last memory (logical shape unchanged); inputs in another memory format are converted and
     the output is returned channels-last.  The generic kernels work on NCHW-contiguous memory.
+
+    ``deterministic``: bit-reproducible results (CCA_FLAG_DETERMINISTIC); None follows
+    ``torch.are_deterministic_algorithms_enabled()``.
     """
     _check_inputs(q, k, v)
+    det = _resolve_deterministic(deterministic)
     lib = capi.load()
     B, Cq, H, W = q.shape
     C = v.shape[1]
@@ -69,8 +109,8 @@ def cca_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "
     use_tc = impl in ("auto", "tc") and lib.cca_b200_tc_supported(capi.CCA_WS_FORWARD, B, Cq, C, H, W, dt) == 1
     if impl == "tc" and not use_tc:
         raise RuntimeError(f"ccnet_b200: tensor-core kernels do not cover q{tuple(q.shape)} v{tuple(v.shape)} {q.dtype}")
-    if use_tc and _half_long_lines(q.dtype, H, W):
-        out32, lse = cca_forward(q.float(), k.float(), v.float(), impl)
+    if use_tc and _half_long_lines(q.dtype, H, W, det):
+        out32, lse = cca_forward(q.float(), k.float(), v.float(), impl, det)
         return out32.to(q.dtype), lse
     if use_tc:
         fmt = torch.channels_last
@@ -79,27 +119,32 @@ def cca_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "
     else:
         fmt = torch.contiguous_format
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()   # reference calls .contiguous() too
+    if det:
+        flags |= capi.CCA_FLAG_DETERMINISTIC
     with torch.cuda.device(q.device):
         out = torch.empty_like(v, memory_format=fmt)
         lse = torch.empty((B, H, W), dtype=torch.float32, device=q.device)
-        nws = lib.cca_b200_workspace_bytes(capi.CCA_WS_FORWARD, B, Cq, C, H, W, dt)
-        ws = torch.empty((max(nws, 16),), dtype=torch.uint8, device=q.device)
-        rc = lib.cca_b200_forward(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr(),
-                                  ws.data_ptr(), ws.numel(), B, Cq, C, H, W, dt, flags,
-                                  _stream_ptr(q.device))
-    capi.check(rc, "cca_b200_forward")
+        for b0, b1 in _sample_groups(lib, capi.CCA_WS_FORWARD, B, Cq, C, H, W, dt, flags):
+            n = b1 - b0
+            nws = lib.cca_b200_workspace_bytes_ex(capi.CCA_WS_FORWARD, n, Cq, C, H, W, dt, flags)
+            ws = _workspace(nws, q.device)
+            rc = lib.cca_b200_forward(q[b0:b1].data_ptr(), k[b0:b1].data_ptr(), v[b0:b1].data_ptr(), out[b0:b1].data_ptr(),
+                                      lse[b0:b1].data_ptr(), ws.data_ptr(), ws.numel(), n, Cq, C, H, W, dt, flags,
+                                      _stream_ptr(q.device))
+            capi.check(rc, "cca_b200_forward")
     return out, lse
 
 
-def cca_backward(dout, q, k, v, out, lse, impl: str = "auto", want_delta: bool = False):
+def cca_backward(dout, q, k, v, out, lse, impl: str = "auto", want_delta: bool = False, deterministic=None):
     """Gradients (dq, dk, dv) of ``cca_forward`` given dout and the saved forward tensors.
     ``want_delta``: also return delta[B,H,W] = <dout, out> per pixel as a 4th value when the tensor-core kernels ran (they
     leave it in the workspace; its sum is the gradient of the residual's gamma), else None.
 
-    Same ``impl`` / memory-format rules as ``cca_forward``: the tensor-core kernels take and return
+    Same ``impl`` / memory-format / ``deterministic`` rules as ``cca_forward``: the tensor-core kernels take and return
     channels-last tensors, the generic kernels NCHW-contiguous ones.
     """
     _check_inputs(q, k, v)
+    det = _resolve_deterministic(deterministic)
     lib = capi.load()
     if dout.dtype != q.dtype or out.dtype != q.dtype or dout.shape != v.shape or out.shape != v.shape:
         raise RuntimeError("ccnet_b200: dout/out must match v in shape and dtype")
@@ -114,8 +159,8 @@ def cca_backward(dout, q, k, v, out, lse, impl: str = "auto", want_delta: bool =
     use_tc = impl in ("auto", "tc") and lib.cca_b200_tc_supported(capi.CCA_WS_BACKWARD, B, Cq, C, H, W, dt) == 1
     if impl == "tc" and not use_tc:
         raise RuntimeError(f"ccnet_b200: tensor-core kernels do not cover q{tuple(q.shape)} v{tuple(v.shape)} {q.dtype}")
-    if use_tc and _half_long_lines(q.dtype, H, W):
-        res = cca_backward(dout.float(), q.float(), k.float(), v.float(), out.float(), lse, impl, want_delta)
+    if use_tc and _half_long_lines(q.dtype, H, W, det):
+        res = cca_backward(dout.float(), q.float(), k.float(), v.float(), out.float(), lse, impl, want_delta, det)
         return tuple(g.to(q.dtype) for g in res[:3]) + tuple(res[3:])
     if use_tc:
         fmt = torch.channels_last
@@ -125,19 +170,28 @@ def cca_backward(dout, q, k, v, out, lse, impl: str = "auto", want_delta: bool =
         fmt = torch.contiguous_format
         dout, q, k, v, out = (t.contiguous() for t in (dout, q, k, v, out))
     lse = lse.contiguous()
+    if det:
+        flags |= capi.CCA_FLAG_DETERMINISTIC
     with torch.cuda.device(q.device):
         dq = torch.empty_like(q, memory_format=fmt)
         dk = torch.empty_like(k, memory_format=fmt)
         dv = torch.empty_like(v, memory_format=fmt)
-        nws = lib.cca_b200_workspace_bytes(capi.CCA_WS_BACKWARD, B, Cq, C, H, W, dt)
-        ws = torch.empty((max(nws, 16),), dtype=torch.uint8, device=q.device)
-        rc = lib.cca_b200_backward(dout.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(),
-                                   lse.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
-                                   ws.data_ptr(), ws.numel(), B, Cq, C, H, W, dt, flags,
-                                   _stream_ptr(q.device))
-    capi.check(rc, "cca_b200_backward")
+        groups = _sample_groups(lib, capi.CCA_WS_BACKWARD, B, Cq, C, H, W, dt, flags)
+        delta = torch.empty((B, H, W), dtype=torch.float32, device=q.device) if want_delta and len(groups) > 1 else None
+        for b0, b1 in groups:
+            n = b1 - b0
+            nws = lib.cca_b200_workspace_bytes_ex(capi.CCA_WS_BACKWARD, n, Cq, C, H, W, dt, flags)
+            ws = _workspace(nws, q.device)
+            rc = lib.cca_b200_backward(dout[b0:b1].data_ptr(), q[b0:b1].data_ptr(), k[b0:b1].data_ptr(), v[b0:b1].data_ptr(),
+                                       out[b0:b1].data_ptr(), lse[b0:b1].data_ptr(), dq[b0:b1].data_ptr(),
+                                       dk[b0:b1].data_ptr(), dv[b0:b1].data_ptr(), ws.data_ptr(), ws.numel(),
+                                       n, Cq, C, H, W, dt, flags, _stream_ptr(q.device))
+            capi.check(rc, "cca_b200_backward")
+            if delta is not None and use_tc:     # (the delta of each group is in its workspace)
+                delta[b0:b1].copy_(ws[:n * H * W * 4].view(torch.float32).view(n, H, W))
     if want_delta:
-        delta = ws[:B * H * W * 4].view(torch.float32).view(B, H, W) if use_tc else None
+        if delta is None:
+            delta = ws[:B * H * W * 4].view(torch.float32).view(B, H, W) if use_tc else None
         return dq, dk, dv, delta
     return dq, dk, dv
 
@@ -199,9 +253,12 @@ def qkv_wgrad_eligible(C: int, Cq: int) -> bool:
     return capi.load().cca_b200_qkv_wgrad_supported(C, Cq) == 1
 
 
-def qkv_project_wgrad(x, dq, dk, dv, scale=None):
-    """(dWq, dbq, dWk, dbk, dWv, dbv) = s * (gradients of the three 1x1 convs' parameters), one split-K wgmma launch."""
+def qkv_project_wgrad(x, dq, dk, dv, scale=None, deterministic=None):
+    """(dWq, dbq, dWk, dbk, dWv, dbv) = s * (gradients of the three 1x1 convs' parameters), one split-K wgmma launch.
+    ``deterministic`` (None: ``torch.are_deterministic_algorithms_enabled()``): the splits' partials are added in a fixed
+    order (reproducible on one GPU model) instead of with atomics."""
     lib = capi.load()
+    det = _resolve_deterministic(deterministic)
     B, C, H, W = x.shape
     Cq = dq.shape[1]
     x, dq, dk, dv = (t.contiguous(memory_format=torch.channels_last) for t in (x, dq, dk, dv))
@@ -210,28 +267,34 @@ def qkv_project_wgrad(x, dq, dk, dv, scale=None):
         dwk = torch.empty((Cq, C), dtype=x.dtype, device=x.device)
         dwv = torch.empty((C, C), dtype=x.dtype, device=x.device)
         db = torch.empty((2 * Cq + C,), dtype=x.dtype, device=x.device)
-        rc = lib.cca_b200_qkv_project_wgrad(x.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
-                                            scale.data_ptr() if scale is not None else None, dwq.data_ptr(), dwk.data_ptr(),
-                                            dwv.data_ptr(), db.data_ptr(), B * H * W, C, Cq, _stream_ptr(x.device))
-    capi.check(rc, "cca_b200_qkv_project_wgrad")
+        nws = lib.cca_b200_qkv_wgrad_workspace_bytes(C, Cq) if det else 0
+        ws = _workspace(nws, x.device) if det else None
+        rc = lib.cca_b200_qkv_project_wgrad_ex(x.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
+                                               scale.data_ptr() if scale is not None else None, dwq.data_ptr(),
+                                               dwk.data_ptr(), dwv.data_ptr(), db.data_ptr(), B * H * W, C, Cq,
+                                               ws.data_ptr() if det else None, nws,
+                                               capi.CCA_FLAG_DETERMINISTIC if det else 0, _stream_ptr(x.device))
+    capi.check(rc, "cca_b200_qkv_project_wgrad_ex")
     return dwq, db[:Cq], dwk, db[Cq:2 * Cq], dwv, db[2 * Cq:]
 
 
 class _CCAFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, impl):
-        out, lse = cca_forward(q, k, v, impl)
+    def forward(ctx, q, k, v, impl, deterministic):
+        out, lse = cca_forward(q, k, v, impl, deterministic)
         ctx.save_for_backward(q, k, v, out, lse)
         ctx.impl = impl
+        ctx.deterministic = deterministic
         return out
 
     @staticmethod
     def backward(ctx, dout):
         q, k, v, out, lse = ctx.saved_tensors
-        dq, dk, dv = cca_backward(dout, q, k, v, out, lse, ctx.impl)
-        return dq, dk, dv, None
+        dq, dk, dv = cca_backward(dout, q, k, v, out, lse, ctx.impl, deterministic=ctx.deterministic)
+        return dq, dk, dv, None, None
 
 
-def cca(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto") -> torch.Tensor:
-    """Differentiable criss-cross attention step (out only)."""
-    return _CCAFunction.apply(q, k, v, impl)
+def cca(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", deterministic=None) -> torch.Tensor:
+    """Differentiable criss-cross attention step (out only).  ``deterministic``: as for ``cca_forward``; the mode is fixed
+    when the forward runs and the backward uses it too."""
+    return _CCAFunction.apply(q, k, v, impl, _resolve_deterministic(deterministic))

@@ -76,6 +76,14 @@ typedef enum cca_status {
                                  * both "L pixels with contiguous channels", so TMA boxes and UMMA operand
                                  * tiles serve the two branches symmetrically.  Without the flag tensors
                                  * are NCHW-contiguous and the generic kernels run.                      */
+#define CCA_FLAG_DETERMINISTIC 8u /* bit-reproducible results (what torch.use_deterministic_algorithms asks
+                                 * for).  One-tile shapes and the generic kernels are deterministic anyway:
+                                 * the flag changes nothing there.  Lines longer than 112 pixels on the
+                                 * tensor-core kernels: every item stores its share into partial planes of
+                                 * the workspace (cca_b200_workspace_bytes_ex) instead of reduce-adding it
+                                 * onto the output in no fixed order, and one more kernel adds the planes
+                                 * in a fixed order.  fp32 only there: 16-bit I/O on such lines returns
+                                 * CCA_ERR_UNSUPPORTED (call CCA_F32 on upcast tensors).                   */
 
 /* which workspace */
 #define CCA_WS_FORWARD 0
@@ -104,9 +112,16 @@ CCA_API int cca_b200_tc_supported(int which, int B, int Cq, int C, int H, int W,
  *   lagged = 0: samples one after the other; 1: the consumers of a sample trail its producers by one block. */
 CCA_API void cca_b200_item_space(int B, int H, int W, int *out8);
 CCA_API void cca_b200_decode_item(int B, int H, int W, int index, int lagged, int *out10);
+/* item_planes: out2 = {partial plane of the item's out / dQ tile, partial plane of its dK / dV tile} in the deterministic
+ *   mode (CCA_FLAG_DETERMINISTIC) on tiled lines; same index / lagged as decode_item. */
+CCA_API void cca_b200_item_planes(int B, int H, int W, int index, int lagged, int *out2);
 
-/* Bytes of device workspace the forward / backward call needs for this problem. */
+/* Bytes of device workspace the forward / backward call needs for this problem.  _ex: for these flags (with
+ * CCA_FLAG_DETERMINISTIC | CCA_FLAG_NHWC on tiled lines it adds the partial planes: nparts * B*H*W * C floats forward,
+ * nparts * B*H*W * (2 Cq + C) backward, nparts = ceil(H/112) + ceil(W/112)); the plain call assumes flags without
+ * CCA_FLAG_DETERMINISTIC. */
 CCA_API size_t cca_b200_workspace_bytes(int which, int B, int Cq, int C, int H, int W, int dtype);
+CCA_API size_t cca_b200_workspace_bytes_ex(int which, int B, int Cq, int C, int H, int W, int dtype, unsigned flags);
 
 /*
  * One criss-cross attention step, forward (replaces functions.py:30-47):
@@ -154,6 +169,14 @@ CCA_API int cca_b200_qkv_wgrad_supported(int C, int Cq);
 CCA_API int cca_b200_qkv_project_wgrad(const float *x, const float *dq, const float *dk, const float *dv, const float *scale,
                                        float *dwq, float *dwk, float *dwv, float *db,
                                        long long pixels, int C, int Cq, void *cuda_stream);
+/* qkv_project_wgrad with flags.  CCA_FLAG_DETERMINISTIC: every split-K CTA stores its partial dW and db into the device
+ * workspace (cca_b200_qkv_wgrad_workspace_bytes, which depends on the current device's SM count) and a second kernel adds
+ * them in split order -- bit-reproducible on one card model (the split count follows the SM count).  Without the flag it
+ * is cca_b200_qkv_project_wgrad (the workspace may be NULL). */
+CCA_API size_t cca_b200_qkv_wgrad_workspace_bytes(int C, int Cq);
+CCA_API int cca_b200_qkv_project_wgrad_ex(const float *x, const float *dq, const float *dk, const float *dv, const float *scale,
+                                          float *dwq, float *dwk, float *dwv, float *db, long long pixels, int C, int Cq,
+                                          void *workspace, size_t workspace_bytes, unsigned flags, void *cuda_stream);
 
 /*
  * Host-buffer variants: same maths, pointers are HOST memory (pinned or pageable).
