@@ -271,6 +271,110 @@ int cca_b200_backward(const void *dout, const void *q, const void *k, const void
 }
 
 // ---------------------------------------------------------------------------------------
+// attention map (functions.py:40 `concate`) and its gradient w.r.t. q, k
+// ---------------------------------------------------------------------------------------
+namespace {
+int check_attention_dims(int B, int Cq, int H, int W, int dtype)
+{
+    int rc = check_dims(B, Cq, 1, H, W, dtype);
+    if (rc) return rc;
+    if ((long long)B * Cq * H * W >= (1ll << 40) || (long long)B * H * W * (H + W) >= (1ll << 40))
+        return fail(CCA_ERR_UNSUPPORTED, "tensor too large%s%s");
+    return CCA_OK;
+}
+bool attention_det_planes(Dims d, int dtype, unsigned flags)
+{
+    return (flags & CCA_FLAG_DETERMINISTIC) && (flags & CCA_FLAG_NHWC) && dtype == CCA_F32 && tc::shape_fits(Dims{d.B, d.Cq, tc::kNC, d.H, d.W}, dtype);
+}
+// which family runs (after the common checks): 1 tensor cores, 0 generic kernels, < 0 an error status
+int attention_family(Dims d, int dtype, unsigned flags, bool backward)
+{
+    if ((flags & CCA_FLAG_FORCE_SIMT) && (flags & CCA_FLAG_FORCE_TC))
+        return fail(CCA_ERR_INVALID, "FORCE_SIMT and FORCE_TC are exclusive%s%s");
+    const bool nhwc = (flags & CCA_FLAG_NHWC) != 0;
+    int rc = check_device();
+    if (rc) return rc;
+    const bool tc_ok = nhwc && tc_attention_supported(d, dtype);
+    if ((flags & CCA_FLAG_FORCE_TC) && !tc_ok)
+        return fail(CCA_ERR_UNSUPPORTED, "tensor-core attention map needs CCA_FLAG_NHWC and a covered shape%s%s");
+    if (nhwc && (!tc_ok || (flags & CCA_FLAG_FORCE_SIMT)))
+        return fail(CCA_ERR_UNSUPPORTED, "channels-last tensors are only handled by the tensor-core kernels; pass NCHW%s%s");
+    // (the forward writes every map element once: deterministic in every mode)
+    if (backward && tc_ok && (flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d) && dtype != CCA_F32)
+        return fail(CCA_ERR_UNSUPPORTED, kDetHalfMsg);
+    return tc_ok ? 1 : 0;
+}
+}  // namespace
+
+int cca_b200_attention_tc_supported(int B, int Cq, int H, int W, int dtype)
+{
+    if (check_attention_dims(B, Cq, H, W, dtype)) return 0;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && device_major() != 9) return 0;   // (no device at all: shape answer only)
+    return tc_attention_supported(Dims{B, Cq, 0, H, W}, dtype) ? 1 : 0;
+}
+
+size_t cca_b200_attention_workspace_bytes(int backward, int B, int Cq, int H, int W, int dtype, unsigned flags)
+{
+    if (B <= 0 || Cq <= 0 || H <= 0 || W <= 0) return 0;
+    const Dims d{B, Cq, 0, H, W};
+    const size_t simt = backward ? (size_t)B * H * W * sizeof(float) + 16 : 16;   // backward: rho
+    const size_t tcb = tc_attention_workspace(backward, d, attention_det_planes(d, dtype, flags));
+    return simt > tcb ? simt : tcb;
+}
+
+int cca_b200_attention_forward(const void *q, const void *k, float *attn, void *ws, size_t ws_bytes, int B, int Cq, int H, int W,
+                               int dtype, unsigned flags, void *stream)
+{
+    int rc = check_attention_dims(B, Cq, H, W, dtype);
+    if (rc) return rc;
+    if (!q || !k || !attn || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
+    if (reinterpret_cast<uintptr_t>(attn) & 3) return fail(CCA_ERR_INVALID, "attn must be 4-byte aligned%s%s");
+    if (ws_bytes < cca_b200_attention_workspace_bytes(0, B, Cq, H, W, dtype, flags))
+        return fail(CCA_ERR_WORKSPACE, "attention map workspace too small%s%s");
+    const Dims d{B, Cq, 0, H, W};
+    const int fam = attention_family(d, dtype, flags, false);
+    if (fam < 0) return fam;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const char *why = "";
+    if (fam == 1) {
+        if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(ws)) & 15)
+            return fail(CCA_ERR_INVALID, "tensor-core path needs 16-byte aligned tensors%s%s");
+        cudaError_t e = tc_attention_forward(q, k, attn, ws, d, dtype, st, &why);
+        return e != cudaSuccess ? cuda_fail(e, why && *why ? why : "tc_attention_forward") : CCA_OK;
+    }
+    cudaError_t e = simt_attention_forward(q, k, attn, d, dtype, st);
+    return e != cudaSuccess ? cuda_fail(e, "simt_attention_forward") : CCA_OK;
+}
+
+int cca_b200_attention_backward(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk, void *ws,
+                                size_t ws_bytes, int B, int Cq, int H, int W, int dtype, unsigned flags, void *stream)
+{
+    int rc = check_attention_dims(B, Cq, H, W, dtype);
+    if (rc) return rc;
+    if (!dattn || !attn || !q || !k || !dq || !dk || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
+    if ((reinterpret_cast<uintptr_t>(attn) | reinterpret_cast<uintptr_t>(dattn)) & 3)
+        return fail(CCA_ERR_INVALID, "attn and dattn must be 4-byte aligned%s%s");
+    if (ws_bytes < cca_b200_attention_workspace_bytes(1, B, Cq, H, W, dtype, flags))
+        return fail(CCA_ERR_WORKSPACE, "attention map backward workspace too small%s%s");
+    const Dims d{B, Cq, 0, H, W};
+    const int fam = attention_family(d, dtype, flags, true);
+    if (fam < 0) return fam;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const char *why = "";
+    if (fam == 1) {
+        if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(dq) |
+             reinterpret_cast<uintptr_t>(dk) | reinterpret_cast<uintptr_t>(ws)) & 15)
+            return fail(CCA_ERR_INVALID, "tensor-core path needs 16-byte aligned tensors%s%s");
+        cudaError_t e = tc_attention_backward(dattn, attn, q, k, dq, dk, ws, d, dtype, st, &why,
+                                              (flags & CCA_FLAG_DETERMINISTIC) != 0);
+        return e != cudaSuccess ? cuda_fail(e, why && *why ? why : "tc_attention_backward") : CCA_OK;
+    }
+    cudaError_t e = simt_attention_backward(dattn, attn, q, k, dq, dk, ws, d, dtype, st);
+    return e != cudaSuccess ? cuda_fail(e, "simt_attention_backward") : CCA_OK;
+}
+
+// ---------------------------------------------------------------------------------------
 // 1x1 Q/K/V projections (functions.py:29,32,35) as tensor-core GEMMs on the channels-last view
 // ---------------------------------------------------------------------------------------
 int cca_b200_qkv_supported(int C, int Cq)

@@ -66,6 +66,23 @@ cudaError_t tc_backward(const void *dout, const void *q, const void *k, const vo
                         void *dq, void *dk, void *dv, void *ws, Dims d, int dtype, cudaStream_t st, const char **why,
                         bool det = false);
 
+// the attention map attn[B,H,W,H+W] (fp32) and its gradient w.r.t. q, k (Dims.C is not used)
+//   generic kernels, NCHW q, k (cca_simt_attn.cu); the backward's workspace is rho [B*H*W]
+cudaError_t simt_attention_forward(const void *q, const void *k, float *attn, Dims d, int dtype, cudaStream_t st);
+cudaError_t simt_attention_backward(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk,
+                                    void *ws, Dims d, int dtype, cudaStream_t st);
+//   rho[p] = sum_j attn[p,j] dattn[p,j] over the hw2 = H+W entries of each of the npix pixels (one warp per pixel, fixed
+//   order); also clears clear_bytes at each of c0 and c1 (may be 0)
+cudaError_t attn_rho(const float *dattn, const float *attn, float *rho, long npix, int hw2, void *c0, void *c1, long clear_bytes,
+                     cudaStream_t st);
+//   tensor-core kernels, channels-last q, k (cca_tc_attn.cu); det: planes mode on tiled lines (fp32 only)
+bool tc_attention_supported(Dims d, int dtype);
+size_t tc_attention_workspace(int backward, Dims d, bool det);
+cudaError_t tc_attention_forward(const void *q, const void *k, float *attn, void *ws, Dims d, int dtype, cudaStream_t st,
+                                 const char **why);
+cudaError_t tc_attention_backward(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk, void *ws,
+                                  Dims d, int dtype, cudaStream_t st, const char **why, bool det);
+
 // wgmma GEMMs of the 1x1 Q/K/V projections (cca_gemm.cu), fp32 channels-last tensors as [pixels, channels] matrices
 bool qkv_gemm_supported(int C, int Cq);
 size_t qkv_gemm_workspace(int C, int Cq);

@@ -221,6 +221,8 @@ inline bool make_map(CUtensorMap *m, const void *base, int B, int H, int W, int 
                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
+// byte offsets of the workspace's plane buffers (256-byte aligned; TMA needs 16)
+inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 // LK template (padded tile length) for the longest tile of a problem
 inline int lk_for(int tile) { return tile <= 80 ? 80 : (tile <= 112 ? 112 : 0); }
 // Cached tensor maps (cca_tc_host.cu): encoding costs ~1 us of driver time per map and an op call needs 8-15 of them;
@@ -228,6 +230,9 @@ inline int lk_for(int tile) { return tile <= 80 ? 80 : (tile <= 112 ? 112 : 0); 
 bool get_map(CUtensorMap *m, const void *base, int B, int H, int W, int C, int LK, bool col, int dtype);
 // SM count of the CURRENT device (cached per device id)
 int sm_count();
+// dst[t] = sum of the nparts planes [nparts][n[t]] at src[t], added in plane order, for count <= 3 tensors; launched with
+// programmatic dependent launch after the kernel that writes the planes (cca_tc_det.cu)
+cudaError_t planes_sum(const float *const *src, float *const *dst, const long *n, int count, int nparts, cudaStream_t st);
 // the shapes the kernels are written for (no device query)
 inline bool shape_fits(Dims d, int dtype)
 {

@@ -45,6 +45,8 @@ __global__ void __launch_bounds__(256) cca_planes_sum_kernel(const __grid_consta
     }
 }
 
+}  // namespace
+
 cudaError_t planes_sum(const float *const *src, float *const *dst, const long *n, int count, int nparts, cudaStream_t st)
 {
     PlaneSums p = {};
@@ -70,8 +72,6 @@ cudaError_t planes_sum(const float *const *src, float *const *dst, const long *n
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-}  // namespace
 }  // namespace tc
 
 using namespace tc;

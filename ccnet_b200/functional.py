@@ -298,3 +298,129 @@ def cca(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", d
     """Differentiable criss-cross attention step (out only).  ``deterministic``: as for ``cca_forward``; the mode is fixed
     when the forward runs and the backward uses it too."""
     return _CCAFunction.apply(q, k, v, impl, _resolve_deterministic(deterministic))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# attention map (cc_attention/functions.py:40, the softmax output `concate`) and its gradient
+# ---------------------------------------------------------------------------------------------------------------------
+def _check_qk(q, k):
+    if not (q.is_cuda and k.is_cuda):
+        raise RuntimeError("ccnet_b200: the attention map needs CUDA tensors on an H100 (sm_90) "
+                           "(there is no CPU path in this package)")
+    if q.dtype not in _DTYPES or k.dtype != q.dtype:
+        raise RuntimeError(f"ccnet_b200: q,k must share dtype float32, bfloat16 or float16, got {q.dtype},{k.dtype}")
+    if q.dim() != 4 or k.shape != q.shape:
+        raise RuntimeError(f"ccnet_b200: expected q,k [B,Cq,H,W], got {tuple(q.shape)},{tuple(k.shape)}")
+    if q.device != k.device:
+        raise RuntimeError("ccnet_b200: q,k must be on the same device")
+
+
+def attention_tc_eligible(B: int, Cq: int, H: int, W: int, dtype: torch.dtype) -> bool:
+    """True if the wgmma (channels-last) attention-map kernels cover this problem."""
+    return dtype in _DTYPES and capi.load().cca_b200_attention_tc_supported(B, Cq, H, W, _DTYPES[dtype]) == 1
+
+
+def cca_attention_forward(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", deterministic=None) -> torch.Tensor:
+    """The attention map of one criss-cross step, attn[B,H,W,H+W] float32 (the reference's ``concate``): attn[b,h,w,g] is
+    the weight of column key (g, w) for g < H (0 at g == h) and of row key (h, g - H) for g >= H.
+
+    ``impl`` as for ``cca_forward``.  Every map element is written once, so the result is the same in every mode;
+    ``deterministic`` only sets the flag the C ABI is called with."""
+    _check_qk(q, k)
+    det = _resolve_deterministic(deterministic)
+    lib = capi.load()
+    B, Cq, H, W = q.shape
+    dt = _DTYPES[q.dtype]
+    flags = _IMPL_FLAGS[impl]
+    use_tc = impl in ("auto", "tc") and lib.cca_b200_attention_tc_supported(B, Cq, H, W, dt) == 1
+    if impl == "tc" and not use_tc:
+        raise RuntimeError(f"ccnet_b200: tensor-core kernels do not cover q{tuple(q.shape)} {q.dtype}")
+    if use_tc:
+        q, k = (t.contiguous(memory_format=torch.channels_last) for t in (q, k))
+        flags |= capi.CCA_FLAG_NHWC
+    else:
+        q, k = q.contiguous(), k.contiguous()
+    if det:
+        flags |= capi.CCA_FLAG_DETERMINISTIC
+    with torch.cuda.device(q.device):
+        attn = torch.empty((B, H, W, H + W), dtype=torch.float32, device=q.device)
+        ws = _workspace(lib.cca_b200_attention_workspace_bytes(0, B, Cq, H, W, dt, flags), q.device)
+        rc = lib.cca_b200_attention_forward(q.data_ptr(), k.data_ptr(), attn.data_ptr(), ws.data_ptr(), ws.numel(),
+                                            B, Cq, H, W, dt, flags, _stream_ptr(q.device))
+        capi.check(rc, "cca_b200_attention_forward")
+    return attn
+
+
+def cca_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministic=None):
+    """Gradients (dq, dk) of ``cca_attention_forward`` given dattn = dL/dattn and the forward's map:
+    dS = attn * (dattn - rho), rho = sum_j attn dattn;  dq = dS k,  dk = dS^T q.  Same ``impl`` / memory-format /
+    ``deterministic`` rules as ``cca_backward``."""
+    _check_qk(q, k)
+    det = _resolve_deterministic(deterministic)
+    lib = capi.load()
+    B, Cq, H, W = q.shape
+    for name, t in (("attn", attn), ("dattn", dattn)):
+        if t.dtype != torch.float32 or tuple(t.shape) != (B, H, W, H + W) or t.device != q.device:
+            raise RuntimeError(f"ccnet_b200: {name} must be a float32 [B,H,W,H+W] tensor on the device of q, k")
+    dt = _DTYPES[q.dtype]
+    flags = _IMPL_FLAGS[impl]
+    use_tc = impl in ("auto", "tc") and lib.cca_b200_attention_tc_supported(B, Cq, H, W, dt) == 1
+    if impl == "tc" and not use_tc:
+        raise RuntimeError(f"ccnet_b200: tensor-core kernels do not cover q{tuple(q.shape)} {q.dtype}")
+    if use_tc and _half_long_lines(q.dtype, H, W, det):
+        dq, dk = cca_attention_backward(dattn, attn, q.float(), k.float(), impl, det)
+        return dq.to(q.dtype), dk.to(q.dtype)
+    if use_tc:
+        fmt = torch.channels_last
+        q, k = (t.contiguous(memory_format=fmt) for t in (q, k))
+        flags |= capi.CCA_FLAG_NHWC
+    else:
+        fmt = torch.contiguous_format
+        q, k = q.contiguous(), k.contiguous()
+    dattn, attn = dattn.contiguous(), attn.contiguous()
+    if det:
+        flags |= capi.CCA_FLAG_DETERMINISTIC
+    with torch.cuda.device(q.device):
+        dq = torch.empty_like(q, memory_format=fmt)
+        dk = torch.empty_like(k, memory_format=fmt)
+        for b0, b1 in _attention_groups(lib, B, Cq, H, W, dt, flags):
+            n = b1 - b0
+            ws = _workspace(lib.cca_b200_attention_workspace_bytes(1, n, Cq, H, W, dt, flags), q.device)
+            rc = lib.cca_b200_attention_backward(dattn[b0:b1].data_ptr(), attn[b0:b1].data_ptr(), q[b0:b1].data_ptr(),
+                                                 k[b0:b1].data_ptr(), dq[b0:b1].data_ptr(), dk[b0:b1].data_ptr(),
+                                                 ws.data_ptr(), ws.numel(), n, Cq, H, W, dt, flags, _stream_ptr(q.device))
+            capi.check(rc, "cca_b200_attention_backward")
+    return dq, dk
+
+
+def _attention_groups(lib, B, Cq, H, W, dt, flags):
+    """``_sample_groups`` for the map backward: batch slices whose plane workspace stays under
+    ``deterministic_workspace_cap``"""
+    if not flags & capi.CCA_FLAG_DETERMINISTIC:
+        return [(0, B)]
+    per_sample = (lib.cca_b200_attention_workspace_bytes(1, 1, Cq, H, W, dt, flags)
+                  - lib.cca_b200_attention_workspace_bytes(1, 1, Cq, H, W, dt, flags & ~capi.CCA_FLAG_DETERMINISTIC))
+    g = max(1, deterministic_workspace_cap // per_sample) if per_sample > 0 else B
+    return [(b0, min(B, b0 + g)) for b0 in range(0, B, g)]
+
+
+class _CCAAttentionFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, q, k, impl, deterministic):
+        attn = cca_attention_forward(q, k, impl, deterministic)
+        ctx.save_for_backward(q, k, attn)
+        ctx.impl = impl
+        ctx.deterministic = deterministic
+        return attn
+
+    @staticmethod
+    def backward(ctx, dattn):
+        q, k, attn = ctx.saved_tensors
+        dq, dk = cca_attention_backward(dattn, attn, q, k, ctx.impl, ctx.deterministic)
+        return dq, dk, None, None
+
+
+def cca_attention(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", deterministic=None) -> torch.Tensor:
+    """Differentiable attention map attn[B,H,W,H+W] (float32) of one criss-cross step; the gradient flows to q and k.
+    ``deterministic``: as for ``cca``; the mode is fixed when the forward runs and the backward uses it too."""
+    return _CCAAttentionFunction.apply(q, k, impl, _resolve_deterministic(deterministic))

@@ -11,6 +11,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from . import ops  # noqa: F401  (torch.ops.cca.attention)
+
 from .functional import (cca, cca_backward, cca_forward, qkv_gemm_eligible, qkv_project, qkv_project_dgrad,
                          qkv_project_wgrad, qkv_wgrad_eligible, tc_eligible)
 
@@ -106,7 +108,18 @@ class CrissCrossAttention(nn.Module):
         self.gamma = nn.Parameter(torch.zeros(1))                                                  # functions.py:24
         self.impl = impl
 
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
+    def forward(self, x: torch.Tensor, return_attention: bool = False):
+        """``return_attention=True`` returns ``(y, attn)``: y exactly as without it, and the step's attention map
+        attn[B,H,W,H+W] (float32; the reference's softmax output ``concate``, functions.py:40), differentiable back to x and
+        the query / key convs.  The fused kernels never materialise the map, so it costs two more Cq-channel 1x1 convs, a
+        second statistics pass and B*H*W*(H+W)*4 bytes; a hook on ``self.softmax`` still does not fire."""
+        y = self._step(x)
+        if not return_attention:
+            return y
+        q, k = self.query_conv(x), self.key_conv(x)      # functions.py:29,32
+        return y, torch.ops.cca.attention(q, k, self.impl)
+
+    def _step(self, x: torch.Tensor) -> torch.Tensor:
         if not x.is_cuda:
             raise RuntimeError("ccnet_b200.CrissCrossAttention runs on CUDA (H100, sm_90) only; "
                                "the CPU restatement lives in oracle/ and is test-only")
@@ -142,8 +155,13 @@ class RCCA(nn.Module):
         self.cca = CrissCrossAttention(in_dim, impl)
         self.recurrence = recurrence
 
-    def forward(self, x):
-        out = x
+    def forward(self, x, return_attention: bool = False):
+        """``return_attention=True`` returns ``(out, [attn_1, ..., attn_R])``, the map of every step."""
+        out, maps = x, []
         for _ in range(self.recurrence):
-            out = self.cca(out)
-        return out
+            if return_attention:
+                out, a = self.cca(out, return_attention=True)
+                maps.append(a)
+            else:
+                out = self.cca(out)
+        return (out, maps) if return_attention else out

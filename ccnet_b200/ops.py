@@ -3,10 +3,12 @@
     torch.ops.cca.forward(q, k, v)                        -> (out, lse)
     torch.ops.cca.backward(dout, q, k, v, out, lse)       -> (dq, dk, dv)
     torch.ops.cca.forward_residual(q, k, v, x, gamma)     -> (y, lse)        y = gamma * out + x  (functions.py:49)
+    torch.ops.cca.attention(q, k)                         -> attn            [B,H,W,H+W] fp32 (functions.py:40, `concate`)
+    torch.ops.cca.attention_backward(dattn, attn, q, k)   -> (dq, dk)
 
 CUDA implementations call the C ABI (ccnet_b200.functional -> libcca_b200.so); FakeTensor ("meta") implementations give
 shapes / dtypes / memory formats so that ``torch.compile`` and ``torch.export`` trace through ``networks/ccnet.py`` without a
-graph break; autograd is registered on ``forward`` and ``forward_residual``.  Registration happens through ``torch.library``
+graph break; autograd is registered on ``forward``, ``forward_residual`` and ``attention``.  Registration happens through ``torch.library``
 (the Python face of TORCH_LIBRARY): the kernels themselves stay behind the torch-free C ABI."""
 from __future__ import annotations
 
@@ -90,3 +92,48 @@ def _res_backward(ctx, dy, dlse, dout_unused):
 
 
 forward_residual.register_autograd(_res_backward, setup_context=_res_setup)
+
+
+# ---- the attention map (functions.py:40 `concate`):  attention(q, k) -> attn[B,H,W,H+W] fp32,
+#      attention_backward(dattn, attn, q, k) -> (dq, dk)
+def _qk_format(q: Tensor) -> torch.memory_format:
+    B, Cq, H, W = q.shape
+    return torch.channels_last if F_.attention_tc_eligible(B, Cq, H, W, q.dtype) else torch.contiguous_format
+
+
+@torch.library.custom_op("cca::attention", mutates_args=(), device_types="cuda")
+def attention(q: Tensor, k: Tensor, impl: str = "auto") -> Tensor:
+    return F_.cca_attention_forward(q, k, impl)
+
+
+@attention.register_fake
+def _(q, k, impl="auto"):
+    B, _, H, W = q.shape
+    return q.new_empty((B, H, W, H + W), dtype=torch.float32)
+
+
+@torch.library.custom_op("cca::attention_backward", mutates_args=(), device_types="cuda")
+def attention_backward(dattn: Tensor, attn: Tensor, q: Tensor, k: Tensor, impl: str = "auto") -> Tuple[Tensor, Tensor]:
+    return F_.cca_attention_backward(dattn, attn, q, k, impl)
+
+
+@attention_backward.register_fake
+def _(dattn, attn, q, k, impl="auto"):
+    fmt = torch.channels_last if impl != "simt" and _qk_format(q) == torch.channels_last else torch.contiguous_format
+    mk = lambda t: torch.empty(t.shape, dtype=t.dtype, device=t.device).contiguous(memory_format=fmt)
+    return mk(q), mk(k)
+
+
+def _attn_setup(ctx, inputs, output):
+    q, k, impl = inputs
+    ctx.save_for_backward(q, k, output)
+    ctx.impl = impl
+
+
+def _attn_backward(ctx, dattn):
+    q, k, attn = ctx.saved_tensors
+    dq, dk = torch.ops.cca.attention_backward(dattn.contiguous(), attn, q, k, ctx.impl)
+    return dq, dk, None
+
+
+attention.register_autograd(_attn_backward, setup_context=_attn_setup)

@@ -179,6 +179,26 @@ CCA_API int cca_b200_qkv_project_wgrad_ex(const float *x, const float *dq, const
                                           void *workspace, size_t workspace_bytes, unsigned flags, void *cuda_stream);
 
 /*
+ * The attention map of one step (functions.py:40, the softmax output `concate`) and its gradient:
+ *   attn[b,h,w,g] = a of the forward above: g < H the weight of column key (g, w) (0 at g == h), g >= H the weight of row
+ *                   key (h, g - H).  Always fp32, contiguous [B,H,W,H+W], for every dtype of q, k.
+ *   backward: rho[p] = sum_j attn[p,j] dattn[p,j],  dS = attn * (dattn - rho),  dq[p] = sum_j dS[p,j] k[key j],
+ *             dk[key] = sum_p dS[p,key] q[p]   (attn and dattn are read, S and lse are not recomputed).
+ * q, k (and dq, dk) are [B,Cq,H,W] NCHW (generic kernels, any Cq and line length) or channels-last with CCA_FLAG_NHWC
+ * (tensor-core kernels: Cq in {16,32,48,64}, H and W up to 896, any C).  Flags as for cca_b200_forward; the forward is
+ * deterministic in every mode, the backward with one tile per line and with CCA_FLAG_DETERMINISTIC (fp32 on tiled lines;
+ * 16-bit I/O there returns CCA_ERR_UNSUPPORTED).  The map holds B*H*W*(H+W) floats: indices into it are 64-bit.  attn and
+ * dattn need only the alignment of a float (views at any element offset are fine).
+ */
+CCA_API int cca_b200_attention_tc_supported(int B, int Cq, int H, int W, int dtype);
+CCA_API size_t cca_b200_attention_workspace_bytes(int backward, int B, int Cq, int H, int W, int dtype, unsigned flags);
+CCA_API int cca_b200_attention_forward(const void *q, const void *k, float *attn, void *workspace, size_t workspace_bytes,
+                                       int B, int Cq, int H, int W, int dtype, unsigned flags, void *cuda_stream);
+CCA_API int cca_b200_attention_backward(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk,
+                                        void *workspace, size_t workspace_bytes, int B, int Cq, int H, int W, int dtype,
+                                        unsigned flags, void *cuda_stream);
+
+/*
  * Host-buffer variants: same maths, pointers are HOST memory (pinned or pageable).
  * They allocate device memory, copy in, run on an internal stream, copy out, free and
  * synchronise.  These are the calls a non-CUDA host language binds directly.
