@@ -3,4 +3,4 @@
 Put this repository ahead of the reference on ``sys.path`` and ``networks/ccnet.py:13``
 (``from cc_attention import CrissCrossAttention``) picks up this repository's operator unchanged.
 """
-from ccnet_b200.module import CrissCrossAttention  # noqa: F401
+from ccnet_b200.module import CrissCrossAttention, CrissCrossAttention3D  # noqa: F401

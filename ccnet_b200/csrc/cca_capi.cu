@@ -375,6 +375,115 @@ int cca_b200_attention_backward(const float *dattn, const float *attn, const voi
 }
 
 // ---------------------------------------------------------------------------------------
+// criss-cross attention over clips (the 3D op): tensor-core path (cca_tc_time.cu) or generic kernels (cca_simt_3d.cu)
+// ---------------------------------------------------------------------------------------
+namespace {
+int check_dims3d(int B, int Cq, int C, int T, int H, int W, int dtype)
+{
+    if (T <= 0) return fail(CCA_ERR_INVALID, "non-positive dimension%s%s");
+    if ((long long)B * T >= (1ll << 31)) return fail(CCA_ERR_UNSUPPORTED, "tensor too large%s%s");
+    return check_dims(B * T, Cq, C, H, W, dtype);
+}
+bool det3d_planes(Dims3 d, int dtype, unsigned flags)
+{
+    return (flags & CCA_FLAG_DETERMINISTIC) && (flags & CCA_FLAG_NHWC) && dtype == CCA_F32 && tc::shape_fits(d.frames(), dtype);
+}
+// which family runs (after the dimension checks): 1 tensor cores, 0 generic kernels, < 0 an error status
+int family3d(Dims3 d, int dtype, unsigned flags)
+{
+    if ((flags & CCA_FLAG_FORCE_SIMT) && (flags & CCA_FLAG_FORCE_TC))
+        return fail(CCA_ERR_INVALID, "FORCE_SIMT and FORCE_TC are exclusive%s%s");
+    int rc = check_device();
+    if (rc) return rc;
+    const bool nhwc = (flags & CCA_FLAG_NHWC) != 0;
+    const bool tc_ok = nhwc && tc3d_supported(d, dtype);
+    if ((flags & CCA_FLAG_FORCE_TC) && !tc_ok)
+        return fail(CCA_ERR_UNSUPPORTED, "tensor-core 3D op needs CCA_FLAG_NHWC and a covered shape%s%s");
+    if (nhwc && (!tc_ok || (flags & CCA_FLAG_FORCE_SIMT)))
+        return fail(CCA_ERR_UNSUPPORTED, "channels-last tensors are only handled by the tensor-core kernels; pass NCDHW%s%s");
+    if (tc_ok) {
+        if ((flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d.frames()) && dtype != CCA_F32) return fail(CCA_ERR_UNSUPPORTED, kDetHalfMsg);
+        return 1;
+    }
+    if (!simt3d_supported(d)) return fail(CCA_ERR_UNSUPPORTED, "H + W + T - 2 above 2048 for the generic 3D kernels%s%s");
+    return 0;
+}
+}  // namespace
+
+int cca_b200_tc3d_supported(int which, int B, int Cq, int C, int T, int H, int W, int dtype)
+{
+    (void)which;                              // (forward and backward cover the same shapes)
+    if (B <= 0 || T <= 0 || check_dims3d(B, Cq, C, T, H, W, dtype)) return 0;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && device_major() != 9) return 0;   // (no device at all: shape answer only)
+    return tc3d_supported(Dims3{B, Cq, C, T, H, W}, dtype) ? 1 : 0;
+}
+
+// one size that covers whichever family runs (as cca_b200_workspace_bytes_ex does in 2D)
+size_t cca_b200_workspace_bytes3d(int which, int B, int Cq, int C, int T, int H, int W, int dtype, unsigned flags)
+{
+    if (B <= 0 || Cq <= 0 || C <= 0 || T <= 0 || H <= 0 || W <= 0 || (long long)B * T >= (1ll << 31)) return 0;
+    const Dims3 d{B, Cq, C, T, H, W};
+    const size_t tcb = (which == CCA_WS_FORWARD ? tc_forward3d_workspace(d) : tc_backward3d_workspace(d)) +
+                       (det3d_planes(d, dtype, flags) ? tc_planes_bytes(which, d.frames()) : 0);
+    const size_t simt = simt3d_workspace(which, d);
+    return tcb > simt ? tcb : simt;
+}
+
+int cca_b200_forward3d(const void *q, const void *k, const void *v, void *out, float *lse, void *ws, size_t ws_bytes,
+                       int B, int Cq, int C, int T, int H, int W, int dtype, unsigned flags, void *stream)
+{
+    int rc = check_dims3d(B, Cq, C, T, H, W, dtype);
+    if (rc) return rc;
+    if (!q || !k || !v || !out || !lse || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
+    if (ws_bytes < cca_b200_workspace_bytes3d(CCA_WS_FORWARD, B, Cq, C, T, H, W, dtype, flags))
+        return fail(CCA_ERR_WORKSPACE, "forward workspace too small%s%s");
+    const Dims3 d{B, Cq, C, T, H, W};
+    const int fam = family3d(d, dtype, flags);
+    if (fam < 0) return fam;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (fam == 0) {
+        cudaError_t e = simt_forward3d(q, k, v, out, lse, d, dtype, st);
+        return e != cudaSuccess ? cuda_fail(e, "simt_forward3d") : CCA_OK;
+    }
+    if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
+         reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(ws)) & 15)
+        return fail(CCA_ERR_INVALID, "tensor-core path needs 16-byte aligned tensors%s%s");
+    const char *why = "";
+    const bool det = (flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d.frames());
+    cudaError_t e = tc_forward3d(q, k, v, out, lse, ws, d, dtype, st, &why, det);
+    return e != cudaSuccess ? cuda_fail(e, why && *why ? why : "tc_forward3d") : CCA_OK;
+}
+
+int cca_b200_backward3d(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
+                        void *dq, void *dk, void *dv, void *ws, size_t ws_bytes, int B, int Cq, int C, int T, int H, int W,
+                        int dtype, unsigned flags, void *stream)
+{
+    int rc = check_dims3d(B, Cq, C, T, H, W, dtype);
+    if (rc) return rc;
+    if (!dout || !q || !k || !v || !out || !lse || !dq || !dk || !dv || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
+    if (ws_bytes < cca_b200_workspace_bytes3d(CCA_WS_BACKWARD, B, Cq, C, T, H, W, dtype, flags))
+        return fail(CCA_ERR_WORKSPACE, "backward workspace too small%s%s");
+    const Dims3 d{B, Cq, C, T, H, W};
+    const int fam = family3d(d, dtype, flags);
+    if (fam < 0) return fam;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (fam == 0) {
+        if (reinterpret_cast<uintptr_t>(ws) & 3) return fail(CCA_ERR_INVALID, "workspace must be 4-byte aligned%s%s");
+        cudaError_t e = simt_backward3d(dout, q, k, v, out, lse, dq, dk, dv, ws, d, dtype, st);
+        return e != cudaSuccess ? cuda_fail(e, "simt_backward3d") : CCA_OK;
+    }
+    if ((reinterpret_cast<uintptr_t>(dout) | reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) |
+         reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(dq) |
+         reinterpret_cast<uintptr_t>(dk) | reinterpret_cast<uintptr_t>(dv) | reinterpret_cast<uintptr_t>(ws)) & 15)
+        return fail(CCA_ERR_INVALID, "tensor-core path needs 16-byte aligned tensors%s%s");
+    const char *why = "";
+    const bool det = (flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d.frames());
+    cudaError_t e = tc_backward3d(dout, q, k, v, out, lse, dq, dk, dv, ws, d, dtype, st, &why, det);
+    return e != cudaSuccess ? cuda_fail(e, why && *why ? why : "tc_backward3d") : CCA_OK;
+}
+
+// ---------------------------------------------------------------------------------------
 // 1x1 Q/K/V projections (functions.py:29,32,35) as tensor-core GEMMs on the channels-last view
 // ---------------------------------------------------------------------------------------
 int cca_b200_qkv_supported(int C, int Cq)

@@ -12,6 +12,11 @@ namespace cca {
 struct Dims {
     int B, Cq, C, H, W;
 };
+// a batch of clips [B, C, T, H, W] (the 3D op, cca_tc_time.cu); frames(): the [B*T, C, H, W] view of its frames
+struct Dims3 {
+    int B, Cq, C, T, H, W;
+    Dims frames() const { return Dims{B * T, Cq, C, H, W}; }
+};
 
 // A "line" is one image row (row branch) or one image column (column branch) of a sample.
 // Element (channel c, position j) of the line lives at  c*cs + base + j*sj  inside the sample.
@@ -47,6 +52,10 @@ size_t tc_forward_workspace(Dims d);
 // det: planes mode on tiled lines (fp32 only; the workspace then has tc_planes_bytes more at its end)
 cudaError_t tc_forward(const void *q, const void *k, const void *v, void *out, float *lse, void *ws,
                        Dims d, int dtype, cudaStream_t st, const char **why, bool det = false);
+// values pass alone (tc_forward = tc_stats + tc_values): the final lse combines the statistics pass's planes and extra_parts
+// more planes of `parts`; `planes` is the planes-mode buffer (det on tiled lines)
+cudaError_t tc_values(const void *q, const void *k, const void *v, void *out, float *lse, const float *parts, unsigned int *cdone,
+                      void *planes, Dims d, int dtype, cudaStream_t st, const char **why, bool det, int extra_parts);
 // statistics pre-pass of the tensor-core forward (cca_tc_stats.cu): partial lse planes; also clears a byte range and counters
 cudaError_t tc_stats(const void *q, const void *k, float *parts, void *zero_ptr, long zero_bytes, unsigned int *counters,
                      int n_counters, Dims d, int dtype, cudaStream_t st, const char **why);
@@ -55,7 +64,7 @@ cudaError_t tc_stats(const void *q, const void *k, float *parts, void *zero_ptr,
 bool tc_tiled(Dims d);                          // a line longer than one tile in either direction
 size_t tc_planes_bytes(int which, Dims d);      // plane workspace (0 on one-tile shapes)
 cudaError_t tc_forward_planes(const void *q, const void *k, const void *v, float *out, float *lse, const float *parts,
-                              unsigned int *cdone, void *planes, Dims d, cudaStream_t st, const char **why);
+                              unsigned int *cdone, void *planes, Dims d, cudaStream_t st, const char **why, int extra_parts = 0);
 cudaError_t tc_backward_planes(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
                                float *delta, unsigned int *counters, float *dq, float *dk, float *dv, void *planes, Dims d,
                                int delta_mode, cudaStream_t st, const char **why);
@@ -65,6 +74,25 @@ size_t tc_backward_workspace(Dims d);
 cudaError_t tc_backward(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
                         void *dq, void *dk, void *dv, void *ws, Dims d, int dtype, cudaStream_t st, const char **why,
                         bool det = false);
+
+// the 3D op over clips (criss-cross attention along H, W and T; cca_tc_time.cu): the H and W branches are the 2D kernels on
+// the frames view of NDHWC tensors, the time branch has kernels of its own.  T up to kTimeMaxT.
+constexpr int kTimeMaxT = 32;
+bool tc3d_supported(Dims3 d, int dtype);
+size_t tc_forward3d_workspace(Dims3 d);
+size_t tc_backward3d_workspace(Dims3 d);
+cudaError_t tc_forward3d(const void *q, const void *k, const void *v, void *out, float *lse, void *ws, Dims3 d, int dtype,
+                         cudaStream_t st, const char **why, bool det);
+//   generic kernels, NCDHW tensors of any Cq and C (cca_simt_3d.cu): one warp per pixel, its H + W + T - 2 keys in shared
+//   memory, so H + W + T - 2 <= kMaxKeys3d; the backward's workspace is delta [B*T*H*W]
+constexpr int kMaxKeys3d = 2048;
+bool simt3d_supported(Dims3 d);
+size_t simt3d_workspace(int which, Dims3 d);
+cudaError_t simt_forward3d(const void *q, const void *k, const void *v, void *out, float *lse, Dims3 d, int dtype, cudaStream_t st);
+cudaError_t simt_backward3d(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
+                            void *dq, void *dk, void *dv, void *ws, Dims3 d, int dtype, cudaStream_t st);
+cudaError_t tc_backward3d(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
+                          void *dq, void *dk, void *dv, void *ws, Dims3 d, int dtype, cudaStream_t st, const char **why, bool det);
 
 // the attention map attn[B,H,W,H+W] (fp32) and its gradient w.r.t. q, k (Dims.C is not used)
 //   generic kernels, NCHW q, k (cca_simt_attn.cu); the backward's workspace is rho [B*H*W]

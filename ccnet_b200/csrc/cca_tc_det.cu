@@ -9,9 +9,9 @@ namespace cca {
 namespace tc {
 
 template cudaError_t launch_fwd<80, float, true>(const void *, const void *, const void *, void *, float *, const float *,
-                                                 unsigned int *, Dims, cudaStream_t, const char **);
+                                                 unsigned int *, Dims, cudaStream_t, const char **, int);
 template cudaError_t launch_fwd<112, float, true>(const void *, const void *, const void *, void *, float *, const float *,
-                                                  unsigned int *, Dims, cudaStream_t, const char **);
+                                                  unsigned int *, Dims, cudaStream_t, const char **, int);
 template cudaError_t launch_bwd<80, float, true>(const void *, const void *, const void *, const void *, const void *, const float *,
                                                  float *, unsigned int *, void *, void *, void *, Dims, int, cudaStream_t,
                                                  const char **);
@@ -90,13 +90,13 @@ size_t tc_planes_bytes(int which, Dims d)
 }
 
 cudaError_t tc_forward_planes(const void *q, const void *k, const void *v, float *out, float *lse, const float *parts,
-                              unsigned int *cdone, void *planes, Dims d, cudaStream_t st, const char **why)
+                              unsigned int *cdone, void *planes, Dims d, cudaStream_t st, const char **why, int extra_parts)
 {
     const ItemSpace sp = make_space(d.B, d.H, d.W);
     const int lk = lk_for(max_tile(sp));
     float *po = reinterpret_cast<float *>((reinterpret_cast<uintptr_t>(planes) + 255) & ~(uintptr_t)255);
-    cudaError_t e = lk == 80 ? launch_fwd<80, float, true>(q, k, v, po, lse, parts, cdone, d, st, why)
-                             : launch_fwd<112, float, true>(q, k, v, po, lse, parts, cdone, d, st, why);
+    cudaError_t e = lk == 80 ? launch_fwd<80, float, true>(q, k, v, po, lse, parts, cdone, d, st, why, extra_parts)
+                             : launch_fwd<112, float, true>(q, k, v, po, lse, parts, cdone, d, st, why, extra_parts);
     if (e != cudaSuccess) return e;
     const float *src[1] = {po};
     float *dst[1] = {out};

@@ -26,18 +26,24 @@ cudaError_t tc_forward(const void *q, const void *k, const void *v, void *out, f
     // statistics; it also clears the per-sample counters of the values kernel
     cudaError_t e = tc_stats(q, k, parts, nullptr, 0, cdone, d.B, d, dtype, st, why);
     if (e != cudaSuccess) return e;
+    return tc_values(q, k, v, out, lse, parts, cdone, reinterpret_cast<uint8_t *>(ws) + tc_forward_workspace(d), d, dtype, st,
+                     why, det, 0);
+}
+
+cudaError_t tc_values(const void *q, const void *k, const void *v, void *out, float *lse, const float *parts, unsigned int *cdone,
+                      void *planes, Dims d, int dtype, cudaStream_t st, const char **why, bool det, int extra_parts)
+{
     if (det && tc_tiled(d))       // (fp32: cca_capi.cu refuses 16-bit I/O here)
-        return tc_forward_planes(q, k, v, reinterpret_cast<float *>(out), lse, parts, cdone,
-                                 reinterpret_cast<uint8_t *>(ws) + tc_forward_workspace(d), d, st, why);
-    const int lk = lk_for(max_tile(sp));
+        return tc_forward_planes(q, k, v, reinterpret_cast<float *>(out), lse, parts, cdone, planes, d, st, why, extra_parts);
+    const int lk = lk_for(max_tile(make_space(d.B, d.H, d.W)));
     if (dtype == CCA_F16)
-        return lk == 80 ? launch_fwd<80, __half>(q, k, v, out, lse, parts, cdone, d, st, why)
-                        : launch_fwd<112, __half>(q, k, v, out, lse, parts, cdone, d, st, why);
+        return lk == 80 ? launch_fwd<80, __half>(q, k, v, out, lse, parts, cdone, d, st, why, extra_parts)
+                        : launch_fwd<112, __half>(q, k, v, out, lse, parts, cdone, d, st, why, extra_parts);
     if (dtype == CCA_BF16)
-        return lk == 80 ? launch_fwd<80, __nv_bfloat16>(q, k, v, out, lse, parts, cdone, d, st, why)
-                        : launch_fwd<112, __nv_bfloat16>(q, k, v, out, lse, parts, cdone, d, st, why);
-    return lk == 80 ? launch_fwd<80, float>(q, k, v, out, lse, parts, cdone, d, st, why)
-                    : launch_fwd<112, float>(q, k, v, out, lse, parts, cdone, d, st, why);
+        return lk == 80 ? launch_fwd<80, __nv_bfloat16>(q, k, v, out, lse, parts, cdone, d, st, why, extra_parts)
+                        : launch_fwd<112, __nv_bfloat16>(q, k, v, out, lse, parts, cdone, d, st, why, extra_parts);
+    return lk == 80 ? launch_fwd<80, float>(q, k, v, out, lse, parts, cdone, d, st, why, extra_parts)
+                    : launch_fwd<112, float>(q, k, v, out, lse, parts, cdone, d, st, why, extra_parts);
 }
 
 }  // namespace cca

@@ -45,9 +45,11 @@
 namespace cca {
 namespace tc {
 
+// extra_parts: planes of `parts` past the statistics pass's own (the time branch of the 3D op, cca_tc_time.cu) that the final
+// lse combines too; the item space and the planes-mode output buffer stay those of the 2D problem
 template <int LK, typename E, bool PL = false>
 cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, float *lse, const float *parts, unsigned int *cdone,
-                       Dims d, cudaStream_t st, const char **why);
+                       Dims d, cudaStream_t st, const char **why, int extra_parts = 0);
 
 struct FwdParams {
     ItemSpace sp;
@@ -345,7 +347,7 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
 // PL: `out` is the [nparts*B, H, W, C] plane buffer (cca_tc_det.cu sums it into the output)
 template <int LK, typename E, bool PL>
 cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, float *lse, const float *parts, unsigned int *cdone,
-                       Dims d, cudaStream_t st, const char **why)
+                       Dims d, cudaStream_t st, const char **why, int extra_parts)
 {
     CUtensorMap m[8];
     const void *base[4] = {q, k, v, out};
@@ -363,6 +365,7 @@ cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, f
                 return cudaErrorInvalidValue;
             }
         }
+    p.sp.nparts += extra_parts;          // (after the maps: the planes-mode output holds the 2D problem's planes only)
     p.C = d.C; p.Cq = d.Cq;
     p.npix = (long)d.B * d.H * d.W;
     p.parts = parts; p.lse = lse; p.cdone = cdone;
@@ -394,14 +397,14 @@ cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, f
 
 // The f16 instantiations live in their own translation unit (cca_tc_f16.cu).
 extern template cudaError_t launch_fwd<80, __half>(const void *, const void *, const void *, void *, float *, const float *,
-                                                   unsigned int *, Dims, cudaStream_t, const char **);
+                                                   unsigned int *, Dims, cudaStream_t, const char **, int);
 extern template cudaError_t launch_fwd<112, __half>(const void *, const void *, const void *, void *, float *, const float *,
-                                                    unsigned int *, Dims, cudaStream_t, const char **);
+                                                    unsigned int *, Dims, cudaStream_t, const char **, int);
 // The planes-mode instantiations (fp32) live in cca_tc_det.cu.
 extern template cudaError_t launch_fwd<80, float, true>(const void *, const void *, const void *, void *, float *, const float *,
-                                                        unsigned int *, Dims, cudaStream_t, const char **);
+                                                        unsigned int *, Dims, cudaStream_t, const char **, int);
 extern template cudaError_t launch_fwd<112, float, true>(const void *, const void *, const void *, void *, float *, const float *,
-                                                         unsigned int *, Dims, cudaStream_t, const char **);
+                                                         unsigned int *, Dims, cudaStream_t, const char **, int);
 
 }  // namespace tc
 }  // namespace cca

@@ -1,0 +1,341 @@
+// Criss-cross attention over clips (the 3D op): q, k [B, Cq, T, H, W], v [B, C, T, H, W] in NDHWC memory
+// (torch.channels_last_3d).  Every pixel (b, t, h, w) attends to its column (b, t, *, w; self masked), its row (b, t, h, *)
+// and its time line (b, *, h, w; self masked), one softmax over all H + W + T logits.
+//
+// In NDHWC memory the frames view [B*T, H, W, C] of a clip batch is an ordinary NHWC tensor whose pixel index is the clip's
+// pixel index, so the column and row branches are the 2D tensor-core kernels run unchanged on that view:
+//   forward : 2D statistics -> time statistics (one more partial lse plane) -> 2D values with that plane folded into the
+//             final lse (launch_fwd's extra_parts) -> time values (out += P_T V_T with the final lse)
+//   backward: 2D backward with the 3D lse and out (its P is the 3D P restricted to a row / column, its delta = <dO, out> is
+//             the 3D delta, left in its workspace) -> time backward
+// The passes are chained with programmatic dependent launch; each time kernel waits (griddepcontrol.wait) before it writes
+// or reads what an earlier pass wrote.
+//
+// Time kernels: one warp owns one T-line (the T pixels at a fixed (b, h, w)).  Lane t < T is query frame t for the T x T
+// logits, P and dS (staged in shared memory); for the products with V, dO, Q and K the lanes walk the channels.  A T-line
+// lives in one warp, so each output element gets exactly one add from the time pass: no atomics, and the result is as
+// reproducible as the 2D passes before it (CCA_FLAG_DETERMINISTIC needs no planes here).  The pass moves ~(2Cq + 3C)
+// elements per pixel for 2T(Cq + C) FLOPs, bandwidth-bound on CUDA cores, so it uses no tensor cores.  The shared memory
+// per warp grows with T * Cq; kTimeMaxT = 32 keeps the backward's four warps under 140 KB.
+#include "cca_items.cuh"
+#include "cca_tc_common.cuh"
+
+namespace cca {
+namespace tc {
+namespace {
+
+constexpr int kWarps = 4;   // T-lines per CTA
+enum TimeKind { kStats = 0, kValues = 1, kBackward = 2 };
+
+struct TimeParams {
+    const void *q, *k, *v, *dout;
+    void *out, *dq, *dk, *dv;
+    float *part;              // stats: the time plane [B*T*H*W] (log2-sum-exp2 of the T-line logits, self excluded)
+    const float *lse;         // final natural-log lse [B*T*H*W]
+    const float *delta;       // backward: <dout, out> per pixel (the 2D backward's workspace)
+    long lines;               // B*H*W
+    long hw;                  // H*W
+    int T, Cq, C;
+};
+
+// floats of shared memory per warp: Q, K [T][Cq+1]; values: + P [T][T+1]; backward: + P, dS [T][T+1], dO, V chunks [T][33]
+__host__ __device__ inline long warp_floats(int kind, int T, int Cq)
+{
+    const long qk = 2L * T * (Cq + 1), pp = (long)T * (T + 1), ch = 32L + 1;
+    return kind == kStats ? qk : kind == kValues ? qk + pp : qk + 2 * pp + 2 * T * ch;
+}
+
+// pixel of frame 0 of a T-line (b, hw); frame t is t * hw pixels further
+__device__ __forceinline__ long line_pix0(long line, const TimeParams &p)
+{
+    const long b = line / p.hw;
+    return b * p.T * p.hw + (line - b * p.hw);
+}
+
+template <typename E>
+__device__ __forceinline__ void stage_qk(const TimeParams &p, long pix0, float *qs, float *ks, int lane)
+{
+    const E *q = static_cast<const E *>(p.q), *k = static_cast<const E *>(p.k);
+    const int ld = p.Cq + 1;
+    for (int t = 0; t < p.T; ++t) {
+        const long base = (pix0 + t * p.hw) * p.Cq;
+        for (int c = lane; c < p.Cq; c += 32) {
+            qs[t * ld + c] = to_f(q[base + c]);
+            ks[t * ld + c] = to_f(k[base + c]);
+        }
+    }
+    __syncwarp();
+}
+
+// s[j] = log2e * (q_t . k_j), j < T, of query frame t
+template <int TM>
+__device__ __forceinline__ void row_logits(const TimeParams &p, const float *qs, const float *ks, int t, float (&s)[TM])
+{
+    const int ld = p.Cq + 1;
+#pragma unroll
+    for (int j = 0; j < TM; ++j) s[j] = 0.f;
+    for (int c = 0; c < p.Cq; ++c) {
+        const float a = qs[t * ld + c];
+#pragma unroll
+        for (int j = 0; j < TM; ++j)
+            if (j < p.T) s[j] = fmaf(a, ks[j * ld + c], s[j]);
+    }
+#pragma unroll
+    for (int j = 0; j < TM; ++j) s[j] *= kLog2e;
+}
+
+// lane t < T: P[t][j] = exp2(s_j - lse2_t), 0 at j == t, into pr and row t of ps
+template <int TM>
+__device__ __forceinline__ void row_probs(const TimeParams &p, const float *qs, const float *ks, long pix0, int t, float (&pr)[TM],
+                                          float *ps)
+{
+    float s[TM];
+    row_logits<TM>(p, qs, ks, t, s);
+    const float nl2 = -__ldcg(p.lse + pix0 + t * p.hw) * kLog2e;
+#pragma unroll
+    for (int j = 0; j < TM; ++j) {
+        pr[j] = j < p.T && j != t ? exp2f(s[j] + nl2) : 0.f;
+        if (j < p.T) ps[t * (p.T + 1) + j] = pr[j];
+    }
+}
+
+template <typename E> __device__ __forceinline__ void add_to(E *dst, float x) { *dst = from_f<E>(to_f(*dst) + x); }
+
+template <int TM, typename E>
+__global__ void __launch_bounds__(32 * kWarps) cca_time_stats_kernel(const __grid_constant__ TimeParams p)
+{
+    extern __shared__ float sm[];
+    pdl_launch_dependents();                  // the 2D values kernel may start its prologue; it waits for this grid
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long line = (long)blockIdx.x * kWarps + warp;
+    const bool ok = line < p.lines;
+    float *qs = sm + warp * warp_floats(kStats, p.T, p.Cq), *ks = qs + (long)p.T * (p.Cq + 1);
+    const long pix0 = ok ? line_pix0(line, p) : 0;
+    float l2 = -INFINITY;                     // (T = 1: no time key)
+    if (ok) {
+        stage_qk<E>(p, pix0, qs, ks, lane);
+        if (lane < p.T) {
+            float s[TM];
+            row_logits<TM>(p, qs, ks, lane, s);
+            float m = -INFINITY;
+#pragma unroll
+            for (int j = 0; j < TM; ++j)
+                if (j < p.T && j != lane) m = fmaxf(m, s[j]);
+            if (m > -INFINITY) {
+                float sum = 0.f;
+#pragma unroll
+                for (int j = 0; j < TM; ++j)
+                    if (j < p.T && j != lane) sum += exp2f(s[j] - m);
+                l2 = m + log2f(sum);
+            }
+        }
+    }
+    pdl_wait();                               // the 2D statistics grid has completed: the values kernel waits for this one only
+    if (ok && lane < p.T) p.part[pix0 + lane * p.hw] = l2;
+}
+
+template <int TM, typename E>
+__global__ void __launch_bounds__(32 * kWarps) cca_time_values_kernel(const __grid_constant__ TimeParams p)
+{
+    extern __shared__ float sm[];
+    pdl_wait();                               // out (stored / added by the 2D values kernel) and the final lse
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long line = (long)blockIdx.x * kWarps + warp;
+    if (line >= p.lines) return;
+    float *qs = sm + warp * warp_floats(kValues, p.T, p.Cq), *ks = qs + (long)p.T * (p.Cq + 1), *ps = ks + (long)p.T * (p.Cq + 1);
+    const long pix0 = line_pix0(line, p);
+    stage_qk<E>(p, pix0, qs, ks, lane);
+    if (lane < p.T) {
+        float pr[TM];
+        row_probs<TM>(p, qs, ks, pix0, lane, pr, ps);
+    }
+    __syncwarp();
+    const E *v = static_cast<const E *>(p.v);
+    E *out = static_cast<E *>(p.out);
+    const int lt = p.T + 1;
+    const long fs = p.hw * p.C;               // elements from one frame to the next
+    v += pix0 * p.C;
+    out += pix0 * p.C;
+    for (int c = lane; c < p.C; c += 32) {
+        float vr[TM];
+#pragma unroll
+        for (int j = 0; j < TM; ++j) vr[j] = j < p.T ? to_f(v[j * fs + c]) : 0.f;
+        for (int t = 0; t < p.T; ++t) {
+            float a = 0.f;
+#pragma unroll
+            for (int j = 0; j < TM; ++j)
+                if (j < p.T) a = fmaf(ps[t * lt + j], vr[j], a);
+            add_to(out + t * fs + c, a);
+        }
+    }
+}
+
+template <int TM, typename E>
+__global__ void __launch_bounds__(32 * kWarps) cca_time_bwd_kernel(const __grid_constant__ TimeParams p)
+{
+    extern __shared__ float sm[];
+    pdl_wait();                               // dq, dk, dv (written by the 2D backward) and its delta
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long line = (long)blockIdx.x * kWarps + warp;
+    if (line >= p.lines) return;
+    const int T = p.T, ld = p.Cq + 1, lt = T + 1;
+    float *qs = sm + warp * warp_floats(kBackward, T, p.Cq), *ks = qs + (long)T * ld, *ps = ks + (long)T * ld, *ds = ps + T * lt;
+    float *gs = ds + T * lt, *vs = gs + T * 33;
+    const long pix0 = line_pix0(line, p), hw = p.hw;
+    stage_qk<E>(p, pix0, qs, ks, lane);
+    float pr[TM], dp[TM];
+#pragma unroll
+    for (int j = 0; j < TM; ++j) dp[j] = 0.f;
+    if (lane < T) row_probs<TM>(p, qs, ks, pix0, lane, pr, ps);
+    __syncwarp();
+    // 32 channels at a time: dv[s] += sum_t P[t][s] dO[t] (lane = channel), dP[t][s] += dO[t] . v[s] (lane = frame t)
+    const E *dO = static_cast<const E *>(p.dout), *v = static_cast<const E *>(p.v);
+    E *dv = static_cast<E *>(p.dv);
+    for (int c0 = 0; c0 < p.C; c0 += 32) {
+        const int c = c0 + lane;              // (C % 64 == 0 on this path)
+        for (int t = 0; t < T; ++t) {
+            const long e = (pix0 + t * hw) * p.C + c;
+            gs[t * 33 + lane] = to_f(dO[e]);
+            vs[t * 33 + lane] = to_f(v[e]);
+        }
+        __syncwarp();
+        for (int s = 0; s < T; ++s) {
+            float a = 0.f;
+            for (int t = 0; t < T; ++t) a = fmaf(ps[t * lt + s], gs[t * 33 + lane], a);
+            add_to(dv + (pix0 + s * hw) * p.C + c, a);
+        }
+        if (lane < T)
+            for (int cc = 0; cc < 32; ++cc) {
+                const float g = gs[lane * 33 + cc];
+#pragma unroll
+                for (int j = 0; j < TM; ++j)
+                    if (j < T) dp[j] = fmaf(g, vs[j * 33 + cc], dp[j]);
+            }
+        __syncwarp();
+    }
+    // dS = P (dP - delta)
+    if (lane < T) {
+        const float dl = __ldcg(p.delta + pix0 + lane * hw);
+#pragma unroll
+        for (int j = 0; j < TM; ++j)
+            if (j < T) ds[lane * lt + j] = pr[j] * (dp[j] - dl);
+    }
+    __syncwarp();
+    // dq[t] += sum_s dS[t][s] k[s],  dk[s] += sum_t dS[t][s] q[t]   (lane = channel)
+    E *dq = static_cast<E *>(p.dq), *dk = static_cast<E *>(p.dk);
+    for (int c = lane; c < p.Cq; c += 32)
+        for (int t = 0; t < T; ++t) {
+            float a = 0.f, b = 0.f;
+            for (int j = 0; j < T; ++j) {
+                a = fmaf(ds[t * lt + j], ks[j * ld + c], a);
+                b = fmaf(ds[j * lt + t], qs[j * ld + c], b);
+            }
+            add_to(dq + (pix0 + t * hw) * p.Cq + c, a);
+            add_to(dk + (pix0 + t * hw) * p.Cq + c, b);
+        }
+}
+
+template <int TM, typename E> cudaError_t launch_time_tm(int kind, const TimeParams &p, cudaStream_t st)
+{
+    void (*kern)(TimeParams) = kind == kStats    ? cca_time_stats_kernel<TM, E>
+                               : kind == kValues ? cca_time_values_kernel<TM, E>
+                                                 : cca_time_bwd_kernel<TM, E>;
+    const size_t smem = (size_t)kWarps * warp_floats(kind, p.T, p.Cq) * sizeof(float);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)((p.lines + kWarps - 1) / kWarps)); cfg.blockDim = dim3(32 * kWarps);
+    cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = tc_pdl() ? 1 : 0;
+    e = cudaLaunchKernelEx(&cfg, kern, p);
+    count_launch();
+    return e != cudaSuccess ? e : cudaGetLastError();
+}
+
+template <typename E> cudaError_t launch_time_e(int kind, const TimeParams &p, cudaStream_t st)
+{
+    if (p.T <= 8) return launch_time_tm<8, E>(kind, p, st);
+    if (p.T <= 16) return launch_time_tm<16, E>(kind, p, st);
+    return launch_time_tm<kTimeMaxT, E>(kind, p, st);
+}
+
+cudaError_t launch_time(int kind, const TimeParams &p, int dtype, cudaStream_t st)
+{
+    if (dtype == CCA_F16) return launch_time_e<__half>(kind, p, st);
+    if (dtype == CCA_BF16) return launch_time_e<__nv_bfloat16>(kind, p, st);
+    return launch_time_e<float>(kind, p, st);
+}
+
+TimeParams time_params(Dims3 d)
+{
+    TimeParams p = {};
+    p.lines = (long)d.B * d.H * d.W;
+    p.hw = (long)d.H * d.W;
+    p.T = d.T; p.Cq = d.Cq; p.C = d.C;
+    return p;
+}
+
+// partial lse planes of the 3D forward: the frames view's 2D planes, then the time plane
+size_t parts3d_bytes(Dims3 d)
+{
+    const Dims f = d.frames();
+    const size_t npix = (size_t)f.B * f.H * f.W;
+    return ((size_t)(make_space(f.B, f.H, f.W).nparts + 1) * npix * sizeof(float) + 15) & ~(size_t)15;
+}
+
+}  // namespace
+}  // namespace tc
+
+using namespace tc;
+
+bool tc3d_supported(Dims3 d, int dtype)
+{
+    return d.T >= 1 && d.T <= kTimeMaxT && (long)d.B * d.T < (1L << 31) && shape_supported(d.frames(), dtype);
+}
+
+// Workspace of the 3D forward: [nparts + 1][B*T*H*W] fp32 partial lse planes, then [B*T] per-frame counters of the values
+// kernel (planes mode: tc_planes_bytes of the frames view follow).
+size_t tc_forward3d_workspace(Dims3 d)
+{
+    return parts3d_bytes(d) + (((size_t)d.B * d.T * sizeof(unsigned int) + 15) & ~(size_t)15);
+}
+
+// Workspace of the 3D backward: that of the 2D backward on the frames view (delta first)
+size_t tc_backward3d_workspace(Dims3 d) { return tc_backward_workspace(d.frames()); }
+
+cudaError_t tc_forward3d(const void *q, const void *k, const void *v, void *out, float *lse, void *ws, Dims3 d, int dtype,
+                         cudaStream_t st, const char **why, bool det)
+{
+    const Dims f = d.frames();
+    const long npix = (long)f.B * f.H * f.W;
+    float *parts = reinterpret_cast<float *>(ws);
+    unsigned int *cdone = reinterpret_cast<unsigned int *>(reinterpret_cast<uint8_t *>(ws) + parts3d_bytes(d));
+    cudaError_t e = tc_stats(q, k, parts, nullptr, 0, cdone, f.B, f, dtype, st, why);
+    if (e != cudaSuccess) return e;
+    TimeParams p = time_params(d);
+    p.q = q; p.k = k; p.v = v; p.out = out; p.lse = lse;
+    p.part = parts + (long)make_space(f.B, f.H, f.W).nparts * npix;
+    if ((e = launch_time(kStats, p, dtype, st)) != cudaSuccess) return e;
+    e = tc_values(q, k, v, out, lse, parts, cdone, reinterpret_cast<uint8_t *>(ws) + tc_forward3d_workspace(d), f, dtype, st, why,
+                  det, 1);
+    if (e != cudaSuccess) return e;
+    return launch_time(kValues, p, dtype, st);
+}
+
+cudaError_t tc_backward3d(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
+                          void *dq, void *dk, void *dv, void *ws, Dims3 d, int dtype, cudaStream_t st, const char **why, bool det)
+{
+    cudaError_t e = tc_backward(dout, q, k, v, out, lse, dq, dk, dv, ws, d.frames(), dtype, st, why, det);
+    if (e != cudaSuccess) return e;
+    TimeParams p = time_params(d);
+    p.q = q; p.k = k; p.v = v; p.dout = dout; p.lse = lse;
+    p.dq = dq; p.dk = dk; p.dv = dv;
+    p.delta = reinterpret_cast<const float *>(ws);      // (tc_backward leaves delta at the start of its workspace)
+    return launch_time(kBackward, p, dtype, st);
+}
+
+}  // namespace cca

@@ -424,3 +424,147 @@ def cca_attention(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", determin
     """Differentiable attention map attn[B,H,W,H+W] (float32) of one criss-cross step; the gradient flows to q and k.
     ``deterministic``: as for ``cca``; the mode is fixed when the forward runs and the backward uses it too."""
     return _CCAAttentionFunction.apply(q, k, impl, _resolve_deterministic(deterministic))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# criss-cross attention over clips (the 3D op): column, row and time branches under one softmax
+# ---------------------------------------------------------------------------------------------------------------------
+def _check_inputs3d(q, k, v):
+    if not (q.is_cuda and k.is_cuda and v.is_cuda):
+        raise RuntimeError("ccnet_b200: criss-cross attention needs CUDA tensors on an H100 (sm_90) "
+                           "(there is no CPU path in this package)")
+    if q.dtype not in _DTYPES or k.dtype != q.dtype or v.dtype != q.dtype:
+        raise RuntimeError(f"ccnet_b200: q,k,v must share dtype float32, bfloat16 or float16, got "
+                           f"{q.dtype},{k.dtype},{v.dtype}")
+    if q.dim() != 5 or k.shape != q.shape or v.dim() != 5 or v.shape[0] != q.shape[0] or v.shape[2:] != q.shape[2:]:
+        raise RuntimeError(f"ccnet_b200: expected q,k [B,Cq,T,H,W] and v [B,C,T,H,W], got "
+                           f"{tuple(q.shape)},{tuple(k.shape)},{tuple(v.shape)}")
+    if not (q.device == k.device == v.device):
+        raise RuntimeError("ccnet_b200: q,k,v must be on the same device")
+
+
+def tc3d_eligible(B: int, Cq: int, C: int, T: int, H: int, W: int, dtype: torch.dtype) -> bool:
+    """True if the 3D op's kernels cover this problem (the 2D tensor-core shapes for B*T frames, 1 <= T <= 32)."""
+    return dtype in _DTYPES and capi.load().cca_b200_tc3d_supported(capi.CCA_WS_FORWARD, B, Cq, C, T, H, W, _DTYPES[dtype]) == 1
+
+
+def _setup3d(q, v, impl, det):
+    """(lib, dims, dtype code, flags, use_tc) of a 3D call: the tensor-core path where it covers the shape and ``impl`` allows
+    it, else the generic kernels"""
+    lib = capi.load()
+    B, Cq, T, H, W = q.shape
+    C = v.shape[1]
+    dt = _DTYPES[q.dtype]
+    use_tc = impl in ("auto", "tc") and lib.cca_b200_tc3d_supported(capi.CCA_WS_FORWARD, B, Cq, C, T, H, W, dt) == 1
+    if impl == "tc" and not use_tc:
+        raise RuntimeError(f"ccnet_b200: tensor-core kernels do not cover q{tuple(q.shape)} v{tuple(v.shape)} {q.dtype}")
+    flags = _IMPL_FLAGS[impl] | (capi.CCA_FLAG_NHWC if use_tc else 0) | (capi.CCA_FLAG_DETERMINISTIC if det else 0)
+    return lib, (B, Cq, C, T, H, W), dt, flags, use_tc
+
+
+def _upcast3d(dtype, T: int, H: int, W: int, deterministic: bool) -> bool:
+    """16-bit calls of the 3D tensor-core path that run on the fp32 kernels, rounded to the 16-bit type once: those of
+    ``_half_long_lines``, and bf16 with T > 1.  The time pass adds onto out, dq, dk and dv after the 2D passes have rounded
+    them to the I/O type, a third rounding of every output element; in bf16 that puts the emulated floor at up to 0.73 of
+    the 1e-2 budget (tests/test_cca3d_host.py), in fp16 at a third of its budget.  CCA_B200_BF16_NATIVE=1 keeps the native
+    kernels, as in 2D.  At T = 1 the time pass adds nothing and the native kernels give the 2D op's bits."""
+    import os
+    return _half_long_lines(dtype, H, W, deterministic) or (
+        dtype == torch.bfloat16 and T > 1 and not os.environ.get("CCA_B200_BF16_NATIVE"))
+
+
+def _sample_groups3d(lib, which, dims, dt, flags):
+    """``_sample_groups`` of the 3D op: clip slices whose plane workspace stays under ``deterministic_workspace_cap``"""
+    B = dims[0]
+    if not flags & capi.CCA_FLAG_DETERMINISTIC:
+        return [(0, B)]
+    per_clip = (lib.cca_b200_workspace_bytes3d(which, 1, *dims[1:], dt, flags)
+                - lib.cca_b200_workspace_bytes3d(which, 1, *dims[1:], dt, flags & ~capi.CCA_FLAG_DETERMINISTIC))
+    g = max(1, deterministic_workspace_cap // per_clip) if per_clip > 0 else B
+    return [(b0, min(B, b0 + g)) for b0 in range(0, B, g)]
+
+
+def cca3d_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", deterministic=None):
+    """Criss-cross attention over clips: returns (out[B,C,T,H,W], lse[B,T,H,W] fp32).  q, k are [B,Cq,T,H,W], v [B,C,T,H,W].
+    Pixel (b,t,h,w) attends to its column (self masked), its row and its time line (self masked), one softmax over the
+    H + W + T logits.  At T = 1 this is ``cca_forward`` on every frame.
+
+    ``impl``: "auto" (the tensor-core path where ``tc3d_eligible``, else the generic kernels), "tc" (tensor-core path or
+    error), "simt" (generic kernels: any Cq and C, H + W + T - 2 <= 2048).  The tensor-core path works on channels_last_3d
+    memory (inputs in another format are converted, the output is channels_last_3d), the generic kernels on contiguous
+    NCDHW memory.  ``deterministic`` as for ``cca_forward``."""
+    _check_inputs3d(q, k, v)
+    det = _resolve_deterministic(deterministic)
+    lib, dims, dt, flags, use_tc = _setup3d(q, v, impl, det)
+    B, Cq, C, T, H, W = dims
+    if use_tc and _upcast3d(q.dtype, T, H, W, det):
+        out32, lse = cca3d_forward(q.float(), k.float(), v.float(), impl, det)
+        return out32.to(q.dtype), lse
+    fmt = torch.channels_last_3d if use_tc else torch.contiguous_format
+    q, k, v = (t.contiguous(memory_format=fmt) for t in (q, k, v))
+    with torch.cuda.device(q.device):
+        out = torch.empty_like(v, memory_format=fmt)
+        lse = torch.empty((B, T, H, W), dtype=torch.float32, device=q.device)
+        for b0, b1 in _sample_groups3d(lib, capi.CCA_WS_FORWARD, dims, dt, flags):
+            n = b1 - b0
+            ws = _workspace(lib.cca_b200_workspace_bytes3d(capi.CCA_WS_FORWARD, n, *dims[1:], dt, flags), q.device)
+            rc = lib.cca_b200_forward3d(q[b0:b1].data_ptr(), k[b0:b1].data_ptr(), v[b0:b1].data_ptr(), out[b0:b1].data_ptr(),
+                                        lse[b0:b1].data_ptr(), ws.data_ptr(), ws.numel(), n, *dims[1:], dt, flags,
+                                        _stream_ptr(q.device))
+            capi.check(rc, "cca_b200_forward3d")
+    return out, lse
+
+
+def cca3d_backward(dout, q, k, v, out, lse, impl: str = "auto", deterministic=None):
+    """Gradients (dq, dk, dv) of ``cca3d_forward`` given dout and the saved forward tensors.  Same ``impl`` / memory-format /
+    ``deterministic`` rules as ``cca3d_forward``."""
+    _check_inputs3d(q, k, v)
+    det = _resolve_deterministic(deterministic)
+    if dout.dtype != q.dtype or out.dtype != q.dtype or dout.shape != v.shape or out.shape != v.shape:
+        raise RuntimeError("ccnet_b200: dout/out must match v in shape and dtype")
+    if dout.device != q.device or out.device != q.device:
+        raise RuntimeError("ccnet_b200: dout/out must be on the same device as q,k,v")
+    B, Cq, T, H, W = q.shape
+    if lse.dtype != torch.float32 or tuple(lse.shape) != (B, T, H, W) or lse.device != q.device:
+        raise RuntimeError("ccnet_b200: lse must be the forward's float32 [B,T,H,W] tensor on the same device")
+    lib, dims, dt, flags, use_tc = _setup3d(q, v, impl, det)
+    if use_tc and _upcast3d(q.dtype, T, H, W, det):
+        res = cca3d_backward(dout.float(), q.float(), k.float(), v.float(), out.float(), lse, impl, det)
+        return tuple(g.to(q.dtype) for g in res)
+    fmt = torch.channels_last_3d if use_tc else torch.contiguous_format
+    dout, q, k, v, out = (t.contiguous(memory_format=fmt) for t in (dout, q, k, v, out))
+    lse = lse.contiguous()
+    with torch.cuda.device(q.device):
+        dq = torch.empty_like(q, memory_format=fmt)
+        dk = torch.empty_like(k, memory_format=fmt)
+        dv = torch.empty_like(v, memory_format=fmt)
+        for b0, b1 in _sample_groups3d(lib, capi.CCA_WS_BACKWARD, dims, dt, flags):
+            n = b1 - b0
+            ws = _workspace(lib.cca_b200_workspace_bytes3d(capi.CCA_WS_BACKWARD, n, *dims[1:], dt, flags), q.device)
+            rc = lib.cca_b200_backward3d(dout[b0:b1].data_ptr(), q[b0:b1].data_ptr(), k[b0:b1].data_ptr(), v[b0:b1].data_ptr(),
+                                         out[b0:b1].data_ptr(), lse[b0:b1].data_ptr(), dq[b0:b1].data_ptr(),
+                                         dk[b0:b1].data_ptr(), dv[b0:b1].data_ptr(), ws.data_ptr(), ws.numel(),
+                                         n, *dims[1:], dt, flags, _stream_ptr(q.device))
+            capi.check(rc, "cca_b200_backward3d")
+    return dq, dk, dv
+
+
+class _CCA3DFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, q, k, v, impl, deterministic):
+        out, lse = cca3d_forward(q, k, v, impl, deterministic)
+        ctx.save_for_backward(q, k, v, out, lse)
+        ctx.impl = impl
+        ctx.deterministic = deterministic
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        q, k, v, out, lse = ctx.saved_tensors
+        dq, dk, dv = cca3d_backward(dout, q, k, v, out, lse, ctx.impl, ctx.deterministic)
+        return dq, dk, dv, None, None
+
+
+def cca3d(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", deterministic=None) -> torch.Tensor:
+    """Differentiable criss-cross attention over clips (out only); see ``cca3d_forward``."""
+    return _CCA3DFunction.apply(q, k, v, impl, _resolve_deterministic(deterministic))

@@ -13,8 +13,8 @@ import torch.nn.functional as F
 
 from . import ops  # noqa: F401  (torch.ops.cca.attention)
 
-from .functional import (cca, cca_backward, cca_forward, qkv_gemm_eligible, qkv_project, qkv_project_dgrad,
-                         qkv_project_wgrad, qkv_wgrad_eligible, tc_eligible)
+from .functional import (cca, cca3d, cca_backward, cca_forward, qkv_gemm_eligible, qkv_project, qkv_project_dgrad,
+                         qkv_project_wgrad, qkv_wgrad_eligible, tc3d_eligible, tc_eligible)
 
 
 class _QKVProject(torch.autograd.Function):
@@ -165,3 +165,37 @@ class RCCA(nn.Module):
             else:
                 out = self.cca(out)
         return (out, maps) if return_attention else out
+
+
+class CrissCrossAttention3D(nn.Module):
+    """Criss-cross attention over clips x[B, C, T, H, W]: every position attends to the positions that share two of its
+    three coordinates (its column, row and time line; T + H + W - 2 keys), y = gamma * cca3d(q(x), k(x), v(x)) + x.
+    Parameters mirror ``CrissCrossAttention`` with 1x1x1 Conv3d projections (weights [Cq, C, 1, 1, 1], Cq = C // 8).
+
+    Where the tensor-core path covers the shape, the projections (per pixel) run as GEMMs on the [B*T, C, H, W] frames view
+    of channels_last_3d x (a view, no copy) and q, k, v come out channels_last_3d, the layout of those kernels.  Elsewhere
+    (other channel counts, T > 32, lines over 896, ``impl="simt"``) the convs are stock Conv3d and the generic kernels run."""
+
+    def __init__(self, in_dim: int, impl: str = "auto"):
+        super().__init__()
+        self.query_conv = nn.Conv3d(in_channels=in_dim, out_channels=in_dim // 8, kernel_size=1)
+        self.key_conv = nn.Conv3d(in_channels=in_dim, out_channels=in_dim // 8, kernel_size=1)
+        self.value_conv = nn.Conv3d(in_channels=in_dim, out_channels=in_dim, kernel_size=1)
+        self.gamma = nn.Parameter(torch.zeros(1))
+        self.impl = impl
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        if not x.is_cuda:
+            raise RuntimeError("ccnet_b200.CrissCrossAttention3D runs on CUDA (H100, sm_90) only")
+        B, C, T, H, W = x.shape
+        if self.impl != "simt" and tc3d_eligible(B, C // 8, C, T, H, W, x.dtype):
+            x = x.contiguous(memory_format=torch.channels_last_3d)
+            frames = x.transpose(1, 2).reshape(B * T, C, H, W)             # a channels-last view of the same memory
+            q, k, v = _QKVProject.apply(frames, self.query_conv.weight, self.query_conv.bias, self.key_conv.weight,
+                                        self.key_conv.bias, self.value_conv.weight, self.value_conv.bias)
+            q, k, v = (t.view(B, T, t.shape[1], H, W).transpose(1, 2) for t in (q, k, v))   # channels_last_3d [B, c, T, H, W]
+        else:
+            q, k, v = self.query_conv(x), self.key_conv(x), self.value_conv(x)
+        if q.dtype != v.dtype or k.dtype != v.dtype:       # autocast corner: keep one dtype
+            q, k = q.to(v.dtype), k.to(v.dtype)
+        return torch.addcmul(x, self.gamma, cca3d(q, k, v, self.impl))

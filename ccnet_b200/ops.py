@@ -5,10 +5,12 @@
     torch.ops.cca.forward_residual(q, k, v, x, gamma)     -> (y, lse)        y = gamma * out + x  (functions.py:49)
     torch.ops.cca.attention(q, k)                         -> attn            [B,H,W,H+W] fp32 (functions.py:40, `concate`)
     torch.ops.cca.attention_backward(dattn, attn, q, k)   -> (dq, dk)
+    torch.ops.cca.forward3d(q, k, v)                      -> (out, lse)      clips [B,C,T,H,W], lse [B,T,H,W]
+    torch.ops.cca.backward3d(dout, q, k, v, out, lse)     -> (dq, dk, dv)
 
 CUDA implementations call the C ABI (ccnet_b200.functional -> libcca_b200.so); FakeTensor ("meta") implementations give
 shapes / dtypes / memory formats so that ``torch.compile`` and ``torch.export`` trace through ``networks/ccnet.py`` without a
-graph break; autograd is registered on ``forward``, ``forward_residual`` and ``attention``.  Registration happens through ``torch.library``
+graph break; autograd is registered on ``forward``, ``forward_residual``, ``attention`` and ``forward3d``.  Registration happens through ``torch.library``
 (the Python face of TORCH_LIBRARY): the kernels themselves stay behind the torch-free C ABI."""
 from __future__ import annotations
 
@@ -137,3 +139,38 @@ def _attn_backward(ctx, dattn):
 
 
 attention.register_autograd(_attn_backward, setup_context=_attn_setup)
+
+
+# ---- criss-cross attention over clips:  forward3d(q, k, v) -> (out, lse[B,T,H,W]),  backward3d(...) -> (dq, dk, dv)
+#      (channels_last_3d results on the tensor-core path, contiguous ones on the generic kernels)
+@torch.library.custom_op("cca::forward3d", mutates_args=(), device_types="cuda")
+def forward3d(q: Tensor, k: Tensor, v: Tensor) -> Tuple[Tensor, Tensor]:
+    return F_.cca3d_forward(q, k, v)
+
+
+@forward3d.register_fake
+def _(q, k, v):
+    B, Cq, T, H, W = q.shape
+    fmt = torch.channels_last_3d if F_.tc3d_eligible(B, Cq, v.shape[1], T, H, W, q.dtype) else torch.contiguous_format
+    return torch.empty(v.shape, dtype=v.dtype, device=v.device).contiguous(memory_format=fmt), \
+        torch.empty((B, T, H, W), dtype=torch.float32, device=q.device)
+
+
+@torch.library.custom_op("cca::backward3d", mutates_args=(), device_types="cuda")
+def backward3d(dout: Tensor, q: Tensor, k: Tensor, v: Tensor, out: Tensor, lse: Tensor) -> Tuple[Tensor, Tensor, Tensor]:
+    return F_.cca3d_backward(dout, q, k, v, out, lse)
+
+
+@backward3d.register_fake
+def _(dout, q, k, v, out, lse):
+    fmt = torch.channels_last_3d if out.is_contiguous(memory_format=torch.channels_last_3d) and out.dim() == 5 else torch.contiguous_format
+    mk = lambda t: torch.empty(t.shape, dtype=t.dtype, device=t.device).contiguous(memory_format=fmt)
+    return mk(q), mk(k), mk(v)
+
+
+def _fwd3d_backward(ctx, dout, dlse):
+    q, k, v, out, lse = ctx.saved_tensors
+    return torch.ops.cca.backward3d(dout.contiguous(), q, k, v, out, lse)
+
+
+forward3d.register_autograd(_fwd3d_backward, setup_context=_fwd_setup)

@@ -199,6 +199,29 @@ CCA_API int cca_b200_attention_backward(const float *dattn, const float *attn, c
                                         unsigned flags, void *cuda_stream);
 
 /*
+ * Criss-cross attention over clips (the 3D op of CCNet's video extension): q, k [B,Cq,T,H,W], v, out [B,C,T,H,W].  Pixel
+ * (b,t,h,w) attends to its column {(b,t,g,w)} (self masked), its row {(b,t,h,g)} and its time line {(b,s,h,w)} (self masked):
+ * one softmax over the H+W+T logits <q_u, k_j>, out_u = sum_j a_uj v_j, lse[B,T,H,W] fp32 as for the 2D step.  At T = 1 it
+ * is the 2D step on every frame.
+ * NDHWC tensors (torch.channels_last_3d, CCA_FLAG_NHWC): the tensor-core path.  The column and row branches run on the 2D
+ * tensor-core kernels over the [B*T,H,W,C] frames view, the time branch on kernels of its own.  It covers
+ * (cca_b200_tc3d_supported) the shapes cca_b200_tc_supported covers for B*T frames, and 1 <= T <= 32.
+ * NCDHW-contiguous tensors (no CCA_FLAG_NHWC): generic kernels, any Cq and C, H + W + T - 2 <= 2048; beyond that
+ * CCA_ERR_UNSUPPORTED.  Flags, alignment and the deterministic mode as for cca_b200_forward / cca_b200_backward (the time
+ * pass adds each output element once, in a fixed order; the generic kernels are deterministic).  Workspace:
+ * cca_b200_workspace_bytes3d for the same flags (one size that covers whichever family runs).
+ */
+CCA_API int cca_b200_tc3d_supported(int which, int B, int Cq, int C, int T, int H, int W, int dtype);
+CCA_API size_t cca_b200_workspace_bytes3d(int which, int B, int Cq, int C, int T, int H, int W, int dtype, unsigned flags);
+CCA_API int cca_b200_forward3d(const void *q, const void *k, const void *v, void *out, float *lse,
+                               void *workspace, size_t workspace_bytes,
+                               int B, int Cq, int C, int T, int H, int W, int dtype, unsigned flags, void *cuda_stream);
+CCA_API int cca_b200_backward3d(const void *dout, const void *q, const void *k, const void *v,
+                                const void *out, const float *lse, void *dq, void *dk, void *dv,
+                                void *workspace, size_t workspace_bytes,
+                                int B, int Cq, int C, int T, int H, int W, int dtype, unsigned flags, void *cuda_stream);
+
+/*
  * Host-buffer variants: same maths, pointers are HOST memory (pinned or pageable).
  * They allocate device memory, copy in, run on an internal stream, copy out, free and
  * synchronise.  These are the calls a non-CUDA host language binds directly.
