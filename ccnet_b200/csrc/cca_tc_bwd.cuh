@@ -55,7 +55,6 @@ struct BwdParams {
     int out_mode;              // 1: producers store, consumers add after cdone (one tile per line); 0: cleared outputs, everything adds
     unsigned int *cdone;       // [B] producer items of sample b whose stores have completed (out_mode 1)
     int lag;                   // item order (cca_items.cuh): 1 = consumers trail the producers by one block
-    int hints;                 // L2 eviction hints on the loads and the output stores
 };
 
 // The load ring holds ONE 128-byte TMA box per slot: 32 channels for fp32 (converted in place to hi/lo planes), 64 for 16-bit
@@ -139,33 +138,29 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
         // =============================== TMA producer ===============================
         setmaxnreg_dec<kProducerRegs>();
         if (warp == 0 && lane == 0) {
-            const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
             // the next ring slot <- the 128-byte TMA box from channel c0 on.  The producer waits for nothing but free slots, so it
             // runs ahead into the next item (its Q, K and first chunks) while the consumers finish this one.
+            // No L2 eviction hints (loads or output copies): with evict_last on the producers' operands and stores and
+            // evict_first on the rest, the backward was 6 % (fp32) and 1.5 % (bf16) slower at 8x512x97x97 (DESIGN.md 4).
             uint32_t g = 0;
-            auto ring = [&](const CUtensorMap *m, int c0, const Item &it, int start, bool last_use) {
+            auto ring = [&](const CUtensorMap *m, int c0, const Item &it, int start) {
                 const int slot = g % kNLd;
                 mbar_wait(&empty[slot], ((g / kNLd) & 1) ^ 1);
                 mbar_expect_tx(&full[slot], S::kRSlot);
                 uint8_t *dst = smem + S::off_ld + slot * S::kRSlot;
                 const int cw = it.col ? it.line : start, ch = it.col ? start : it.line;
-                if (p.hints == 1) {     // what the sample's consumers read again stays; O and the consumers' own operands stream
-                    const uint64_t pol = (is_producer(it) && !last_use) ? pol_keep : pol_stream;
-                    tma_load_4d(dst, m, &full[slot], c0, cw, ch, it.b, pol);
-                } else {
-                    tma_load_4d(dst, m, &full[slot], c0, cw, ch, it.b);
-                }
+                tma_load_4d(dst, m, &full[slot], c0, cw, ch, it.b);
                 ++g;
             };
             for (int k = 0; k < nk; ++k) {
                 const Item it = item_of(k);
                 const bool calc = calc_delta(p, it);
-                for (int bx = 0; bx < kQKBoxes; ++bx) ring(it.col ? &mqc : &mqr, 32 * bx, it, it.q0, false);
-                for (int bx = 0; bx < kQKBoxes; ++bx) ring(it.col ? &mkc : &mkr, 32 * bx, it, it.k0, false);
+                for (int bx = 0; bx < kQKBoxes; ++bx) ring(it.col ? &mqc : &mqr, 32 * bx, it, it.q0);
+                for (int bx = 0; bx < kQKBoxes; ++bx) ring(it.col ? &mkc : &mkr, 32 * bx, it, it.k0);
                 for (int n = 0; n < NCH; ++n) {
-                    ring(it.col ? &mvc : &mvr, n * kCh, it, it.k0, false);
-                    ring(it.col ? &mdoc : &mdor, n * kCh, it, it.q0, false);
-                    if (calc) ring(it.col ? &moc : &mor, n * kCh, it, it.q0, p.delta_mode == 1);   // (mode 1: nobody reads O again)
+                    ring(it.col ? &mvc : &mvr, n * kCh, it, it.k0);
+                    ring(it.col ? &mdoc : &mdor, n * kCh, it, it.q0);
+                    if (calc) ring(it.col ? &moc : &mor, n * kCh, it, it.q0);
                 }
             }
         }
@@ -178,7 +173,6 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
         const uint32_t qb = smem_u32(smem + S::off_qk), kb = qb + T::kSlot, ld_base = smem_u32(smem + S::off_ld);
         const uint32_t pb = smem_u32(smem + S::off_p);
         uint8_t *pgen = smem + S::off_p;
-        const uint64_t pol_keep = l2_policy_evict_last(), pol_stream = l2_policy_evict_first();
         // this thread's accumulator rows rbase, rbase + 8 (nc channels from 0) -> `tile`, laid out as the output's swizzled TMA
         // box(es) [tile px][128 B] (fp32: 32-channel boxes T::kTile apart); rows past LK are padding and are skipped
         auto stage = [&](const float *acc, int nc, uint8_t *tile) {
@@ -198,20 +192,15 @@ cca_tc_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
                 }
             }
         };
-        // (thread 0) the staged boxes -> global: producers store, everybody else reduce-adds; L2 hints as for the loads
+        // (thread 0) the staged boxes -> global: producers store, everybody else reduce-adds
         // (PL: `part` is the plane of the box, sample coordinate part * B + b)
         auto put = [&](const CUtensorMap *m, const uint8_t *tile, int boxes, int c0, int px0, const Item &it, bool prod, int part) {
             const int cw = it.col ? it.line : px0, ch = it.col ? px0 : it.line;
             const int ob = PL ? part * p.sp.B + it.b : it.b;
             for (int bx = 0; bx < boxes; ++bx) {
                 const uint8_t *src = tile + bx * T::kTile;
-                if (p.hints == 1) {
-                    if (prod) tma_store_4d(m, src, c0 + 32 * bx, cw, ch, ob, pol_keep);
-                    else tma_reduce_add_4d(m, src, c0 + 32 * bx, cw, ch, ob, pol_stream);
-                } else {
-                    if (prod) tma_store_4d(m, src, c0 + 32 * bx, cw, ch, ob);
-                    else tma_reduce_add_4d(m, src, c0 + 32 * bx, cw, ch, ob);
-                }
+                if (prod) tma_store_4d(m, src, c0 + 32 * bx, cw, ch, ob);
+                else tma_reduce_add_4d(m, src, c0 + 32 * bx, cw, ch, ob);
             }
             bulk_commit();
         };
@@ -610,7 +599,6 @@ cudaError_t launch_bwd(const void *dout, const void *q, const void *k, const voi
     const bool one_tile = p.sp.col.nt == 1 && p.sp.row.nt == 1;
     p.out_mode = one_tile || PL ? 1 : 0;          // (PL: every item stores; 1 only skips the clear below)
     p.lag = tc_lag() != 0 ? 1 : 0;
-    p.hints = tc_l2_hints();
     const long es = sizeof(E);
     const long nq = p.out_mode == 1 ? 0 : p.npix * d.Cq * es, nv = p.out_mode == 1 ? 0 : p.npix * d.C * es;
     cca_bwd_prep_kernel<<<p.out_mode == 1 ? 1 : sm_count(), 256, 0, st>>>(
