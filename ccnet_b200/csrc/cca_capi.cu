@@ -2,6 +2,7 @@
 // host-buffer variants.  No torch types anywhere in this library.
 #include <atomic>
 #include <cstdio>
+#include <initializer_list>
 #include <cstdlib>
 #include <cstring>
 
@@ -49,7 +50,7 @@ int env_int(const char *name, int dflt, int lo, int hi)
     return v < lo || v > hi ? dflt : v;
 }
 constexpr int kUnset = -1000;
-std::atomic<int> g_pdl{kUnset}, g_zero_ahead{kUnset}, g_delta{kUnset}, g_lag{kUnset}, g_hints{kUnset};
+std::atomic<int> g_pdl{kUnset}, g_delta{kUnset}, g_lag{kUnset}, g_hints{kUnset};
 int knob(std::atomic<int> &g, const char *name, int dflt, int lo, int hi)
 {
     int v = g.load(std::memory_order_relaxed);
@@ -61,13 +62,11 @@ int knob(std::atomic<int> &g, const char *name, int dflt, int lo, int hi)
 }
 }  // namespace
 int tc_pdl() { return knob(g_pdl, "CCA_B200_PDL", 1, 0, 1); }
-int tc_zero_ahead() { return knob(g_zero_ahead, "CCA_B200_ZERO_AHEAD", 1, 1, 4); }
 int tc_delta_mode() { return knob(g_delta, "CCA_B200_DELTA", -1, -1, 1); }
 int tc_lag() { return knob(g_lag, "CCA_B200_LAG", -1, -1, 1); }
 int tc_l2_hints() { return knob(g_hints, "CCA_B200_L2HINT", 1, 0, 2); }
 #ifdef CCA_DEBUG_HOOKS
 void set_tc_pdl(int on) { g_pdl.store(on ? 1 : 0); }
-void set_tc_zero_ahead(int n) { g_zero_ahead.store(n < 1 ? 1 : (n > 4 ? 4 : n)); }
 void set_tc_delta_mode(int m) { g_delta.store(m < -1 || m > 1 ? -1 : m); }
 void set_tc_lag(int v) { g_lag.store(v < -1 || v > 1 ? -1 : v); }
 void set_tc_l2_hints(int v) { g_hints.store(v < 0 || v > 2 ? 1 : v); }
@@ -82,7 +81,6 @@ int cca_b200_version(void) { return CCA_B200_VERSION; }
 #ifdef CCA_DEBUG_HOOKS
 // A/B aids of debug builds (`python -m ccnet_b200.build --debug`); not part of the ABI, absent from release builds
 CCA_API void cca_b200__set_pdl(int on) { set_tc_pdl(on); }
-CCA_API void cca_b200__set_zero_ahead(int n) { set_tc_zero_ahead(n); }
 CCA_API void cca_b200__set_delta_mode(int m) { set_tc_delta_mode(m); }
 CCA_API void cca_b200__set_lag(int v) { set_tc_lag(v); }
 CCA_API void cca_b200__set_l2_hints(int v) { set_tc_l2_hints(v); }
@@ -126,6 +124,39 @@ int check_device()
     if (major != 9) return fail(CCA_ERR_DEVICE, "the current device is not sm_90 (H100); this library has no other code path%s%s");
     return CCA_OK;
 }
+// the *_supported queries: 0 on a device that is not sm_90; with no device at all they answer from the shape alone
+bool other_device()
+{
+    int ndev = 0;
+    return cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && device_major() != 9;
+}
+bool aligned16(std::initializer_list<const void *> ptrs)
+{
+    uintptr_t a = 0;
+    for (const void *p : ptrs) a |= reinterpret_cast<uintptr_t>(p);
+    return (a & 15) == 0;
+}
+constexpr const char *kAlignMsg = "tensor-core path needs 16-byte aligned tensors%s%s";
+// Which kernel family runs a call that passed its dimension, pointer and workspace checks: 1 tensor cores, 0 generic
+// kernels, < 0 an error status.  tc_covered: the tensor-core kernels cover the shape; det_16bit: CCA_FLAG_DETERMINISTIC with
+// 16-bit I/O on tiled lines, which only the fp32 kernels have a planes mode for.  op and layout name the call and the
+// generic kernels' layout in messages.  The generic kernels' own limits are the caller's.
+int kernel_family(unsigned flags, bool tc_covered, bool det_16bit, const char *op, const char *layout)
+{
+    if ((flags & CCA_FLAG_FORCE_SIMT) && (flags & CCA_FLAG_FORCE_TC))
+        return fail(CCA_ERR_INVALID, "FORCE_SIMT and FORCE_TC are exclusive%s%s");
+    int rc = check_device();
+    if (rc) return rc;
+    const bool nhwc = (flags & CCA_FLAG_NHWC) != 0;
+    const bool tc_ok = nhwc && tc_covered;
+    if ((flags & CCA_FLAG_FORCE_TC) && !tc_ok)
+        return fail(CCA_ERR_UNSUPPORTED, "tensor-core %s needs CCA_FLAG_NHWC and a covered shape%s", op);
+    if (nhwc && (!tc_ok || (flags & CCA_FLAG_FORCE_SIMT)))
+        return fail(CCA_ERR_UNSUPPORTED, "channels-last tensors are only handled by the tensor-core kernels; pass %s%s", layout);
+    if (tc_ok && det_16bit) return fail(CCA_ERR_UNSUPPORTED, kDetHalfMsg);
+    return tc_ok ? 1 : 0;
+}
+bool det_16bit_tiled(unsigned flags, Dims d, int dtype) { return (flags & CCA_FLAG_DETERMINISTIC) && dtype != CCA_F32 && tc_tiled(d); }
 }  // namespace
 
 int cca_b200_device_ok(void)
@@ -140,9 +171,7 @@ int cca_b200_device_ok(void)
 
 int cca_b200_tc_supported(int which, int B, int Cq, int C, int H, int W, int dtype)
 {
-    if (check_dims(B, Cq, C, H, W, dtype)) return 0;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && device_major() != 9) return 0;   // (no device at all: shape answer only)
+    if (check_dims(B, Cq, C, H, W, dtype) || other_device()) return 0;
     const Dims d{B, Cq, C, H, W};
     return (which == CCA_WS_BACKWARD ? tc_backward_supported(d, dtype) : tc_forward_supported(d, dtype)) ? 1 : 0;
 }
@@ -201,25 +230,16 @@ int cca_b200_forward(const void *q, const void *k, const void *v, void *out, flo
     if (!q || !k || !v || !out || !lse || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
     if (ws_bytes < cca_b200_workspace_bytes_ex(CCA_WS_FORWARD, B, Cq, C, H, W, dtype, flags))
         return fail(CCA_ERR_WORKSPACE, "forward workspace too small%s%s");
-    if ((flags & CCA_FLAG_FORCE_SIMT) && (flags & CCA_FLAG_FORCE_TC))
-        return fail(CCA_ERR_INVALID, "FORCE_SIMT and FORCE_TC are exclusive%s%s");
-    if ((rc = check_device())) return rc;
     const Dims d{B, Cq, C, H, W};
+    const int fam = kernel_family(flags, (flags & CCA_FLAG_NHWC) && tc_forward_supported(d, dtype), det_16bit_tiled(flags, d, dtype),
+                                  "forward", "NCHW");
+    if (fam < 0) return fam;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const char *why = "";
-    const bool nhwc = (flags & CCA_FLAG_NHWC) != 0;
-    const bool tc_ok = nhwc && tc_forward_supported(d, dtype);
-    if ((flags & CCA_FLAG_FORCE_TC) && !tc_ok)
-        return fail(CCA_ERR_UNSUPPORTED, "tensor-core forward needs CCA_FLAG_NHWC and a covered shape%s%s");
-    if (nhwc && (!tc_ok || (flags & CCA_FLAG_FORCE_SIMT)))
-        return fail(CCA_ERR_UNSUPPORTED, "channels-last tensors are only handled by the tensor-core kernels; pass NCHW%s%s");
     cudaError_t e;
-    if (tc_ok) {
-        if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
-             reinterpret_cast<uintptr_t>(out)) & 15)
-            return fail(CCA_ERR_INVALID, "tensor-core path needs 16-byte aligned tensors%s%s");
+    if (fam == 1) {
+        if (!aligned16({q, k, v, out})) return fail(CCA_ERR_INVALID, kAlignMsg);
         const bool det = (flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d);
-        if (det && dtype != CCA_F32) return fail(CCA_ERR_UNSUPPORTED, kDetHalfMsg);
         e = tc_forward(q, k, v, out, lse, ws, d, dtype, st, &why, det);
         if (e != cudaSuccess) return cuda_fail(e, why && *why ? why : "tc_forward");
         return CCA_OK;
@@ -240,24 +260,14 @@ int cca_b200_backward(const void *dout, const void *q, const void *k, const void
         return fail(CCA_ERR_INVALID, "null pointer%s%s");
     if (ws_bytes < cca_b200_workspace_bytes_ex(CCA_WS_BACKWARD, B, Cq, C, H, W, dtype, flags))
         return fail(CCA_ERR_WORKSPACE, "backward workspace too small%s%s");
-    if ((flags & CCA_FLAG_FORCE_SIMT) && (flags & CCA_FLAG_FORCE_TC))
-        return fail(CCA_ERR_INVALID, "FORCE_SIMT and FORCE_TC are exclusive%s%s");
-    if ((rc = check_device())) return rc;
     const Dims d{B, Cq, C, H, W};
+    const int fam = kernel_family(flags, (flags & CCA_FLAG_NHWC) && tc_backward_supported(d, dtype), det_16bit_tiled(flags, d, dtype),
+                                  "backward", "NCHW");
+    if (fam < 0) return fam;
     const char *why = "";
-    const bool nhwc = (flags & CCA_FLAG_NHWC) != 0;
-    const bool tc_ok = nhwc && tc_backward_supported(d, dtype);
-    if ((flags & CCA_FLAG_FORCE_TC) && !tc_ok)
-        return fail(CCA_ERR_UNSUPPORTED, "tensor-core backward needs CCA_FLAG_NHWC and a covered shape%s%s");
-    if (nhwc && (!tc_ok || (flags & CCA_FLAG_FORCE_SIMT)))
-        return fail(CCA_ERR_UNSUPPORTED, "channels-last tensors are only handled by the tensor-core kernels; pass NCHW%s%s");
-    if (tc_ok) {
-        if ((reinterpret_cast<uintptr_t>(dout) | reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) |
-             reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(dq) |
-             reinterpret_cast<uintptr_t>(dk) | reinterpret_cast<uintptr_t>(dv)) & 15)
-            return fail(CCA_ERR_INVALID, "tensor-core path needs 16-byte aligned tensors%s%s");
+    if (fam == 1) {
+        if (!aligned16({dout, q, k, v, out, dq, dk, dv})) return fail(CCA_ERR_INVALID, kAlignMsg);
         const bool det = (flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d);
-        if (det && dtype != CCA_F32) return fail(CCA_ERR_UNSUPPORTED, kDetHalfMsg);
         cudaError_t e = tc_backward(dout, q, k, v, out, lse, dq, dk, dv, ws, d, dtype,
                                     reinterpret_cast<cudaStream_t>(stream), &why, det);
         if (e != cudaSuccess) return cuda_fail(e, why && *why ? why : "tc_backward");
@@ -286,31 +296,11 @@ bool attention_det_planes(Dims d, int dtype, unsigned flags)
 {
     return (flags & CCA_FLAG_DETERMINISTIC) && (flags & CCA_FLAG_NHWC) && dtype == CCA_F32 && tc::shape_fits(Dims{d.B, d.Cq, tc::kNC, d.H, d.W}, dtype);
 }
-// which family runs (after the common checks): 1 tensor cores, 0 generic kernels, < 0 an error status
-int attention_family(Dims d, int dtype, unsigned flags, bool backward)
-{
-    if ((flags & CCA_FLAG_FORCE_SIMT) && (flags & CCA_FLAG_FORCE_TC))
-        return fail(CCA_ERR_INVALID, "FORCE_SIMT and FORCE_TC are exclusive%s%s");
-    const bool nhwc = (flags & CCA_FLAG_NHWC) != 0;
-    int rc = check_device();
-    if (rc) return rc;
-    const bool tc_ok = nhwc && tc_attention_supported(d, dtype);
-    if ((flags & CCA_FLAG_FORCE_TC) && !tc_ok)
-        return fail(CCA_ERR_UNSUPPORTED, "tensor-core attention map needs CCA_FLAG_NHWC and a covered shape%s%s");
-    if (nhwc && (!tc_ok || (flags & CCA_FLAG_FORCE_SIMT)))
-        return fail(CCA_ERR_UNSUPPORTED, "channels-last tensors are only handled by the tensor-core kernels; pass NCHW%s%s");
-    // (the forward writes every map element once: deterministic in every mode)
-    if (backward && tc_ok && (flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d) && dtype != CCA_F32)
-        return fail(CCA_ERR_UNSUPPORTED, kDetHalfMsg);
-    return tc_ok ? 1 : 0;
-}
 }  // namespace
 
 int cca_b200_attention_tc_supported(int B, int Cq, int H, int W, int dtype)
 {
-    if (check_attention_dims(B, Cq, H, W, dtype)) return 0;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && device_major() != 9) return 0;   // (no device at all: shape answer only)
+    if (check_attention_dims(B, Cq, H, W, dtype) || other_device()) return 0;
     return tc_attention_supported(Dims{B, Cq, 0, H, W}, dtype) ? 1 : 0;
 }
 
@@ -333,13 +323,13 @@ int cca_b200_attention_forward(const void *q, const void *k, float *attn, void *
     if (ws_bytes < cca_b200_attention_workspace_bytes(0, B, Cq, H, W, dtype, flags))
         return fail(CCA_ERR_WORKSPACE, "attention map workspace too small%s%s");
     const Dims d{B, Cq, 0, H, W};
-    const int fam = attention_family(d, dtype, flags, false);
+    // (the forward writes every map element once: deterministic in every mode)
+    const int fam = kernel_family(flags, (flags & CCA_FLAG_NHWC) && tc_attention_supported(d, dtype), false, "attention map", "NCHW");
     if (fam < 0) return fam;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const char *why = "";
     if (fam == 1) {
-        if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(ws)) & 15)
-            return fail(CCA_ERR_INVALID, "tensor-core path needs 16-byte aligned tensors%s%s");
+        if (!aligned16({q, k, ws})) return fail(CCA_ERR_INVALID, kAlignMsg);
         cudaError_t e = tc_attention_forward(q, k, attn, ws, d, dtype, st, &why);
         return e != cudaSuccess ? cuda_fail(e, why && *why ? why : "tc_attention_forward") : CCA_OK;
     }
@@ -358,14 +348,13 @@ int cca_b200_attention_backward(const float *dattn, const float *attn, const voi
     if (ws_bytes < cca_b200_attention_workspace_bytes(1, B, Cq, H, W, dtype, flags))
         return fail(CCA_ERR_WORKSPACE, "attention map backward workspace too small%s%s");
     const Dims d{B, Cq, 0, H, W};
-    const int fam = attention_family(d, dtype, flags, true);
+    const int fam = kernel_family(flags, (flags & CCA_FLAG_NHWC) && tc_attention_supported(d, dtype), det_16bit_tiled(flags, d, dtype),
+                                  "attention map", "NCHW");
     if (fam < 0) return fam;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const char *why = "";
     if (fam == 1) {
-        if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(dq) |
-             reinterpret_cast<uintptr_t>(dk) | reinterpret_cast<uintptr_t>(ws)) & 15)
-            return fail(CCA_ERR_INVALID, "tensor-core path needs 16-byte aligned tensors%s%s");
+        if (!aligned16({q, k, dq, dk, ws})) return fail(CCA_ERR_INVALID, kAlignMsg);
         cudaError_t e = tc_attention_backward(dattn, attn, q, k, dq, dk, ws, d, dtype, st, &why,
                                               (flags & CCA_FLAG_DETERMINISTIC) != 0);
         return e != cudaSuccess ? cuda_fail(e, why && *why ? why : "tc_attention_backward") : CCA_OK;
@@ -388,34 +377,12 @@ bool det3d_planes(Dims3 d, int dtype, unsigned flags)
 {
     return (flags & CCA_FLAG_DETERMINISTIC) && (flags & CCA_FLAG_NHWC) && dtype == CCA_F32 && tc::shape_fits(d.frames(), dtype);
 }
-// which family runs (after the dimension checks): 1 tensor cores, 0 generic kernels, < 0 an error status
-int family3d(Dims3 d, int dtype, unsigned flags)
-{
-    if ((flags & CCA_FLAG_FORCE_SIMT) && (flags & CCA_FLAG_FORCE_TC))
-        return fail(CCA_ERR_INVALID, "FORCE_SIMT and FORCE_TC are exclusive%s%s");
-    int rc = check_device();
-    if (rc) return rc;
-    const bool nhwc = (flags & CCA_FLAG_NHWC) != 0;
-    const bool tc_ok = nhwc && tc3d_supported(d, dtype);
-    if ((flags & CCA_FLAG_FORCE_TC) && !tc_ok)
-        return fail(CCA_ERR_UNSUPPORTED, "tensor-core 3D op needs CCA_FLAG_NHWC and a covered shape%s%s");
-    if (nhwc && (!tc_ok || (flags & CCA_FLAG_FORCE_SIMT)))
-        return fail(CCA_ERR_UNSUPPORTED, "channels-last tensors are only handled by the tensor-core kernels; pass NCDHW%s%s");
-    if (tc_ok) {
-        if ((flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d.frames()) && dtype != CCA_F32) return fail(CCA_ERR_UNSUPPORTED, kDetHalfMsg);
-        return 1;
-    }
-    if (!simt3d_supported(d)) return fail(CCA_ERR_UNSUPPORTED, "H + W + T - 2 above 2048 for the generic 3D kernels%s%s");
-    return 0;
-}
 }  // namespace
 
 int cca_b200_tc3d_supported(int which, int B, int Cq, int C, int T, int H, int W, int dtype)
 {
     (void)which;                              // (forward and backward cover the same shapes)
-    if (B <= 0 || T <= 0 || check_dims3d(B, Cq, C, T, H, W, dtype)) return 0;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && device_major() != 9) return 0;   // (no device at all: shape answer only)
+    if (B <= 0 || T <= 0 || check_dims3d(B, Cq, C, T, H, W, dtype) || other_device()) return 0;
     return tc3d_supported(Dims3{B, Cq, C, T, H, W}, dtype) ? 1 : 0;
 }
 
@@ -439,16 +406,16 @@ int cca_b200_forward3d(const void *q, const void *k, const void *v, void *out, f
     if (ws_bytes < cca_b200_workspace_bytes3d(CCA_WS_FORWARD, B, Cq, C, T, H, W, dtype, flags))
         return fail(CCA_ERR_WORKSPACE, "forward workspace too small%s%s");
     const Dims3 d{B, Cq, C, T, H, W};
-    const int fam = family3d(d, dtype, flags);
+    const int fam = kernel_family(flags, (flags & CCA_FLAG_NHWC) && tc3d_supported(d, dtype), det_16bit_tiled(flags, d.frames(), dtype),
+                                  "3D op", "NCDHW");
     if (fam < 0) return fam;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (fam == 0) {
+        if (!simt3d_supported(d)) return fail(CCA_ERR_UNSUPPORTED, "H + W + T - 2 above 2048 for the generic 3D kernels%s%s");
         cudaError_t e = simt_forward3d(q, k, v, out, lse, d, dtype, st);
         return e != cudaSuccess ? cuda_fail(e, "simt_forward3d") : CCA_OK;
     }
-    if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
-         reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(ws)) & 15)
-        return fail(CCA_ERR_INVALID, "tensor-core path needs 16-byte aligned tensors%s%s");
+    if (!aligned16({q, k, v, out, ws})) return fail(CCA_ERR_INVALID, kAlignMsg);
     const char *why = "";
     const bool det = (flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d.frames());
     cudaError_t e = tc_forward3d(q, k, v, out, lse, ws, d, dtype, st, &why, det);
@@ -465,18 +432,17 @@ int cca_b200_backward3d(const void *dout, const void *q, const void *k, const vo
     if (ws_bytes < cca_b200_workspace_bytes3d(CCA_WS_BACKWARD, B, Cq, C, T, H, W, dtype, flags))
         return fail(CCA_ERR_WORKSPACE, "backward workspace too small%s%s");
     const Dims3 d{B, Cq, C, T, H, W};
-    const int fam = family3d(d, dtype, flags);
+    const int fam = kernel_family(flags, (flags & CCA_FLAG_NHWC) && tc3d_supported(d, dtype), det_16bit_tiled(flags, d.frames(), dtype),
+                                  "3D op", "NCDHW");
     if (fam < 0) return fam;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (fam == 0) {
+        if (!simt3d_supported(d)) return fail(CCA_ERR_UNSUPPORTED, "H + W + T - 2 above 2048 for the generic 3D kernels%s%s");
         if (reinterpret_cast<uintptr_t>(ws) & 3) return fail(CCA_ERR_INVALID, "workspace must be 4-byte aligned%s%s");
         cudaError_t e = simt_backward3d(dout, q, k, v, out, lse, dq, dk, dv, ws, d, dtype, st);
         return e != cudaSuccess ? cuda_fail(e, "simt_backward3d") : CCA_OK;
     }
-    if ((reinterpret_cast<uintptr_t>(dout) | reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) |
-         reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(dq) |
-         reinterpret_cast<uintptr_t>(dk) | reinterpret_cast<uintptr_t>(dv) | reinterpret_cast<uintptr_t>(ws)) & 15)
-        return fail(CCA_ERR_INVALID, "tensor-core path needs 16-byte aligned tensors%s%s");
+    if (!aligned16({dout, q, k, v, out, dq, dk, dv, ws})) return fail(CCA_ERR_INVALID, kAlignMsg);
     const char *why = "";
     const bool det = (flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d.frames());
     cudaError_t e = tc_backward3d(dout, q, k, v, out, lse, dq, dk, dv, ws, d, dtype, st, &why, det);
@@ -486,11 +452,26 @@ int cca_b200_backward3d(const void *dout, const void *q, const void *k, const vo
 // ---------------------------------------------------------------------------------------
 // 1x1 Q/K/V projections (functions.py:29,32,35) as tensor-core GEMMs on the channels-last view
 // ---------------------------------------------------------------------------------------
+namespace {
+// the projection GEMMs' checks before their alignment, in this order: null pointers, dimensions, the workspace (not for the
+// weight gradient: its size follows the device's SM count), the device, the shapes the GEMM covers
+int check_gemm(bool null_ptr, long long pixels, int C, int Cq, bool wgrad, size_t ws_bytes)
+{
+    if (null_ptr) return fail(CCA_ERR_INVALID, "null pointer%s%s");
+    if (pixels <= 0 || pixels >= (1ll << 31) || C <= 0 || Cq <= 0) return fail(CCA_ERR_INVALID, "bad dimension%s%s");
+    if (!wgrad && ws_bytes < qkv_gemm_workspace(C, Cq)) return fail(CCA_ERR_WORKSPACE, "projection workspace too small%s%s");
+    int rc = check_device();
+    if (rc) return rc;
+    if (wgrad && !qkv_wgrad_supported(C, Cq))
+        return fail(CCA_ERR_UNSUPPORTED, "weight-gradient GEMM needs C %% 256 == 0 and Cq %% 64 == 0%s%s");
+    if (!wgrad && !qkv_gemm_supported(C, Cq)) return fail(CCA_ERR_UNSUPPORTED, "projection GEMM needs C %% 64 == 0 and Cq %% 64 == 0%s%s");
+    return CCA_OK;
+}
+}  // namespace
+
 int cca_b200_qkv_supported(int C, int Cq)
 {
-    if (C <= 0 || Cq <= 0) return 0;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && device_major() != 9) return 0;
+    if (C <= 0 || Cq <= 0 || other_device()) return 0;
     return qkv_gemm_supported(C, Cq) ? 1 : 0;
 }
 size_t cca_b200_qkv_workspace_bytes(int C, int Cq) { return C > 0 && Cq > 0 ? qkv_gemm_workspace(C, Cq) : 0; }
@@ -499,15 +480,9 @@ int cca_b200_qkv_project(const float *x, const float *wq, const float *bq, const
                          const float *bv, float *q, float *k, float *v, void *ws, size_t ws_bytes, long long pixels, int C, int Cq,
                          void *stream)
 {
-    if (!x || !wq || !bq || !wk || !bk || !wv || !bv || !q || !k || !v || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
-    if (pixels <= 0 || pixels >= (1ll << 31) || C <= 0 || Cq <= 0) return fail(CCA_ERR_INVALID, "bad dimension%s%s");
-    if (ws_bytes < qkv_gemm_workspace(C, Cq)) return fail(CCA_ERR_WORKSPACE, "projection workspace too small%s%s");
-    int rc = check_device();
+    int rc = check_gemm(!x || !wq || !bq || !wk || !bk || !wv || !bv || !q || !k || !v || !ws, pixels, C, Cq, false, ws_bytes);
     if (rc) return rc;
-    if (!qkv_gemm_supported(C, Cq)) return fail(CCA_ERR_UNSUPPORTED, "projection GEMM needs C %% 64 == 0 and Cq %% 64 == 0%s%s");
-    if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
-         reinterpret_cast<uintptr_t>(ws)) & 15)
-        return fail(CCA_ERR_INVALID, "projection GEMM needs 16-byte aligned tensors%s%s");
+    if (!aligned16({x, q, k, v, ws})) return fail(CCA_ERR_INVALID, "projection GEMM needs 16-byte aligned tensors%s%s");
     const char *why = "";
     cudaError_t e = qkv_project(x, wq, bq, wk, bk, wv, bv, q, k, v, ws, (long)pixels, C, Cq, reinterpret_cast<cudaStream_t>(stream), &why);
     if (e != cudaSuccess) return cuda_fail(e, why && *why ? why : "qkv_project");
@@ -518,15 +493,9 @@ int cca_b200_qkv_project_dgrad(const float *dq, const float *dk, const float *dv
                                const float *scale, float *dx, void *ws, size_t ws_bytes, long long pixels, int C, int Cq,
                                int accumulate, void *stream)
 {
-    if (!dq || !dk || !dv || !wq || !wk || !wv || !dx || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
-    if (pixels <= 0 || pixels >= (1ll << 31) || C <= 0 || Cq <= 0) return fail(CCA_ERR_INVALID, "bad dimension%s%s");
-    if (ws_bytes < qkv_gemm_workspace(C, Cq)) return fail(CCA_ERR_WORKSPACE, "projection workspace too small%s%s");
-    int rc = check_device();
+    int rc = check_gemm(!dq || !dk || !dv || !wq || !wk || !wv || !dx || !ws, pixels, C, Cq, false, ws_bytes);
     if (rc) return rc;
-    if (!qkv_gemm_supported(C, Cq)) return fail(CCA_ERR_UNSUPPORTED, "projection GEMM needs C %% 64 == 0 and Cq %% 64 == 0%s%s");
-    if ((reinterpret_cast<uintptr_t>(dx) | reinterpret_cast<uintptr_t>(dq) | reinterpret_cast<uintptr_t>(dk) | reinterpret_cast<uintptr_t>(dv) |
-         reinterpret_cast<uintptr_t>(ws)) & 15)
-        return fail(CCA_ERR_INVALID, "projection GEMM needs 16-byte aligned tensors%s%s");
+    if (!aligned16({dx, dq, dk, dv, ws})) return fail(CCA_ERR_INVALID, "projection GEMM needs 16-byte aligned tensors%s%s");
     const char *why = "";
     cudaError_t e = qkv_project_dgrad(dq, dk, dv, wq, wk, wv, scale, dx, ws, (long)pixels, C, Cq, accumulate,
                                       reinterpret_cast<cudaStream_t>(stream), &why);
@@ -537,18 +506,7 @@ int cca_b200_qkv_project_dgrad(const float *dq, const float *dk, const float *dv
 int cca_b200_qkv_project_wgrad(const float *x, const float *dq, const float *dk, const float *dv, const float *scale, float *dwq,
                                float *dwk, float *dwv, float *db, long long pixels, int C, int Cq, void *stream)
 {
-    if (!x || !dq || !dk || !dv || !dwq || !dwk || !dwv) return fail(CCA_ERR_INVALID, "null pointer%s%s");
-    if (pixels <= 0 || pixels >= (1ll << 31) || C <= 0 || Cq <= 0) return fail(CCA_ERR_INVALID, "bad dimension%s%s");
-    int rc = check_device();
-    if (rc) return rc;
-    if (!qkv_wgrad_supported(C, Cq)) return fail(CCA_ERR_UNSUPPORTED, "weight-gradient GEMM needs C %% 256 == 0 and Cq %% 64 == 0%s%s");
-    if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dq) | reinterpret_cast<uintptr_t>(dk) | reinterpret_cast<uintptr_t>(dv) |
-         reinterpret_cast<uintptr_t>(dwq) | reinterpret_cast<uintptr_t>(dwk) | reinterpret_cast<uintptr_t>(dwv)) & 15)
-        return fail(CCA_ERR_INVALID, "weight-gradient GEMM needs 16-byte aligned tensors%s%s");
-    const char *why = "";
-    cudaError_t e = qkv_project_wgrad(x, dq, dk, dv, scale, dwq, dwk, dwv, db, (long)pixels, C, Cq, reinterpret_cast<cudaStream_t>(stream), &why);
-    if (e != cudaSuccess) return cuda_fail(e, why && *why ? why : "qkv_project_wgrad");
-    return CCA_OK;
+    return cca_b200_qkv_project_wgrad_ex(x, dq, dk, dv, scale, dwq, dwk, dwv, db, pixels, C, Cq, nullptr, 0, 0, stream);
 }
 size_t cca_b200_qkv_wgrad_workspace_bytes(int C, int Cq)
 {
@@ -558,28 +516,21 @@ int cca_b200_qkv_project_wgrad_ex(const float *x, const float *dq, const float *
                                   float *dwk, float *dwv, float *db, long long pixels, int C, int Cq, void *ws, size_t ws_bytes,
                                   unsigned flags, void *stream)
 {
-    if (!(flags & CCA_FLAG_DETERMINISTIC))
-        return cca_b200_qkv_project_wgrad(x, dq, dk, dv, scale, dwq, dwk, dwv, db, pixels, C, Cq, stream);
-    if (!x || !dq || !dk || !dv || !dwq || !dwk || !dwv || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
-    if (pixels <= 0 || pixels >= (1ll << 31) || C <= 0 || Cq <= 0) return fail(CCA_ERR_INVALID, "bad dimension%s%s");
-    int rc = check_device();
+    const bool det = (flags & CCA_FLAG_DETERMINISTIC) != 0;
+    int rc = check_gemm(!x || !dq || !dk || !dv || !dwq || !dwk || !dwv || (det && !ws), pixels, C, Cq, true, 0);
     if (rc) return rc;
-    if (!qkv_wgrad_supported(C, Cq)) return fail(CCA_ERR_UNSUPPORTED, "weight-gradient GEMM needs C %% 256 == 0 and Cq %% 64 == 0%s%s");
-    if (ws_bytes < qkv_wgrad_workspace(C, Cq)) return fail(CCA_ERR_WORKSPACE, "weight-gradient workspace too small%s%s");
-    if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dq) | reinterpret_cast<uintptr_t>(dk) | reinterpret_cast<uintptr_t>(dv) |
-         reinterpret_cast<uintptr_t>(ws)) & 15)
+    if (det && ws_bytes < qkv_wgrad_workspace(C, Cq)) return fail(CCA_ERR_WORKSPACE, "weight-gradient workspace too small%s%s");
+    if (!(det ? aligned16({x, dq, dk, dv, ws}) : aligned16({x, dq, dk, dv, dwq, dwk, dwv})))
         return fail(CCA_ERR_INVALID, "weight-gradient GEMM needs 16-byte aligned tensors%s%s");
     const char *why = "";
     cudaError_t e = qkv_project_wgrad(x, dq, dk, dv, scale, dwq, dwk, dwv, db, (long)pixels, C, Cq, reinterpret_cast<cudaStream_t>(stream),
-                                      &why, ws);
+                                      &why, det ? ws : nullptr);
     if (e != cudaSuccess) return cuda_fail(e, why && *why ? why : "qkv_project_wgrad");
     return CCA_OK;
 }
 int cca_b200_qkv_wgrad_supported(int C, int Cq)
 {
-    if (C <= 0 || Cq <= 0) return 0;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) == cudaSuccess && ndev > 0 && device_major() != 9) return 0;
+    if (C <= 0 || Cq <= 0 || other_device()) return 0;
     return qkv_wgrad_supported(C, Cq) ? 1 : 0;
 }
 

@@ -129,19 +129,16 @@ size_t qkv_wgrad_workspace(int C, int Cq);
 void count_launch(int n = 1);
 // Launch knobs of the tensor-core kernels, read once from the environment (std::atomic, safe under DataParallel threads):
 //   CCA_B200_PDL = 0/1        programmatic dependent launch between the launches of one op (default 1)
-//   CCA_B200_ZERO_AHEAD = n   the items of sample b clear the outputs of sample b+n (default 1)
 //   CCA_B200_DELTA = -1/0/1   backward: -1 automatic, 0 every item computes delta, 1 column items produce it for the sample
 //   CCA_B200_LAG = 0/1        item order: consumers of a sample trail its producers by one block (default: 1 in the
 //                             backward; picked from the shape in the forward values kernel, cca_tc_fwd.cuh)
 //   CCA_B200_L2HINT = 0/1     L2 eviction hints on the bulk copies (default 1)
 int tc_pdl();
-int tc_zero_ahead();
 int tc_delta_mode();
 int tc_lag();          // -1 = per-kernel default
 int tc_l2_hints();
 #ifdef CCA_DEBUG_HOOKS
 void set_tc_pdl(int on);
-void set_tc_zero_ahead(int n);
 void set_tc_delta_mode(int m);
 void set_tc_lag(int v);
 void set_tc_l2_hints(int v);

@@ -6,6 +6,8 @@ happens in the CUDA library behind the C ABI; PyTorch only owns memory, streams 
 """
 from __future__ import annotations
 
+import os
+
 import torch
 
 from . import capi
@@ -23,31 +25,6 @@ def _resolve_deterministic(deterministic) -> bool:
     return torch.are_deterministic_algorithms_enabled() if deterministic is None else bool(deterministic)
 
 
-def _sample_groups(lib, which, B, Cq, C, H, W, dt, flags):
-    """[(b0, b1)]: batch slices whose plane workspace stays under ``deterministic_workspace_cap`` (one slice unless the
-    call needs planes)"""
-    if not flags & capi.CCA_FLAG_DETERMINISTIC:
-        return [(0, B)]
-    per_sample = (lib.cca_b200_workspace_bytes_ex(which, 1, Cq, C, H, W, dt, flags)
-                  - lib.cca_b200_workspace_bytes(which, 1, Cq, C, H, W, dt))
-    g = max(1, deterministic_workspace_cap // per_sample) if per_sample > 0 else B
-    return [(b0, min(B, b0 + g)) for b0 in range(0, B, g)]
-
-
-def _check_inputs(q, k, v):
-    if not (q.is_cuda and k.is_cuda and v.is_cuda):
-        raise RuntimeError("ccnet_b200: criss-cross attention needs CUDA tensors on an H100 (sm_90) "
-                           "(there is no CPU path in this package)")
-    if q.dtype not in _DTYPES or k.dtype != q.dtype or v.dtype != q.dtype:
-        raise RuntimeError(f"ccnet_b200: q,k,v must share dtype float32, bfloat16 or float16, got "
-                           f"{q.dtype},{k.dtype},{v.dtype}")
-    if q.dim() != 4 or k.shape != q.shape or v.dim() != 4 or v.shape[0] != q.shape[0] or v.shape[2:] != q.shape[2:]:
-        raise RuntimeError(f"ccnet_b200: expected q,k [B,Cq,H,W] and v [B,C,H,W], got "
-                           f"{tuple(q.shape)},{tuple(k.shape)},{tuple(v.shape)}")
-    if not (q.device == k.device == v.device):
-        raise RuntimeError("ccnet_b200: q,k,v must be on the same device")
-
-
 def _workspace(nbytes: int, device) -> torch.Tensor:
     """Device scratch of the C ABI calls.  The kernels write every byte they read, so torch's deterministic mode need not fill
     it first (its ``torch.empty`` fill would otherwise touch up to ``deterministic_workspace_cap`` bytes per call).  The fill
@@ -63,16 +40,89 @@ def _workspace(nbytes: int, device) -> torch.Tensor:
         td.fill_uninitialized_memory = fill
 
 
-def _half_long_lines(dtype, H: int, W: int, deterministic: bool = False) -> bool:
-    """bf16 or fp16 I/O with lines longer than one 112-pixel tile: every output element of the tensor-core kernels is then the
-    sum of up to 2*ceil(L/112) TMA reduce-adds, each rounded to the 16-bit type in memory, in no fixed order -- measured at the
-    1e-2 budget for bf16 (profiles/r02_parity_report.jsonl).  Such calls run on the fp32 kernels (bf16 and fp16 values are
-    exact in the bf16x3 split) and the result is rounded to the 16-bit type ONCE.  CCA_B200_BF16_NATIVE=1 keeps the native
-    bf16 and fp16 kernels for both types (the C ABI always does), except in deterministic mode: only the fp32 kernels have
-    it on such lines."""
-    import os
-    return (dtype in (torch.bfloat16, torch.float16) and (H > 112 or W > 112)
-            and (deterministic or not os.environ.get("CCA_B200_BF16_NATIVE")))
+def _check_inputs(q, k, v=None, rank: int = 4):
+    """q, k [B,Cq,H,W] (rank 5: [B,Cq,T,H,W]) and, when given, v [B,C,...]: CUDA tensors of one dtype on one device"""
+    ts = (q, k) if v is None else (q, k, v)
+    names = ",".join("qkv"[:len(ts)])
+    if not all(t.is_cuda for t in ts):
+        raise RuntimeError("ccnet_b200: criss-cross attention needs CUDA tensors on an H100 (sm_90) "
+                           "(there is no CPU path in this package)")
+    if q.dtype not in _DTYPES or any(t.dtype != q.dtype for t in ts):
+        raise RuntimeError(f"ccnet_b200: {names} must share dtype float32, bfloat16 or float16, got "
+                           + ",".join(str(t.dtype) for t in ts))
+    if q.dim() != rank or k.shape != q.shape or (v is not None and (v.dim() != rank or v.shape[0] != q.shape[0]
+                                                                    or v.shape[2:] != q.shape[2:])):
+        s = "T,H,W" if rank == 5 else "H,W"
+        raise RuntimeError(f"ccnet_b200: expected q,k [B,Cq,{s}]" + ("" if v is None else f" and v [B,C,{s}]") + ", got "
+                           + ",".join(str(tuple(t.shape)) for t in ts))
+    if any(t.device != q.device for t in ts):
+        raise RuntimeError(f"ccnet_b200: {names} must be on the same device")
+
+
+def _check_saved(q, v, dout, out, lse):
+    """a backward's dout and the forward's out (both like v) and lse (float32 [B,H,W], or [B,T,H,W])"""
+    if dout.dtype != q.dtype or out.dtype != q.dtype or dout.shape != v.shape or out.shape != v.shape:
+        raise RuntimeError("ccnet_b200: dout/out must match v in shape and dtype")
+    if dout.device != q.device or out.device != q.device:
+        raise RuntimeError("ccnet_b200: dout/out must be on the same device as q,k,v")
+    if lse.dtype != torch.float32 or tuple(lse.shape) != (q.shape[0], *q.shape[2:]) or lse.device != q.device:
+        s = "T,H,W" if q.dim() == 5 else "H,W"
+        raise RuntimeError(f"ccnet_b200: lse must be the forward's float32 [B,{s}] tensor on the same device")
+
+
+def _plan(impl: str, det: bool, covered, q, v=None):
+    """(use_tc, flags, memory format) of a call: the tensor-core kernels on channels-last memory where ``covered()``, the
+    op's coverage query, says they take the shape and ``impl`` allows them, else the generic kernels on contiguous memory.
+    impl="tc" on a shape the tensor-core kernels do not cover raises."""
+    use_tc = impl in ("auto", "tc") and covered()
+    if impl == "tc" and not use_tc:
+        shapes = f"q{tuple(q.shape)}" + ("" if v is None else f" v{tuple(v.shape)}")
+        raise RuntimeError(f"ccnet_b200: tensor-core kernels do not cover {shapes} {q.dtype}")
+    flags = _IMPL_FLAGS[impl] | (capi.CCA_FLAG_NHWC if use_tc else 0) | (capi.CCA_FLAG_DETERMINISTIC if det else 0)
+    fmt = (torch.channels_last_3d if q.dim() == 5 else torch.channels_last) if use_tc else torch.contiguous_format
+    return use_tc, flags, fmt
+
+
+def _upcast(dtype, H: int, W: int, deterministic: bool, T: int = 1) -> bool:
+    """16-bit calls of the tensor-core path that run on the fp32 kernels on upcast tensors (bf16 and fp16 values are exact in
+    the bf16x3 split), the result rounded to the 16-bit type ONCE:
+    - lines longer than one 112-pixel tile: every output element of the native kernels is the sum of up to 2*ceil(L/112) TMA
+      reduce-adds, each rounded to the 16-bit type in memory, in no fixed order -- at the 1e-2 budget for bf16.
+    - bf16 with T > 1 (the 3D op): the time pass adds onto out, dq, dk and dv after the 2D passes have rounded them to the
+      I/O type, a third rounding of every output element; in bf16 that puts the emulated floor at up to 0.73 of the 1e-2
+      budget (tests/test_cca3d_host.py), in fp16 at a third of its budget.  At T = 1 the time pass adds nothing and the
+      native kernels give the 2D op's bits.
+    CCA_B200_BF16_NATIVE=1 keeps the native bf16 and fp16 kernels (the C ABI always does), except in deterministic mode on
+    long lines: only the fp32 kernels have it there."""
+    if dtype not in (torch.bfloat16, torch.float16):
+        return False
+    native = bool(os.environ.get("CCA_B200_BF16_NATIVE"))
+    if H > 112 or W > 112:
+        return deterministic or not native
+    return dtype == torch.bfloat16 and T > 1 and not native
+
+
+def _grouped_call(fn, ws_query, which, tensors, dims, dt, flags, each=None):
+    """``fn(*pointers of the tensors, workspace, its bytes, n, *dims, dt, flags, stream)``, a C ABI entry point, over batch
+    slices [b0, b1) of the tensors, each with a workspace of ``ws_query(which, n, *dims, dt, flags)`` bytes.  One slice
+    unless the call is deterministic and needs partial planes: then the planes of a slice, per sample the workspace with the
+    flag minus the one without it, stay under ``deterministic_workspace_cap``.  ``each(b0, b1, ws)`` runs after each
+    slice's call."""
+    B, device = tensors[0].shape[0], tensors[0].device
+    groups = [(0, B)]
+    if flags & capi.CCA_FLAG_DETERMINISTIC:
+        per_sample = (ws_query(which, 1, *dims, dt, flags)
+                      - ws_query(which, 1, *dims, dt, flags & ~capi.CCA_FLAG_DETERMINISTIC))
+        if per_sample > 0:
+            g = max(1, deterministic_workspace_cap // per_sample)
+            groups = [(b0, min(B, b0 + g)) for b0 in range(0, B, g)]
+    stream = _stream_ptr(device)
+    for b0, b1 in groups:
+        ws = _workspace(ws_query(which, b1 - b0, *dims, dt, flags), device)
+        rc = fn(*(t[b0:b1].data_ptr() for t in tensors), ws.data_ptr(), ws.numel(), b1 - b0, *dims, dt, flags, stream)
+        capi.check(rc, fn.__name__)
+        if each is not None:
+            each(b0, b1, ws)
 
 
 def _stream_ptr(device) -> int:
@@ -105,33 +155,16 @@ def cca_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "
     B, Cq, H, W = q.shape
     C = v.shape[1]
     dt = _DTYPES[q.dtype]
-    flags = _IMPL_FLAGS[impl]
-    use_tc = impl in ("auto", "tc") and lib.cca_b200_tc_supported(capi.CCA_WS_FORWARD, B, Cq, C, H, W, dt) == 1
-    if impl == "tc" and not use_tc:
-        raise RuntimeError(f"ccnet_b200: tensor-core kernels do not cover q{tuple(q.shape)} v{tuple(v.shape)} {q.dtype}")
-    if use_tc and _half_long_lines(q.dtype, H, W, det):
+    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc_supported(capi.CCA_WS_FORWARD, B, Cq, C, H, W, dt) == 1, q, v)
+    if use_tc and _upcast(q.dtype, H, W, det):
         out32, lse = cca_forward(q.float(), k.float(), v.float(), impl, det)
         return out32.to(q.dtype), lse
-    if use_tc:
-        fmt = torch.channels_last
-        q, k, v = (t.contiguous(memory_format=fmt) for t in (q, k, v))
-        flags |= capi.CCA_FLAG_NHWC
-    else:
-        fmt = torch.contiguous_format
-        q, k, v = q.contiguous(), k.contiguous(), v.contiguous()   # reference calls .contiguous() too
-    if det:
-        flags |= capi.CCA_FLAG_DETERMINISTIC
+    q, k, v = (t.contiguous(memory_format=fmt) for t in (q, k, v))     # (the reference calls .contiguous() too)
     with torch.cuda.device(q.device):
         out = torch.empty_like(v, memory_format=fmt)
         lse = torch.empty((B, H, W), dtype=torch.float32, device=q.device)
-        for b0, b1 in _sample_groups(lib, capi.CCA_WS_FORWARD, B, Cq, C, H, W, dt, flags):
-            n = b1 - b0
-            nws = lib.cca_b200_workspace_bytes_ex(capi.CCA_WS_FORWARD, n, Cq, C, H, W, dt, flags)
-            ws = _workspace(nws, q.device)
-            rc = lib.cca_b200_forward(q[b0:b1].data_ptr(), k[b0:b1].data_ptr(), v[b0:b1].data_ptr(), out[b0:b1].data_ptr(),
-                                      lse[b0:b1].data_ptr(), ws.data_ptr(), ws.numel(), n, Cq, C, H, W, dt, flags,
-                                      _stream_ptr(q.device))
-            capi.check(rc, "cca_b200_forward")
+        _grouped_call(lib.cca_b200_forward, lib.cca_b200_workspace_bytes_ex, capi.CCA_WS_FORWARD, (q, k, v, out, lse),
+                      (Cq, C, H, W), dt, flags)
     return out, lse
 
 
@@ -144,56 +177,37 @@ def cca_backward(dout, q, k, v, out, lse, impl: str = "auto", want_delta: bool =
     channels-last tensors, the generic kernels NCHW-contiguous ones.
     """
     _check_inputs(q, k, v)
+    _check_saved(q, v, dout, out, lse)
     det = _resolve_deterministic(deterministic)
     lib = capi.load()
-    if dout.dtype != q.dtype or out.dtype != q.dtype or dout.shape != v.shape or out.shape != v.shape:
-        raise RuntimeError("ccnet_b200: dout/out must match v in shape and dtype")
     B, Cq, H, W = q.shape
     C = v.shape[1]
     dt = _DTYPES[q.dtype]
-    flags = _IMPL_FLAGS[impl]
-    if lse.dtype != torch.float32 or tuple(lse.shape) != (q.shape[0], q.shape[2], q.shape[3]) or lse.device != q.device:
-        raise RuntimeError("ccnet_b200: lse must be the forward's float32 [B,H,W] tensor on the same device")
-    if dout.device != q.device or out.device != q.device:
-        raise RuntimeError("ccnet_b200: dout/out must be on the same device as q,k,v")
-    use_tc = impl in ("auto", "tc") and lib.cca_b200_tc_supported(capi.CCA_WS_BACKWARD, B, Cq, C, H, W, dt) == 1
-    if impl == "tc" and not use_tc:
-        raise RuntimeError(f"ccnet_b200: tensor-core kernels do not cover q{tuple(q.shape)} v{tuple(v.shape)} {q.dtype}")
-    if use_tc and _half_long_lines(q.dtype, H, W, det):
+    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc_supported(capi.CCA_WS_BACKWARD, B, Cq, C, H, W, dt) == 1, q, v)
+    if use_tc and _upcast(q.dtype, H, W, det):
         res = cca_backward(dout.float(), q.float(), k.float(), v.float(), out.float(), lse, impl, want_delta, det)
         return tuple(g.to(q.dtype) for g in res[:3]) + tuple(res[3:])
-    if use_tc:
-        fmt = torch.channels_last
-        dout, q, k, v, out = (t.contiguous(memory_format=fmt) for t in (dout, q, k, v, out))
-        flags |= capi.CCA_FLAG_NHWC
-    else:
-        fmt = torch.contiguous_format
-        dout, q, k, v, out = (t.contiguous() for t in (dout, q, k, v, out))
+    dout, q, k, v, out = (t.contiguous(memory_format=fmt) for t in (dout, q, k, v, out))
     lse = lse.contiguous()
-    if det:
-        flags |= capi.CCA_FLAG_DETERMINISTIC
+    delta = None
+
+    def keep_delta(b0, b1, ws):             # (the delta of each slice is at the start of its workspace)
+        nonlocal delta
+        part = ws[:(b1 - b0) * H * W * 4].view(torch.float32).view(b1 - b0, H, W)
+        if b1 - b0 == B:
+            delta = part
+            return
+        if delta is None:
+            delta = torch.empty((B, H, W), dtype=torch.float32, device=q.device)
+        delta[b0:b1].copy_(part)
+
     with torch.cuda.device(q.device):
         dq = torch.empty_like(q, memory_format=fmt)
         dk = torch.empty_like(k, memory_format=fmt)
         dv = torch.empty_like(v, memory_format=fmt)
-        groups = _sample_groups(lib, capi.CCA_WS_BACKWARD, B, Cq, C, H, W, dt, flags)
-        delta = torch.empty((B, H, W), dtype=torch.float32, device=q.device) if want_delta and len(groups) > 1 else None
-        for b0, b1 in groups:
-            n = b1 - b0
-            nws = lib.cca_b200_workspace_bytes_ex(capi.CCA_WS_BACKWARD, n, Cq, C, H, W, dt, flags)
-            ws = _workspace(nws, q.device)
-            rc = lib.cca_b200_backward(dout[b0:b1].data_ptr(), q[b0:b1].data_ptr(), k[b0:b1].data_ptr(), v[b0:b1].data_ptr(),
-                                       out[b0:b1].data_ptr(), lse[b0:b1].data_ptr(), dq[b0:b1].data_ptr(),
-                                       dk[b0:b1].data_ptr(), dv[b0:b1].data_ptr(), ws.data_ptr(), ws.numel(),
-                                       n, Cq, C, H, W, dt, flags, _stream_ptr(q.device))
-            capi.check(rc, "cca_b200_backward")
-            if delta is not None and use_tc:     # (the delta of each group is in its workspace)
-                delta[b0:b1].copy_(ws[:n * H * W * 4].view(torch.float32).view(n, H, W))
-    if want_delta:
-        if delta is None:
-            delta = ws[:B * H * W * 4].view(torch.float32).view(B, H, W) if use_tc else None
-        return dq, dk, dv, delta
-    return dq, dk, dv
+        _grouped_call(lib.cca_b200_backward, lib.cca_b200_workspace_bytes_ex, capi.CCA_WS_BACKWARD,
+                      (dout, q, k, v, out, lse, dq, dk, dv), (Cq, C, H, W), dt, flags, keep_delta if want_delta and use_tc else None)
+    return (dq, dk, dv, delta) if want_delta else (dq, dk, dv)
 
 
 def qkv_gemm_eligible(x: torch.Tensor, Cq: int) -> bool:
@@ -303,18 +317,6 @@ def cca(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", d
 # ---------------------------------------------------------------------------------------------------------------------
 # attention map (cc_attention/functions.py:40, the softmax output `concate`) and its gradient
 # ---------------------------------------------------------------------------------------------------------------------
-def _check_qk(q, k):
-    if not (q.is_cuda and k.is_cuda):
-        raise RuntimeError("ccnet_b200: the attention map needs CUDA tensors on an H100 (sm_90) "
-                           "(there is no CPU path in this package)")
-    if q.dtype not in _DTYPES or k.dtype != q.dtype:
-        raise RuntimeError(f"ccnet_b200: q,k must share dtype float32, bfloat16 or float16, got {q.dtype},{k.dtype}")
-    if q.dim() != 4 or k.shape != q.shape:
-        raise RuntimeError(f"ccnet_b200: expected q,k [B,Cq,H,W], got {tuple(q.shape)},{tuple(k.shape)}")
-    if q.device != k.device:
-        raise RuntimeError("ccnet_b200: q,k must be on the same device")
-
-
 def attention_tc_eligible(B: int, Cq: int, H: int, W: int, dtype: torch.dtype) -> bool:
     """True if the wgmma (channels-last) attention-map kernels cover this problem."""
     return dtype in _DTYPES and capi.load().cca_b200_attention_tc_supported(B, Cq, H, W, _DTYPES[dtype]) == 1
@@ -326,22 +328,13 @@ def cca_attention_forward(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", 
 
     ``impl`` as for ``cca_forward``.  Every map element is written once, so the result is the same in every mode;
     ``deterministic`` only sets the flag the C ABI is called with."""
-    _check_qk(q, k)
+    _check_inputs(q, k)
     det = _resolve_deterministic(deterministic)
     lib = capi.load()
     B, Cq, H, W = q.shape
     dt = _DTYPES[q.dtype]
-    flags = _IMPL_FLAGS[impl]
-    use_tc = impl in ("auto", "tc") and lib.cca_b200_attention_tc_supported(B, Cq, H, W, dt) == 1
-    if impl == "tc" and not use_tc:
-        raise RuntimeError(f"ccnet_b200: tensor-core kernels do not cover q{tuple(q.shape)} {q.dtype}")
-    if use_tc:
-        q, k = (t.contiguous(memory_format=torch.channels_last) for t in (q, k))
-        flags |= capi.CCA_FLAG_NHWC
-    else:
-        q, k = q.contiguous(), k.contiguous()
-    if det:
-        flags |= capi.CCA_FLAG_DETERMINISTIC
+    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_attention_tc_supported(B, Cq, H, W, dt) == 1, q)
+    q, k = (t.contiguous(memory_format=fmt) for t in (q, k))
     with torch.cuda.device(q.device):
         attn = torch.empty((B, H, W, H + W), dtype=torch.float32, device=q.device)
         ws = _workspace(lib.cca_b200_attention_workspace_bytes(0, B, Cq, H, W, dt, flags), q.device)
@@ -355,7 +348,7 @@ def cca_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministic=
     """Gradients (dq, dk) of ``cca_attention_forward`` given dattn = dL/dattn and the forward's map:
     dS = attn * (dattn - rho), rho = sum_j attn dattn;  dq = dS k,  dk = dS^T q.  Same ``impl`` / memory-format /
     ``deterministic`` rules as ``cca_backward``."""
-    _check_qk(q, k)
+    _check_inputs(q, k)
     det = _resolve_deterministic(deterministic)
     lib = capi.load()
     B, Cq, H, W = q.shape
@@ -363,45 +356,18 @@ def cca_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministic=
         if t.dtype != torch.float32 or tuple(t.shape) != (B, H, W, H + W) or t.device != q.device:
             raise RuntimeError(f"ccnet_b200: {name} must be a float32 [B,H,W,H+W] tensor on the device of q, k")
     dt = _DTYPES[q.dtype]
-    flags = _IMPL_FLAGS[impl]
-    use_tc = impl in ("auto", "tc") and lib.cca_b200_attention_tc_supported(B, Cq, H, W, dt) == 1
-    if impl == "tc" and not use_tc:
-        raise RuntimeError(f"ccnet_b200: tensor-core kernels do not cover q{tuple(q.shape)} {q.dtype}")
-    if use_tc and _half_long_lines(q.dtype, H, W, det):
+    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_attention_tc_supported(B, Cq, H, W, dt) == 1, q)
+    if use_tc and _upcast(q.dtype, H, W, det):
         dq, dk = cca_attention_backward(dattn, attn, q.float(), k.float(), impl, det)
         return dq.to(q.dtype), dk.to(q.dtype)
-    if use_tc:
-        fmt = torch.channels_last
-        q, k = (t.contiguous(memory_format=fmt) for t in (q, k))
-        flags |= capi.CCA_FLAG_NHWC
-    else:
-        fmt = torch.contiguous_format
-        q, k = q.contiguous(), k.contiguous()
+    q, k = (t.contiguous(memory_format=fmt) for t in (q, k))
     dattn, attn = dattn.contiguous(), attn.contiguous()
-    if det:
-        flags |= capi.CCA_FLAG_DETERMINISTIC
     with torch.cuda.device(q.device):
         dq = torch.empty_like(q, memory_format=fmt)
         dk = torch.empty_like(k, memory_format=fmt)
-        for b0, b1 in _attention_groups(lib, B, Cq, H, W, dt, flags):
-            n = b1 - b0
-            ws = _workspace(lib.cca_b200_attention_workspace_bytes(1, n, Cq, H, W, dt, flags), q.device)
-            rc = lib.cca_b200_attention_backward(dattn[b0:b1].data_ptr(), attn[b0:b1].data_ptr(), q[b0:b1].data_ptr(),
-                                                 k[b0:b1].data_ptr(), dq[b0:b1].data_ptr(), dk[b0:b1].data_ptr(),
-                                                 ws.data_ptr(), ws.numel(), n, Cq, H, W, dt, flags, _stream_ptr(q.device))
-            capi.check(rc, "cca_b200_attention_backward")
+        _grouped_call(lib.cca_b200_attention_backward, lib.cca_b200_attention_workspace_bytes, 1, (dattn, attn, q, k, dq, dk),
+                      (Cq, H, W), dt, flags)
     return dq, dk
-
-
-def _attention_groups(lib, B, Cq, H, W, dt, flags):
-    """``_sample_groups`` for the map backward: batch slices whose plane workspace stays under
-    ``deterministic_workspace_cap``"""
-    if not flags & capi.CCA_FLAG_DETERMINISTIC:
-        return [(0, B)]
-    per_sample = (lib.cca_b200_attention_workspace_bytes(1, 1, Cq, H, W, dt, flags)
-                  - lib.cca_b200_attention_workspace_bytes(1, 1, Cq, H, W, dt, flags & ~capi.CCA_FLAG_DETERMINISTIC))
-    g = max(1, deterministic_workspace_cap // per_sample) if per_sample > 0 else B
-    return [(b0, min(B, b0 + g)) for b0 in range(0, B, g)]
 
 
 class _CCAAttentionFunction(torch.autograd.Function):
@@ -429,59 +395,9 @@ def cca_attention(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", determin
 # ---------------------------------------------------------------------------------------------------------------------
 # criss-cross attention over clips (the 3D op): column, row and time branches under one softmax
 # ---------------------------------------------------------------------------------------------------------------------
-def _check_inputs3d(q, k, v):
-    if not (q.is_cuda and k.is_cuda and v.is_cuda):
-        raise RuntimeError("ccnet_b200: criss-cross attention needs CUDA tensors on an H100 (sm_90) "
-                           "(there is no CPU path in this package)")
-    if q.dtype not in _DTYPES or k.dtype != q.dtype or v.dtype != q.dtype:
-        raise RuntimeError(f"ccnet_b200: q,k,v must share dtype float32, bfloat16 or float16, got "
-                           f"{q.dtype},{k.dtype},{v.dtype}")
-    if q.dim() != 5 or k.shape != q.shape or v.dim() != 5 or v.shape[0] != q.shape[0] or v.shape[2:] != q.shape[2:]:
-        raise RuntimeError(f"ccnet_b200: expected q,k [B,Cq,T,H,W] and v [B,C,T,H,W], got "
-                           f"{tuple(q.shape)},{tuple(k.shape)},{tuple(v.shape)}")
-    if not (q.device == k.device == v.device):
-        raise RuntimeError("ccnet_b200: q,k,v must be on the same device")
-
-
 def tc3d_eligible(B: int, Cq: int, C: int, T: int, H: int, W: int, dtype: torch.dtype) -> bool:
     """True if the 3D op's kernels cover this problem (the 2D tensor-core shapes for B*T frames, 1 <= T <= 32)."""
     return dtype in _DTYPES and capi.load().cca_b200_tc3d_supported(capi.CCA_WS_FORWARD, B, Cq, C, T, H, W, _DTYPES[dtype]) == 1
-
-
-def _setup3d(q, v, impl, det):
-    """(lib, dims, dtype code, flags, use_tc) of a 3D call: the tensor-core path where it covers the shape and ``impl`` allows
-    it, else the generic kernels"""
-    lib = capi.load()
-    B, Cq, T, H, W = q.shape
-    C = v.shape[1]
-    dt = _DTYPES[q.dtype]
-    use_tc = impl in ("auto", "tc") and lib.cca_b200_tc3d_supported(capi.CCA_WS_FORWARD, B, Cq, C, T, H, W, dt) == 1
-    if impl == "tc" and not use_tc:
-        raise RuntimeError(f"ccnet_b200: tensor-core kernels do not cover q{tuple(q.shape)} v{tuple(v.shape)} {q.dtype}")
-    flags = _IMPL_FLAGS[impl] | (capi.CCA_FLAG_NHWC if use_tc else 0) | (capi.CCA_FLAG_DETERMINISTIC if det else 0)
-    return lib, (B, Cq, C, T, H, W), dt, flags, use_tc
-
-
-def _upcast3d(dtype, T: int, H: int, W: int, deterministic: bool) -> bool:
-    """16-bit calls of the 3D tensor-core path that run on the fp32 kernels, rounded to the 16-bit type once: those of
-    ``_half_long_lines``, and bf16 with T > 1.  The time pass adds onto out, dq, dk and dv after the 2D passes have rounded
-    them to the I/O type, a third rounding of every output element; in bf16 that puts the emulated floor at up to 0.73 of
-    the 1e-2 budget (tests/test_cca3d_host.py), in fp16 at a third of its budget.  CCA_B200_BF16_NATIVE=1 keeps the native
-    kernels, as in 2D.  At T = 1 the time pass adds nothing and the native kernels give the 2D op's bits."""
-    import os
-    return _half_long_lines(dtype, H, W, deterministic) or (
-        dtype == torch.bfloat16 and T > 1 and not os.environ.get("CCA_B200_BF16_NATIVE"))
-
-
-def _sample_groups3d(lib, which, dims, dt, flags):
-    """``_sample_groups`` of the 3D op: clip slices whose plane workspace stays under ``deterministic_workspace_cap``"""
-    B = dims[0]
-    if not flags & capi.CCA_FLAG_DETERMINISTIC:
-        return [(0, B)]
-    per_clip = (lib.cca_b200_workspace_bytes3d(which, 1, *dims[1:], dt, flags)
-                - lib.cca_b200_workspace_bytes3d(which, 1, *dims[1:], dt, flags & ~capi.CCA_FLAG_DETERMINISTIC))
-    g = max(1, deterministic_workspace_cap // per_clip) if per_clip > 0 else B
-    return [(b0, min(B, b0 + g)) for b0 in range(0, B, g)]
 
 
 def cca3d_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", deterministic=None):
@@ -493,59 +409,49 @@ def cca3d_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str =
     error), "simt" (generic kernels: any Cq and C, H + W + T - 2 <= 2048).  The tensor-core path works on channels_last_3d
     memory (inputs in another format are converted, the output is channels_last_3d), the generic kernels on contiguous
     NCDHW memory.  ``deterministic`` as for ``cca_forward``."""
-    _check_inputs3d(q, k, v)
+    _check_inputs(q, k, v, rank=5)
     det = _resolve_deterministic(deterministic)
-    lib, dims, dt, flags, use_tc = _setup3d(q, v, impl, det)
-    B, Cq, C, T, H, W = dims
-    if use_tc and _upcast3d(q.dtype, T, H, W, det):
+    lib = capi.load()
+    B, Cq, T, H, W = q.shape
+    C = v.shape[1]
+    dt = _DTYPES[q.dtype]
+    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc3d_supported(capi.CCA_WS_FORWARD, B, Cq, C, T, H, W, dt) == 1,
+                               q, v)
+    if use_tc and _upcast(q.dtype, H, W, det, T):
         out32, lse = cca3d_forward(q.float(), k.float(), v.float(), impl, det)
         return out32.to(q.dtype), lse
-    fmt = torch.channels_last_3d if use_tc else torch.contiguous_format
     q, k, v = (t.contiguous(memory_format=fmt) for t in (q, k, v))
     with torch.cuda.device(q.device):
         out = torch.empty_like(v, memory_format=fmt)
         lse = torch.empty((B, T, H, W), dtype=torch.float32, device=q.device)
-        for b0, b1 in _sample_groups3d(lib, capi.CCA_WS_FORWARD, dims, dt, flags):
-            n = b1 - b0
-            ws = _workspace(lib.cca_b200_workspace_bytes3d(capi.CCA_WS_FORWARD, n, *dims[1:], dt, flags), q.device)
-            rc = lib.cca_b200_forward3d(q[b0:b1].data_ptr(), k[b0:b1].data_ptr(), v[b0:b1].data_ptr(), out[b0:b1].data_ptr(),
-                                        lse[b0:b1].data_ptr(), ws.data_ptr(), ws.numel(), n, *dims[1:], dt, flags,
-                                        _stream_ptr(q.device))
-            capi.check(rc, "cca_b200_forward3d")
+        _grouped_call(lib.cca_b200_forward3d, lib.cca_b200_workspace_bytes3d, capi.CCA_WS_FORWARD, (q, k, v, out, lse),
+                      (Cq, C, T, H, W), dt, flags)
     return out, lse
 
 
 def cca3d_backward(dout, q, k, v, out, lse, impl: str = "auto", deterministic=None):
     """Gradients (dq, dk, dv) of ``cca3d_forward`` given dout and the saved forward tensors.  Same ``impl`` / memory-format /
     ``deterministic`` rules as ``cca3d_forward``."""
-    _check_inputs3d(q, k, v)
+    _check_inputs(q, k, v, rank=5)
+    _check_saved(q, v, dout, out, lse)
     det = _resolve_deterministic(deterministic)
-    if dout.dtype != q.dtype or out.dtype != q.dtype or dout.shape != v.shape or out.shape != v.shape:
-        raise RuntimeError("ccnet_b200: dout/out must match v in shape and dtype")
-    if dout.device != q.device or out.device != q.device:
-        raise RuntimeError("ccnet_b200: dout/out must be on the same device as q,k,v")
+    lib = capi.load()
     B, Cq, T, H, W = q.shape
-    if lse.dtype != torch.float32 or tuple(lse.shape) != (B, T, H, W) or lse.device != q.device:
-        raise RuntimeError("ccnet_b200: lse must be the forward's float32 [B,T,H,W] tensor on the same device")
-    lib, dims, dt, flags, use_tc = _setup3d(q, v, impl, det)
-    if use_tc and _upcast3d(q.dtype, T, H, W, det):
+    C = v.shape[1]
+    dt = _DTYPES[q.dtype]
+    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc3d_supported(capi.CCA_WS_BACKWARD, B, Cq, C, T, H, W, dt) == 1,
+                               q, v)
+    if use_tc and _upcast(q.dtype, H, W, det, T):
         res = cca3d_backward(dout.float(), q.float(), k.float(), v.float(), out.float(), lse, impl, det)
         return tuple(g.to(q.dtype) for g in res)
-    fmt = torch.channels_last_3d if use_tc else torch.contiguous_format
     dout, q, k, v, out = (t.contiguous(memory_format=fmt) for t in (dout, q, k, v, out))
     lse = lse.contiguous()
     with torch.cuda.device(q.device):
         dq = torch.empty_like(q, memory_format=fmt)
         dk = torch.empty_like(k, memory_format=fmt)
         dv = torch.empty_like(v, memory_format=fmt)
-        for b0, b1 in _sample_groups3d(lib, capi.CCA_WS_BACKWARD, dims, dt, flags):
-            n = b1 - b0
-            ws = _workspace(lib.cca_b200_workspace_bytes3d(capi.CCA_WS_BACKWARD, n, *dims[1:], dt, flags), q.device)
-            rc = lib.cca_b200_backward3d(dout[b0:b1].data_ptr(), q[b0:b1].data_ptr(), k[b0:b1].data_ptr(), v[b0:b1].data_ptr(),
-                                         out[b0:b1].data_ptr(), lse[b0:b1].data_ptr(), dq[b0:b1].data_ptr(),
-                                         dk[b0:b1].data_ptr(), dv[b0:b1].data_ptr(), ws.data_ptr(), ws.numel(),
-                                         n, *dims[1:], dt, flags, _stream_ptr(q.device))
-            capi.check(rc, "cca_b200_backward3d")
+        _grouped_call(lib.cca_b200_backward3d, lib.cca_b200_workspace_bytes3d, capi.CCA_WS_BACKWARD,
+                      (dout, q, k, v, out, lse, dq, dk, dv), (Cq, C, T, H, W), dt, flags)
     return dq, dk, dv
 
 

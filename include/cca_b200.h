@@ -23,7 +23,7 @@
  *   - inputs are never written; outputs need no initialisation.
  *   - re-entrant: no global scratch; the caller supplies the (small) workspace.  Process-wide state is limited to
  *     read-mostly caches (tensor maps, device attributes) and launch knobs read once from the environment.
- *   - every compute entry point returns CCA_ERR_DEVICE unless the current device is compute capability 10.x.
+ *   - every compute entry point returns CCA_ERR_DEVICE unless the current device is compute capability 9.x (sm_90).
  */
 #ifndef CCA_B200_H_
 #define CCA_B200_H_
@@ -93,7 +93,7 @@ CCA_API int cca_b200_version(void);
 CCA_API const char *cca_b200_last_error(void);
 CCA_API const char *cca_b200_strerror(int status);
 
-/* 1 if the current CUDA device can run this library (compute capability 10.x), else 0;
+/* 1 if the current CUDA device can run this library (compute capability 9.x, sm_90), else 0;
  * negative cca_status on CUDA failure. */
 CCA_API int cca_b200_device_ok(void);
 

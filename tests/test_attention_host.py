@@ -97,6 +97,18 @@ def test_attention_entry_points_reject_bad_arguments_before_any_cuda_call():
     assert rc == -1 and b"aligned" in lib.cca_b200_last_error()       # attn not even float-aligned
     rc = lib.cca_b200_attention_backward(p + 2, p, p, p, p, p, p, 1 << 20, 1, 16, 4, 4, capi.CCA_F32, 0, None)
     assert rc == -1 and b"aligned" in lib.cca_b200_last_error()
+    err, big = lib.cca_b200_last_error, 1 << 30
+    both = capi.CCA_FLAG_FORCE_SIMT | capi.CCA_FLAG_FORCE_TC
+    for fn, n in ((lib.cca_b200_attention_forward, 4), (lib.cca_b200_attention_backward, 7)):
+        def call(ptrs=(p,) * n, nbytes=big, B=1, Cq=16, dtype=capi.CCA_F32, flags=0):
+            return fn(*ptrs, nbytes, B, Cq, 4, 4, dtype, flags, None)
+        assert call(ptrs=(p,) * (n - 1) + (None,)) == -1 and b"null" in err()
+        assert call(B=0) == -1 and b"dimension" in err()
+        assert call(Cq=-16) == -1 and b"dimension" in err()
+        assert call(dtype=7) == -1 and b"dtype" in err()
+        assert call(flags=both) == -1 and b"exclusive" in err()
+        assert call(flags=both | capi.CCA_FLAG_NHWC) == -1 and b"exclusive" in err()
+        assert call(nbytes=0) == -3 and b"workspace" in err()
 
 
 def test_attention_workspace_and_coverage_without_gpu():

@@ -102,6 +102,18 @@ def test_3d_entry_points_reject_bad_arguments_before_any_cuda_call():
     assert rc == -3
     rc = lib.cca_b200_backward3d(p, p, p, None, p, p, p, p, p, p, 1 << 30, 1, 16, 64, 4, 5, 5, capi.CCA_F32, nhwc, None)
     assert rc == -1 and b"null" in lib.cca_b200_last_error()
+    err = lib.cca_b200_last_error
+    both = capi.CCA_FLAG_FORCE_SIMT | capi.CCA_FLAG_FORCE_TC
+    for fn, n in ((lib.cca_b200_forward3d, 6), (lib.cca_b200_backward3d, 10)):
+        def call(ptrs=(p,) * n, nbytes=1 << 30, B=1, T=4, dtype=capi.CCA_F32, flags=nhwc):
+            return fn(*ptrs, nbytes, B, 16, 64, T, 5, 5, dtype, flags, None)
+        assert call(ptrs=(p,) * (n - 1) + (None,)) == -1 and b"null" in err()
+        assert call(B=0) == -1 and b"dimension" in err()
+        assert call(T=0) == -1 and b"dimension" in err()
+        assert call(dtype=7) == -1 and b"dtype" in err()
+        assert call(flags=both) == -1 and b"exclusive" in err()
+        assert call(flags=both | nhwc) == -1 and b"exclusive" in err()
+        assert call(nbytes=16) == -3 and b"workspace" in err()
 
 
 def _a16(x):
@@ -233,7 +245,7 @@ def _branch_parts(q, k, v, dout):
 def test_16bit_rounding_chain_of_the_native_3d_path(dtype):
     """The native 16-bit path rounds each output element three times: the column part is stored in the I/O type, the row
     part reduce-added onto it (rounded), the time part added by the time pass (rounded again).  The floor of that chain alone
-    (exact P, dS; 16-bit inputs; max|err| / max(1, max|ref|)) decides the policy of functional._upcast3d: fp16 stays within
+    (exact P, dS; 16-bit inputs; max|err| / max(1, max|ref|)) decides the policy of functional._upcast: fp16 stays within
     a third of its budget (tests/f16_budget.py), bf16 reaches 0.73 of its 1e-2 budget, so bf16 with T > 1 runs on the fp32
     kernels and is rounded once (floor 2.9e-3 here, under half the budget)."""
     from f16_budget import F16_BUDGET
@@ -258,7 +270,7 @@ def test_16bit_rounding_chain_of_the_native_3d_path(dtype):
 
 
 def test_bf16_with_time_runs_on_the_fp32_kernels():
-    from ccnet_b200.functional import _upcast3d
-    assert _upcast3d(torch.bfloat16, 2, 9, 9, False) and not _upcast3d(torch.bfloat16, 1, 9, 9, False)
-    assert not _upcast3d(torch.float16, 8, 97, 97, False) and _upcast3d(torch.float16, 8, 97, 113, False)
-    assert not _upcast3d(torch.float32, 8, 200, 200, False)
+    from ccnet_b200.functional import _upcast
+    assert _upcast(torch.bfloat16, 9, 9, False, T=2) and not _upcast(torch.bfloat16, 9, 9, False, T=1)
+    assert not _upcast(torch.float16, 97, 97, False, T=8) and _upcast(torch.float16, 97, 113, False, T=8)
+    assert not _upcast(torch.float32, 200, 200, False, T=8)

@@ -47,8 +47,8 @@ def test_python_layer_maps_float16():
     assert not F_.tc_eligible(1, 8, 64, 32, 32, torch.float16)
     # lines longer than one tile: both 16-bit types run on the fp32 kernels and round once (unless the native switch is set)
     for dt in (torch.float16, torch.bfloat16):
-        assert F_._half_long_lines(dt, 97, 193) and not F_._half_long_lines(dt, 97, 97)
-    assert not F_._half_long_lines(torch.float32, 193, 193)
+        assert F_._upcast(dt, 97, 193, False) and not F_._upcast(dt, 97, 97, False)
+    assert not F_._upcast(torch.float32, 193, 193, False)
     with pytest.raises(RuntimeError, match="CUDA"):
         ccnet_b200.cca_forward(*(torch.randn(1, c, 4, 4, dtype=torch.float16) for c in (8, 8, 64)))
 

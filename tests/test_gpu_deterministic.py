@@ -23,7 +23,7 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F32, BF, F16 = torch.float32, torch.bfloat16, torch.float16
 TILED = [(2, 32, 128, 113, 200), (1, 16, 64, 7, 225), (1, 64, 128, 129, 257)]
-# 16-bit I/O on tiled lines runs on the fp32 kernels and rounds once (ccnet_b200.functional._half_long_lines)
+# 16-bit I/O on tiled lines runs on the fp32 kernels and rounds once (ccnet_b200.functional._upcast)
 BUDGET = {F32: tb.FP32_BUDGET, BF: {n: 1e-2 for n in tb.TENSORS},
           F16: {n: max(fb.F16_BUDGET[n], tb.FP32_BUDGET[n]) for n in tb.TENSORS}}
 KNOBS = ("CCA_B200_DELTA", "CCA_B200_LAG", "CCA_B200_PDL", "CCA_B200_L2HINT", "CCA_B200_BF16_NATIVE", "CUBLAS_WORKSPACE_CONFIG")

@@ -188,7 +188,6 @@ def test_launch_knobs_are_bit_identical(dtype):
     dev = _dev()
     lib = capi.load()
     pdl = _debug_hook(lib, "cca_b200__set_pdl", [ctypes.c_int])
-    ahead = _debug_hook(lib, "cca_b200__set_zero_ahead", [ctypes.c_int])
     dmode = _debug_hook(lib, "cca_b200__set_delta_mode", [ctypes.c_int])
     lag = _debug_hook(lib, "cca_b200__set_lag", [ctypes.c_int])
     hint = _debug_hook(lib, "cca_b200__set_l2_hints", [ctypes.c_int])

@@ -45,6 +45,50 @@ def test_invalid_arguments_are_rejected_before_any_cuda_call():
     assert rc == -1
     rc = lib.cca_b200_forward(None, None, None, None, None, None, 0, 1, 8, 64, 4, 4, 7, 0, None)
     assert rc == -1 and b"dtype" in lib.cca_b200_last_error()
+    err = lib.cca_b200_last_error
+    p, big = 16, 1 << 30                    # any non-null address: every check below comes before anything touches it
+    both = capi.CCA_FLAG_FORCE_SIMT | capi.CCA_FLAG_FORCE_TC
+    for fn, n in ((lib.cca_b200_forward, 6), (lib.cca_b200_backward, 10)):
+        def call(ptrs=(p,) * n, nbytes=big, B=1, dtype=capi.CCA_F32, flags=0):
+            return fn(*ptrs, nbytes, B, 8, 64, 4, 4, dtype, flags, None)
+        assert call(ptrs=(None,) * n) == -1 and b"null" in err()
+        assert call(ptrs=(p,) * (n - 1) + (None,)) == -1 and b"null" in err()
+        assert call(B=0) == -1 and b"dimension" in err()
+        assert call(B=-2) == -1 and b"dimension" in err()
+        assert call(dtype=7) == -1 and b"dtype" in err()
+        assert call(flags=both) == -1 and b"exclusive" in err()
+        assert call(flags=both | capi.CCA_FLAG_NHWC) == -1 and b"exclusive" in err()
+        assert call(nbytes=16) == -3 and b"workspace" in err()
+
+
+def test_projection_gemms_reject_bad_arguments_before_any_cuda_call():
+    lib = capi.load()
+    err = lib.cca_b200_last_error
+    p, big = 16, 1 << 30                    # any non-null address: every check below comes before anything touches it
+    det = capi.CCA_FLAG_DETERMINISTIC
+    # name -> (pointer count, call(pointers, workspace bytes, pixels, C, Cq))
+    gemms = {
+        "project": (11, lambda ptrs, nb, px, C, Cq: lib.cca_b200_qkv_project(*ptrs, nb, px, C, Cq, None)),
+        "dgrad": (9, lambda ptrs, nb, px, C, Cq: lib.cca_b200_qkv_project_dgrad(*ptrs, nb, px, C, Cq, 0, None)),
+        "wgrad": (9, lambda ptrs, nb, px, C, Cq: lib.cca_b200_qkv_project_wgrad(*ptrs, px, C, Cq, None)),
+        "wgrad_ex": (9, lambda ptrs, nb, px, C, Cq: lib.cca_b200_qkv_project_wgrad_ex(*ptrs, px, C, Cq, p, nb, det, None)),
+    }
+    for name, (n, fn) in gemms.items():
+        def call(ptrs=(p,) * n, nbytes=big, px=64, C=64, Cq=64):
+            return fn(ptrs, nbytes, px, C, Cq)
+        assert call(ptrs=(None,) + (p,) * (n - 1)) == -1 and b"null" in err(), name
+        assert call(ptrs=(None,) * n, px=0) == -1 and b"null" in err(), name          # (null pointers are checked first)
+        for px, C, Cq in ((0, 64, 64), (-1, 64, 64), (1 << 31, 64, 64), (64, 0, 64), (64, 64, 0), (64, -64, 64)):
+            assert call(px=px, C=C, Cq=Cq) == -1 and b"dimension" in err(), (name, px, C, Cq)
+    for name in ("project", "dgrad"):
+        n, fn = gemms[name]
+        assert fn((p,) * n, 16, 64, 64, 64) == -3 and b"workspace" in err(), name
+        assert fn((p,) * (n - 1) + (None,), big, 64, 64, 64) == -1 and b"null" in err(), name    # the workspace
+    assert gemms["dgrad"][1]((p,) * 6 + (None, p, p), big, 0, 64, 64) == -1 and b"dimension" in err()   # scale may be NULL
+    assert gemms["wgrad"][1]((p,) * 8 + (None,), big, 0, 64, 64) == -1 and b"dimension" in err()       # db may be NULL
+    # the deterministic weight gradient needs its workspace; without the flag it may be NULL
+    assert lib.cca_b200_qkv_project_wgrad_ex(*(p,) * 9, 64, 64, 64, None, 0, det, None) == -1 and b"null" in err()
+    assert lib.cca_b200_qkv_project_wgrad_ex(*(p,) * 9, 0, 64, 64, None, 0, 0, None) == -1 and b"dimension" in err()
 
 
 def test_module_surface_matches_reference():
