@@ -193,10 +193,8 @@ size_t cca_b200_workspace_bytes(int which, int B, int Cq, int C, int H, int W, i
     (void)dtype;
     if (B <= 0 || Cq <= 0 || C <= 0 || H <= 0 || W <= 0) return 0;
     const Dims d{B, Cq, C, H, W};
-    const size_t pix = (size_t)B * H * W;
-    // generic kernels: per-pixel (m,l) of the column pass (forward) / delta (backward); tensor-core kernels: partial lse
-    // planes + zero-ahead counters (forward) / delta + counters (backward).  One size that covers whichever family runs.
-    const size_t simt = (which == CCA_WS_FORWARD ? pix * sizeof(float2) : pix * sizeof(float)) + 16;
+    // one size that covers whichever family runs
+    const size_t simt = simt_workspace(which, d);
     const size_t tcb = which == CCA_WS_FORWARD ? tc_forward_workspace(d) : tc_backward_workspace(d);
     return simt > tcb ? simt : tcb;
 }
@@ -245,7 +243,7 @@ int cca_b200_forward(const void *q, const void *k, const void *v, void *out, flo
         return CCA_OK;
     }
     if (!simt_supported(d, false)) return fail(CCA_ERR_UNSUPPORTED, "H or W too large for the generic kernels%s%s");
-    e = simt_forward(q, k, v, out, lse, ws, d, dtype, st, &why);
+    e = simt_forward(q, k, v, out, lse, ws, d, dtype, st);
     if (e != cudaSuccess) return cuda_fail(e, "simt_forward");
     return CCA_OK;
 }
@@ -274,8 +272,7 @@ int cca_b200_backward(const void *dout, const void *q, const void *k, const void
         return CCA_OK;
     }
     if (!simt_supported(d, true)) return fail(CCA_ERR_UNSUPPORTED, "H or W too large for the generic kernels%s%s");
-    cudaError_t e = simt_backward(dout, q, k, v, out, lse, dq, dk, dv, ws, d, dtype,
-                                  reinterpret_cast<cudaStream_t>(stream), &why);
+    cudaError_t e = simt_backward(dout, q, k, v, out, lse, dq, dk, dv, ws, d, dtype, reinterpret_cast<cudaStream_t>(stream));
     if (e != cudaSuccess) return cuda_fail(e, "simt_backward");
     return CCA_OK;
 }
@@ -308,7 +305,7 @@ size_t cca_b200_attention_workspace_bytes(int backward, int B, int Cq, int H, in
 {
     if (B <= 0 || Cq <= 0 || H <= 0 || W <= 0) return 0;
     const Dims d{B, Cq, 0, H, W};
-    const size_t simt = backward ? (size_t)B * H * W * sizeof(float) + 16 : 16;   // backward: rho
+    const size_t simt = simt_attention_workspace(backward, d);
     const size_t tcb = tc_attention_workspace(backward, d, attention_det_planes(d, dtype, flags));
     return simt > tcb ? simt : tcb;
 }

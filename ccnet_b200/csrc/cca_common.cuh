@@ -39,13 +39,45 @@ template <> __device__ __forceinline__ __half from_f<__half>(float x) { return _
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 
+// f(E{}) with E the element type of a cca_dtype: float, __nv_bfloat16 or __half
+template <typename F> decltype(auto) with_elem(int dtype, F &&f)
+{
+    if (dtype == CCA_F16) return f(__half{});
+    if (dtype == CCA_BF16) return f(__nv_bfloat16{});
+    return f(float{});
+}
+
+// device helpers of the generic kernels
+template <typename T> __device__ __forceinline__ float ldg_f(const T *p) { return to_f<T>(__ldg(p)); }
+__device__ __forceinline__ float warp_max(float x)
+{
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, o));
+    return x;
+}
+__device__ __forceinline__ float warp_sum(float x)
+{
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+    return x;
+}
+// grid of a grid-stride kernel with one warp per pixel and `warps` warps per block
+inline int warp_grid(long npix, int warps)
+{
+    const long want = (npix + warps - 1) / warps;
+    return (int)(want < (1L << 20) ? (want > 0 ? want : 1) : (1L << 20));
+}
+
 // host-side launchers (defined in the .cu files, called from cca_capi.cu)
+//   generic kernels, NCHW tensors (cca_simt.cu); the workspace is the column pass's (m, l) per pixel (forward) or delta
+//   (backward)
 cudaError_t simt_forward(const void *q, const void *k, const void *v, void *out, float *lse, void *ws,
-                         Dims d, int dtype, cudaStream_t st, const char **why);
+                         Dims d, int dtype, cudaStream_t st);
 cudaError_t simt_backward(const void *dout, const void *q, const void *k, const void *v, const void *out,
                           const float *lse, void *dq, void *dk, void *dv, void *ws, Dims d, int dtype,
-                          cudaStream_t st, const char **why);
+                          cudaStream_t st);
 bool simt_supported(Dims d, bool backward);
+size_t simt_workspace(int which, Dims d);
 
 bool tc_forward_supported(Dims d, int dtype);
 size_t tc_forward_workspace(Dims d);
@@ -56,9 +88,9 @@ cudaError_t tc_forward(const void *q, const void *k, const void *v, void *out, f
 // more planes of `parts`; `planes` is the planes-mode buffer (det on tiled lines)
 cudaError_t tc_values(const void *q, const void *k, const void *v, void *out, float *lse, const float *parts, unsigned int *cdone,
                       void *planes, Dims d, int dtype, cudaStream_t st, const char **why, bool det, int extra_parts);
-// statistics pre-pass of the tensor-core forward (cca_tc_stats.cu): partial lse planes; also clears a byte range and counters
-cudaError_t tc_stats(const void *q, const void *k, float *parts, void *zero_ptr, long zero_bytes, unsigned int *counters,
-                     int n_counters, Dims d, int dtype, cudaStream_t st, const char **why);
+// statistics pre-pass of the tensor-core forward (cca_tc_stats.cu): partial lse planes; also clears n_counters counters
+cudaError_t tc_stats(const void *q, const void *k, float *parts, unsigned int *counters, int n_counters, Dims d, int dtype,
+                     cudaStream_t st, const char **why);
 
 // deterministic mode on tiled lines (cca_tc_det.cu): fp32 planes-mode item kernels + the plane sum
 bool tc_tiled(Dims d);                          // a line longer than one tile in either direction
@@ -96,6 +128,7 @@ cudaError_t tc_backward3d(const void *dout, const void *q, const void *k, const 
 
 // the attention map attn[B,H,W,H+W] (fp32) and its gradient w.r.t. q, k (Dims.C is not used)
 //   generic kernels, NCHW q, k (cca_simt_attn.cu); the backward's workspace is rho [B*H*W]
+size_t simt_attention_workspace(int backward, Dims d);
 cudaError_t simt_attention_forward(const void *q, const void *k, float *attn, Dims d, int dtype, cudaStream_t st);
 cudaError_t simt_attention_backward(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk,
                                     void *ws, Dims d, int dtype, cudaStream_t st);

@@ -203,16 +203,7 @@ cudaError_t launch_gemm(GemmParams &gp, const PackParams &pp, const void *a[3], 
     if (e != cudaSuccess) return e;
     const int total = ((gp.P + kGM - 1) / kGM) * gp.n_chunks;
     const int sms = sm_count();
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(total < 2 * sms ? total : 2 * sms); cfg.blockDim = dim3(kGThreads); cfg.dynamicSmemBytes = 0; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = tc_pdl() ? 1 : 0;
-    e = cudaLaunchKernelEx(&cfg, cca_gemm_kernel, gp);
-    count_launch();
-    return e != cudaSuccess ? e : cudaGetLastError();
+    return launch_kernel(cca_gemm_kernel, total < 2 * sms ? total : 2 * sms, kGThreads, 0, true, st, gp);
 }
 
 // =====================================================================================================================

@@ -27,9 +27,6 @@ constexpr int kMB = 32;       // contraction block of line_apply
 constexpr int kXP = 132;      // pitch of the [kMB][128] staging tile of line_apply
 constexpr int kCChunk = 128;  // channels per chunk of line_apply (16 per warp)
 
-template <typename T>
-__device__ __forceinline__ float ldg_f(const T *p) { return to_f<T>(__ldg(p)); }
-
 // dst[jk*pitch + q] = sum_c X[c][q0+q] * Y[c][jk]   for q in [0,32R), jk in [0,L)
 // (rows of X/Y beyond the line length read as 0).  All 256 threads participate.
 template <typename T, int R>
@@ -431,23 +428,23 @@ bool simt_supported(Dims d, bool backward)
     return pick_r(d.H, backward) > 0 && pick_r(d.W, backward) > 0 && d.B <= 65535;
 }
 
-cudaError_t simt_forward(const void *q, const void *k, const void *v, void *out, float *lse, void *ws,
-                         Dims d, int dtype, cudaStream_t st, const char **why)
+size_t simt_workspace(int which, Dims d)
 {
-    (void)why;
-    if (dtype == CCA_F16) return fwd_typed<__half>(q, k, v, out, lse, ws, d, st);
-    return dtype == CCA_F32 ? fwd_typed<float>(q, k, v, out, lse, ws, d, st)
-                            : fwd_typed<__nv_bfloat16>(q, k, v, out, lse, ws, d, st);
+    const size_t pix = (size_t)d.B * d.H * d.W;
+    return (which == CCA_WS_FORWARD ? pix * sizeof(float2) : pix * sizeof(float)) + 16;
+}
+
+cudaError_t simt_forward(const void *q, const void *k, const void *v, void *out, float *lse, void *ws,
+                         Dims d, int dtype, cudaStream_t st)
+{
+    return with_elem(dtype, [&](auto e) { return fwd_typed<decltype(e)>(q, k, v, out, lse, ws, d, st); });
 }
 
 cudaError_t simt_backward(const void *dout, const void *q, const void *k, const void *v, const void *out,
                           const float *lse, void *dq, void *dk, void *dv, void *ws, Dims d, int dtype,
-                          cudaStream_t st, const char **why)
+                          cudaStream_t st)
 {
-    (void)why;
-    if (dtype == CCA_F16) return bwd_typed<__half>(dout, q, k, v, out, lse, dq, dk, dv, ws, d, st);
-    return dtype == CCA_F32 ? bwd_typed<float>(dout, q, k, v, out, lse, dq, dk, dv, ws, d, st)
-                            : bwd_typed<__nv_bfloat16>(dout, q, k, v, out, lse, dq, dk, dv, ws, d, st);
+    return with_elem(dtype, [&](auto e) { return bwd_typed<decltype(e)>(dout, q, k, v, out, lse, dq, dk, dv, ws, d, st); });
 }
 
 }  // namespace cca

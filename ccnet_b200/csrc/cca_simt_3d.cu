@@ -16,19 +16,6 @@ namespace {
 constexpr int kWarps3 = 4;
 constexpr int kThreads3 = 32 * kWarps3;
 
-__device__ __forceinline__ float warp_max3(float x)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, o));
-    return x;
-}
-__device__ __forceinline__ float warp_sum3(float x)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-    return x;
-}
-template <typename E> __device__ __forceinline__ float ld(const E *p) { return to_f<E>(__ldg(p)); }
 
 struct Pix {
     long b, off;   // sample, offset inside the sample's [T,H,W] volume
@@ -53,12 +40,6 @@ __device__ __forceinline__ int key_off(int i, const Pix &x, const Dims3 &d)
     return ((i < x.t ? i : i + 1) * d.H + x.h) * d.W + x.w;
 }
 
-int grid_for(long npix)
-{
-    const long want = (npix + kWarps3 - 1) / kWarps3;
-    return (int)(want < (1L << 20) ? (want > 0 ? want : 1) : (1L << 20));
-}
-
 // out = sum_j P_j v_j, lse = log sum_j exp(q . k_j)
 template <typename E>
 __global__ void __launch_bounds__(kThreads3) cca_simt3d_fwd_kernel(const E *__restrict__ q, const E *__restrict__ k,
@@ -77,18 +58,18 @@ __global__ void __launch_bounds__(kThreads3) cca_simt3d_fwd_kernel(const E *__re
         for (int i = lane; i < Le; i += 32) {
             const int o = key_off(i, x, d);
             float e = 0.f;
-            for (int c = 0; c < d.Cq; ++c) e = fmaf(ld(qp + c * vol), ld(kb + c * vol + o), e);
+            for (int c = 0; c < d.Cq; ++c) e = fmaf(ldg_f(qp + c * vol), ldg_f(kb + c * vol + o), e);
             row[i] = e; offs[i] = o;
             m = fmaxf(m, e);
         }
-        m = warp_max3(m);
+        m = warp_max(m);
         float l = 0.f;
         for (int i = lane; i < Le; i += 32) {
             const float pe = expf(row[i] - m);
             row[i] = pe;
             l += pe;
         }
-        l = warp_sum3(l);
+        l = warp_sum(l);
         const float inv = 1.f / l;
         for (int i = lane; i < Le; i += 32) row[i] *= inv;
         if (lane == 0) lse[p] = m + logf(l);
@@ -98,7 +79,7 @@ __global__ void __launch_bounds__(kThreads3) cca_simt3d_fwd_kernel(const E *__re
         for (int c = lane; c < d.C; c += 32) {
             const E *vc = vb + c * vol;
             float acc = 0.f;
-            for (int i = 0; i < Le; ++i) acc = fmaf(row[i], ld(vc + offs[i]), acc);
+            for (int i = 0; i < Le; ++i) acc = fmaf(row[i], ldg_f(vc + offs[i]), acc);
             op[c * vol] = from_f<E>(acc);
         }
         __syncwarp();
@@ -116,8 +97,8 @@ __global__ void __launch_bounds__(kThreads3) cca_simt3d_delta_kernel(const E *__
         const long b = p / vol, off = p - b * vol;
         const E *g = dout + b * d.C * vol + off, *o = out + b * d.C * vol + off;
         float s = 0.f;
-        for (int c = lane; c < d.C; c += 32) s = fmaf(ld(g + c * vol), ld(o + c * vol), s);
-        s = warp_sum3(s);
+        for (int c = lane; c < d.C; c += 32) s = fmaf(ldg_f(g + c * vol), ldg_f(o + c * vol), s);
+        s = warp_sum(s);
         if (lane == 0) delta[p] = s;
     }
 }
@@ -145,12 +126,12 @@ __global__ void __launch_bounds__(kThreads3) cca_simt3d_bwd_kernel(const E *__re
             const int o = key_off(i, x, d);
             float e1 = 0.f, e2 = 0.f, g1 = 0.f, g2 = 0.f;
             for (int c = 0; c < d.Cq; ++c) {
-                e1 = fmaf(ld(qb + c * vol + x.off), ld(kb + c * vol + o), e1);
-                e2 = fmaf(ld(qb + c * vol + o), ld(kb + c * vol + x.off), e2);
+                e1 = fmaf(ldg_f(qb + c * vol + x.off), ldg_f(kb + c * vol + o), e1);
+                e2 = fmaf(ldg_f(qb + c * vol + o), ldg_f(kb + c * vol + x.off), e2);
             }
             for (int c = 0; c < d.C; ++c) {
-                g1 = fmaf(ld(gb + c * vol + x.off), ld(vb + c * vol + o), g1);
-                g2 = fmaf(ld(gb + c * vol + o), ld(vb + c * vol + x.off), g2);
+                g1 = fmaf(ldg_f(gb + c * vol + x.off), ldg_f(vb + c * vol + o), g1);
+                g2 = fmaf(ldg_f(gb + c * vol + o), ldg_f(vb + c * vol + x.off), g2);
             }
             const float p1 = expf(e1 - lse_p), p2 = expf(e2 - lse[s0 + o]);
             sq[i] = p1 * (g1 - delta_p);
@@ -163,8 +144,8 @@ __global__ void __launch_bounds__(kThreads3) cca_simt3d_bwd_kernel(const E *__re
             const E *kc = kb + c * vol, *qc = qb + c * vol;
             float a = 0.f, b = 0.f;
             for (int i = 0; i < Le; ++i) {
-                a = fmaf(sq[i], ld(kc + offs[i]), a);
-                b = fmaf(sk[i], ld(qc + offs[i]), b);
+                a = fmaf(sq[i], ldg_f(kc + offs[i]), a);
+                b = fmaf(sk[i], ldg_f(qc + offs[i]), b);
             }
             dq[sq0 + c * vol + x.off] = from_f<E>(a);
             dk[sq0 + c * vol + x.off] = from_f<E>(b);
@@ -172,7 +153,7 @@ __global__ void __launch_bounds__(kThreads3) cca_simt3d_bwd_kernel(const E *__re
         for (int c = lane; c < d.C; c += 32) {
             const E *gc = gb + c * vol;
             float a = 0.f;
-            for (int i = 0; i < Le; ++i) a = fmaf(pk[i], ld(gc + offs[i]), a);
+            for (int i = 0; i < Le; ++i) a = fmaf(pk[i], ldg_f(gc + offs[i]), a);
             dv[sv0 + c * vol + x.off] = from_f<E>(a);
         }
         __syncwarp();
@@ -186,7 +167,7 @@ cudaError_t fwd3(const void *q, const void *k, const void *v, void *out, float *
     const size_t smem = (size_t)kWarps3 * 2 * (d.H + d.W + d.T - 2) * sizeof(float);
     cudaError_t e = cudaFuncSetAttribute(cca_simt3d_fwd_kernel<E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    cca_simt3d_fwd_kernel<E><<<grid_for(npix), kThreads3, smem, st>>>(static_cast<const E *>(q), static_cast<const E *>(k),
+    cca_simt3d_fwd_kernel<E><<<warp_grid(npix, kWarps3), kThreads3, smem, st>>>(static_cast<const E *>(q), static_cast<const E *>(k),
                                                                        static_cast<const E *>(v), static_cast<E *>(out), lse, d);
     count_launch();
     return cudaGetLastError();
@@ -197,15 +178,15 @@ cudaError_t bwd3(const void *dout, const void *q, const void *k, const void *v, 
                  void *dk, void *dv, float *delta, Dims3 d, cudaStream_t st)
 {
     const long npix = (long)d.B * d.T * d.H * d.W;
-    cca_simt3d_delta_kernel<E><<<grid_for(npix), kThreads3, 0, st>>>(static_cast<const E *>(dout), static_cast<const E *>(out),
-                                                                      delta, d);
+    cca_simt3d_delta_kernel<E><<<warp_grid(npix, kWarps3), kThreads3, 0, st>>>(static_cast<const E *>(dout),
+                                                                                  static_cast<const E *>(out), delta, d);
     count_launch();
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     const size_t smem = (size_t)kWarps3 * 4 * (d.H + d.W + d.T - 2) * sizeof(float);
     if ((e = cudaFuncSetAttribute(cca_simt3d_bwd_kernel<E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
         return e;
-    cca_simt3d_bwd_kernel<E><<<grid_for(npix), kThreads3, smem, st>>>(
+    cca_simt3d_bwd_kernel<E><<<warp_grid(npix, kWarps3), kThreads3, smem, st>>>(
         static_cast<const E *>(dout), static_cast<const E *>(q), static_cast<const E *>(k), static_cast<const E *>(v), lse,
         delta, static_cast<E *>(dq), static_cast<E *>(dk), static_cast<E *>(dv), d);
     count_launch();
@@ -227,18 +208,14 @@ size_t simt3d_workspace(int which, Dims3 d)
 
 cudaError_t simt_forward3d(const void *q, const void *k, const void *v, void *out, float *lse, Dims3 d, int dtype, cudaStream_t st)
 {
-    if (dtype == CCA_F16) return fwd3<__half>(q, k, v, out, lse, d, st);
-    if (dtype == CCA_BF16) return fwd3<__nv_bfloat16>(q, k, v, out, lse, d, st);
-    return fwd3<float>(q, k, v, out, lse, d, st);
+    return with_elem(dtype, [&](auto e) { return fwd3<decltype(e)>(q, k, v, out, lse, d, st); });
 }
 
 cudaError_t simt_backward3d(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
                             void *dq, void *dk, void *dv, void *ws, Dims3 d, int dtype, cudaStream_t st)
 {
     float *delta = reinterpret_cast<float *>(ws);
-    if (dtype == CCA_F16) return bwd3<__half>(dout, q, k, v, out, lse, dq, dk, dv, delta, d, st);
-    if (dtype == CCA_BF16) return bwd3<__nv_bfloat16>(dout, q, k, v, out, lse, dq, dk, dv, delta, d, st);
-    return bwd3<float>(dout, q, k, v, out, lse, dq, dk, dv, delta, d, st);
+    return with_elem(dtype, [&](auto e) { return bwd3<decltype(e)>(dout, q, k, v, out, lse, dq, dk, dv, delta, d, st); });
 }
 
 }  // namespace cca

@@ -9,30 +9,8 @@ namespace {
 
 constexpr int kThreads = 256;
 
-template <typename T>
-__device__ __forceinline__ float ldg_f(const T *p) { return to_f<T>(__ldg(p)); }
-
 // attn[b,h,w,g]: g < H column key (g, w), g >= H row key (h, g - H)
 constexpr int kMapWarps = kThreads / 32;
-
-int map_grid(long npix)
-{
-    const long want = (npix + kMapWarps - 1) / kMapWarps;
-    return (int)(want < (1L << 20) ? (want > 0 ? want : 1) : (1L << 20));
-}
-
-__device__ __forceinline__ float warp_max(float x)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, o));
-    return x;
-}
-__device__ __forceinline__ float warp_sum(float x)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-    return x;
-}
 
 // offset (inside a sample's [H,W] plane) of key g of pixel (h, w)
 __device__ __forceinline__ long map_key(int g, int h, int w, Dims d) { return g < d.H ? (long)g * d.W + w : (long)h * d.W + (g - d.H); }
@@ -144,7 +122,7 @@ template <typename T>
 cudaError_t attn_fwd_typed(const void *q, const void *k, float *attn, Dims d, cudaStream_t st)
 {
     const long npix = (long)d.B * d.H * d.W;
-    cca_attn_map_kernel<T><<<map_grid(npix), kThreads, 0, st>>>((const T *)q, (const T *)k, attn, d);
+    cca_attn_map_kernel<T><<<warp_grid(npix, kMapWarps), kThreads, 0, st>>>((const T *)q, (const T *)k, attn, d);
     count_launch();
     return cudaGetLastError();
 }
@@ -157,10 +135,10 @@ cudaError_t attn_bwd_typed(const float *dattn, const float *attn, const void *q,
     float *rho = reinterpret_cast<float *>(ws);
     cudaError_t e = attn_rho(dattn, attn, rho, npix, d.H + d.W, nullptr, nullptr, 0, st);
     if (e != cudaSuccess) return e;
-    cca_attn_dq_kernel<T><<<map_grid(npix), kThreads, 0, st>>>(dattn, attn, rho, (const T *)k, (T *)dq, d);
+    cca_attn_dq_kernel<T><<<warp_grid(npix, kMapWarps), kThreads, 0, st>>>(dattn, attn, rho, (const T *)k, (T *)dq, d);
     count_launch();
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    cca_attn_dk_kernel<T><<<map_grid(npix), kThreads, 0, st>>>(dattn, attn, rho, (const T *)q, (T *)dk, d);
+    cca_attn_dk_kernel<T><<<warp_grid(npix, kMapWarps), kThreads, 0, st>>>(dattn, attn, rho, (const T *)q, (T *)dk, d);
     count_launch();
     return cudaGetLastError();
 }
@@ -170,24 +148,23 @@ cudaError_t attn_bwd_typed(const float *dattn, const float *attn, const void *q,
 cudaError_t attn_rho(const float *dattn, const float *attn, float *rho, long npix, int hw2, void *c0, void *c1, long clear_bytes,
                      cudaStream_t st)
 {
-    cca_attn_rho_kernel<<<map_grid(npix), kThreads, 0, st>>>(dattn, attn, rho, npix, hw2, reinterpret_cast<uint4 *>(c0),
+    cca_attn_rho_kernel<<<warp_grid(npix, kMapWarps), kThreads, 0, st>>>(dattn, attn, rho, npix, hw2, reinterpret_cast<uint4 *>(c0),
                                                            reinterpret_cast<uint4 *>(c1), clear_bytes / 16);
     count_launch();
     return cudaGetLastError();
 }
 
+size_t simt_attention_workspace(int backward, Dims d) { return backward ? (size_t)d.B * d.H * d.W * sizeof(float) + 16 : 16; }
+
 cudaError_t simt_attention_forward(const void *q, const void *k, float *attn, Dims d, int dtype, cudaStream_t st)
 {
-    if (dtype == CCA_F16) return attn_fwd_typed<__half>(q, k, attn, d, st);
-    return dtype == CCA_F32 ? attn_fwd_typed<float>(q, k, attn, d, st) : attn_fwd_typed<__nv_bfloat16>(q, k, attn, d, st);
+    return with_elem(dtype, [&](auto e) { return attn_fwd_typed<decltype(e)>(q, k, attn, d, st); });
 }
 
 cudaError_t simt_attention_backward(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk,
                                     void *ws, Dims d, int dtype, cudaStream_t st)
 {
-    if (dtype == CCA_F16) return attn_bwd_typed<__half>(dattn, attn, q, k, dq, dk, ws, d, st);
-    return dtype == CCA_F32 ? attn_bwd_typed<float>(dattn, attn, q, k, dq, dk, ws, d, st)
-                            : attn_bwd_typed<__nv_bfloat16>(dattn, attn, q, k, dq, dk, ws, d, st);
+    return with_elem(dtype, [&](auto e) { return attn_bwd_typed<decltype(e)>(dattn, attn, q, k, dq, dk, ws, d, st); });
 }
 
 }  // namespace cca

@@ -39,10 +39,20 @@
 namespace cca {
 namespace tc {
 
-template <int LK, typename E, bool PL = false>
-cudaError_t launch_bwd(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse, float *delta,
-                       unsigned int *counters, void *dq, void *dk, void *dv, Dims d, int delta_mode, cudaStream_t st,
-                       const char **why);
+// PL: dq, dk, dv are the [nparts*B, H, W, Cq or C] plane buffers (cca_tc_det.cu sums them into the gradients).  delta and
+// counters: the workspace's [B,H,W] delta and [3*B] counters
+struct BwdArgs {
+    const void *dout, *q, *k, *v, *out;
+    const float *lse;
+    float *delta;
+    unsigned int *counters;
+    void *dq, *dk, *dv;
+    Dims d;
+    int delta_mode;
+    cudaStream_t st;
+    const char **why;
+};
+template <int LK, typename E, bool PL = false> cudaError_t launch_bwd(const BwdArgs &a);
 
 struct BwdParams {
     ItemSpace sp;
@@ -569,76 +579,44 @@ __global__ void __launch_bounds__(256) cca_bwd_prep_kernel(uint4 *dq, uint4 *dk,
 }
 }  // namespace
 
-// PL: dq, dk, dv are the [nparts*B, H, W, Cq or C] plane buffers (cca_tc_det.cu sums them into the gradients)
-template <int LK, typename E, bool PL>
-cudaError_t launch_bwd(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse, float *delta,
-                       unsigned int *counters, void *dq, void *dk, void *dv, Dims d, int delta_mode, cudaStream_t st,
-                       const char **why)
+template <int LK, typename E, bool PL> cudaError_t launch_bwd(const BwdArgs &a)
 {
     CUtensorMap m[16];
-    const void *base[8] = {q, k, v, dout, out, dq, dk, dv};
-    const int ch[8] = {d.Cq, d.Cq, d.C, d.C, d.C, d.Cq, d.Cq, d.C};
+    const Dims &d = a.d;
     BwdParams p;
     p.sp = make_space(d.B, d.H, d.W);
-    for (int t = 0; t < 8; ++t)
-        for (int r = 0; r < 2; ++r) {
-            // loads: LK-pixel boxes, zero-filled past the line; outputs: boxes of one tile of the direction, so a store never
-            // reaches into the next tile of a line (pixels past the line are not written)
-            const int box = t < 5 ? LK : (r == 0 ? p.sp.col.tl : p.sp.row.tl);
-            const int nb = PL && t >= 5 ? p.sp.nparts * d.B : d.B;
-            if (!get_map(&m[2 * t + r], base[t], nb, d.H, d.W, ch[t], box, r == 0, kDtype<E>)) {
-                if (why) *why = "cuTensorMapEncodeTiled failed";
-                return cudaErrorInvalidValue;
-            }
-        }
+    // loads: LK-pixel boxes, zero-filled past the line; outputs: boxes of one tile of the direction, so a store never reaches
+    // into the next tile of a line (pixels past the line are not written)
+    const int nb = PL ? p.sp.nparts * d.B : d.B, bc = p.sp.col.tl, br = p.sp.row.tl;
+    if (cudaError_t e = get_maps(m, {{a.q, d.B, d.Cq, LK, LK}, {a.k, d.B, d.Cq, LK, LK}, {a.v, d.B, d.C, LK, LK},
+                                     {a.dout, d.B, d.C, LK, LK}, {a.out, d.B, d.C, LK, LK}, {a.dq, nb, d.Cq, bc, br},
+                                     {a.dk, nb, d.Cq, bc, br}, {a.dv, nb, d.C, bc, br}},
+                                 d, kDtype<E>, a.why))
+        return e;
     p.C = d.C; p.Cq = d.Cq;
     p.npix = (long)d.B * d.H * d.W;
-    p.lse = lse; p.delta = delta;
-    p.ddone = counters; p.cdone = counters + d.B;
-    p.delta_mode = delta_mode;
+    p.lse = a.lse; p.delta = a.delta;
+    p.ddone = a.counters; p.cdone = a.counters + d.B;
+    p.delta_mode = a.delta_mode;
     const bool one_tile = p.sp.col.nt == 1 && p.sp.row.nt == 1;
     p.out_mode = one_tile || PL ? 1 : 0;          // (PL: every item stores; 1 only skips the clear below)
     p.lag = tc_lag() != 0 ? 1 : 0;
     const long es = sizeof(E);
     const long nq = p.out_mode == 1 ? 0 : p.npix * d.Cq * es, nv = p.out_mode == 1 ? 0 : p.npix * d.C * es;
-    cca_bwd_prep_kernel<<<p.out_mode == 1 ? 1 : sm_count(), 256, 0, st>>>(
-        reinterpret_cast<uint4 *>(dq), reinterpret_cast<uint4 *>(dk), reinterpret_cast<uint4 *>(dv), nq / 16, nv / 16, counters, 3 * d.B);
+    cca_bwd_prep_kernel<<<p.out_mode == 1 ? 1 : sm_count(), 256, 0, a.st>>>(
+        reinterpret_cast<uint4 *>(a.dq), reinterpret_cast<uint4 *>(a.dk), reinterpret_cast<uint4 *>(a.dv), nq / 16, nv / 16, a.counters,
+        3 * d.B);
     count_launch();
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    auto kern = cca_tc_bwd_kernel<LK, E, PL>;
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem<LK, E>::kBytes);
-    if (e != cudaSuccess) return e;
-    const int sms = sm_count();
-    const int grid = p.sp.total < sms ? p.sp.total : sms;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = BwdSmem<LK, E>::kBytes; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = tc_pdl() ? 1 : 0;
-    e = cudaLaunchKernelEx(&cfg, kern, m[0], m[1], m[2], m[3], m[4], m[5], m[6], m[7], m[8], m[9], m[10], m[11], m[12], m[13],
-                           m[14], m[15], p);
-    count_launch();
-    return e != cudaSuccess ? e : cudaGetLastError();
+    if (cudaError_t e = cudaGetLastError()) return e;
+    return launch_kernel(cca_tc_bwd_kernel<LK, E, PL>, item_grid(p.sp), kThreads, BwdSmem<LK, E>::kBytes, true, a.st, m[0], m[1], m[2],
+                         m[3], m[4], m[5], m[6], m[7], m[8], m[9], m[10], m[11], m[12], m[13], m[14], m[15], p);
 }
 
-
-// The f16 instantiations live in their own translation unit (cca_tc_f16.cu).
-extern template cudaError_t launch_bwd<80, __half>(const void *, const void *, const void *, const void *, const void *, const float *,
-                                                   float *, unsigned int *, void *, void *, void *, Dims, int, cudaStream_t,
-                                                   const char **);
-extern template cudaError_t launch_bwd<112, __half>(const void *, const void *, const void *, const void *, const void *, const float *,
-                                                    float *, unsigned int *, void *, void *, void *, Dims, int, cudaStream_t,
-                                                    const char **);
-// The planes-mode instantiations (fp32) live in cca_tc_det.cu.
-extern template cudaError_t launch_bwd<80, float, true>(const void *, const void *, const void *, const void *, const void *,
-                                                        const float *, float *, unsigned int *, void *, void *, void *, Dims, int,
-                                                        cudaStream_t, const char **);
-extern template cudaError_t launch_bwd<112, float, true>(const void *, const void *, const void *, const void *, const void *,
-                                                         const float *, float *, unsigned int *, void *, void *, void *, Dims, int,
-                                                         cudaStream_t, const char **);
+// The f16 instantiations live in their own translation unit (cca_tc_f16.cu), the planes-mode ones (fp32) in cca_tc_det.cu.
+extern template cudaError_t launch_bwd<80, __half>(const BwdArgs &);
+extern template cudaError_t launch_bwd<112, __half>(const BwdArgs &);
+extern template cudaError_t launch_bwd<80, float, true>(const BwdArgs &);
+extern template cudaError_t launch_bwd<112, float, true>(const BwdArgs &);
 
 }  // namespace tc
 }  // namespace cca

@@ -1,10 +1,13 @@
 // Pieces shared by the wgmma statistics, forward and backward kernels (channels-last; fp32 I/O as a bf16x3 split, or bf16 or
 // f16 I/O).
 #pragma once
+#include <initializer_list>
 #include <mutex>
 #include <type_traits>
+#include <utility>
 
 #include "cca_common.cuh"
+#include "cca_items.cuh"
 #include "cca_sm90.cuh"
 
 namespace cca {
@@ -221,18 +224,130 @@ inline bool make_map(CUtensorMap *m, const void *base, int B, int H, int W, int 
                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
-// byte offsets of the workspace's plane buffers (256-byte aligned; TMA needs 16)
-inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 // LK template (padded tile length) for the longest tile of a problem
 inline int lk_for(int tile) { return tile <= 80 ? 80 : (tile <= 112 ? 112 : 0); }
+// f(std::integral_constant<int, LK>{}): the LK instantiation that serves the lines of d
+template <typename F> decltype(auto) with_tile(Dims d, F &&f)
+{
+    if (lk_for(max_tile(make_space(d.B, d.H, d.W))) == 80) return f(std::integral_constant<int, 80>{});
+    return f(std::integral_constant<int, 112>{});
+}
+// f(E{}, std::integral_constant<int, LK>{}): the instantiation that serves `dtype` on the lines of d
+template <typename F> decltype(auto) with_elem_tile(int dtype, Dims d, F &&f)
+{
+    return with_elem(dtype, [&](auto e) { return with_tile(d, [&](auto lk) { return f(e, lk); }); });
+}
 // Cached tensor maps (cca_tc_host.cu): encoding costs ~1 us of driver time per map and an op call needs 8-15 of them;
 // a map only depends on (base, shape, box, dtype), so it stays valid for as long as that address holds such a tensor.
 bool get_map(CUtensorMap *m, const void *base, int B, int H, int W, int C, int LK, bool col, int dtype);
+// One tensor of a launch: [B, H, W, C] at base, boxes of box_col pixels down a column and box_row pixels along a row
+struct MapSpec {
+    const void *base;
+    int B, C, box_col, box_row;
+};
+// m[2t], m[2t + 1]: the column and row maps of tensor t (H, W from d); cudaErrorInvalidValue and *why set if one fails
+cudaError_t get_maps(CUtensorMap *m, std::initializer_list<MapSpec> tensors, Dims d, int dtype, const char **why);
 // SM count of the CURRENT device (cached per device id)
 int sm_count();
+// One launch: sets the kernel's dynamic shared memory limit when it uses any, lets it start ahead of the previous launch on
+// the stream (programmatic dependent launch; the kernel waits with griddepcontrol.wait) when `pdl` and tc_pdl() are on,
+// and counts it.
+template <typename... Params, typename... Args>
+cudaError_t launch_kernel(void (*kern)(Params...), dim3 grid, dim3 block, size_t smem, bool pdl, cudaStream_t st, Args &&...args)
+{
+    cudaError_t e;
+    if (smem > 0 && (e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
+        return e;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = pdl && tc_pdl() ? 1 : 0;
+    e = cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
+    count_launch();
+    return e != cudaSuccess ? e : cudaGetLastError();
+}
+// persistent item kernels: one CTA per SM, fewer if there are fewer items
+inline int item_grid(const ItemSpace &sp)
+{
+    const int sms = sm_count();
+    return sp.total < sms ? sp.total : sms;
+}
 // dst[t] = sum of the nparts planes [nparts][n[t]] at src[t], added in plane order, for count <= 3 tensors; launched with
 // programmatic dependent launch after the kernel that writes the planes (cca_tc_det.cu)
 cudaError_t planes_sum(const float *const *src, float *const *dst, const long *n, int count, int nparts, cudaStream_t st);
+
+// ---- workspace layouts: each computes its buffers' places once, for the op that carves them and (base nullptr) for the
+// size query.  Sizes are part of the C ABI (callers allocate by them) and must not change.
+inline size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
+inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+template <typename T> T *ws_at(void *base, size_t off) { return reinterpret_cast<T *>(reinterpret_cast<uintptr_t>(base) + off); }
+// forward (2D, and the 3D op on the frames view with extra_parts = 1 for its time plane): [nparts + extra_parts][B*H*W] fp32
+// partial lse planes, then [B] per-sample counters of the values kernel, each rounded up to 16 bytes; the planes-mode
+// buffers (planes_ws) follow at `planes`
+struct FwdWs {
+    float *parts;
+    unsigned int *cdone;
+    void *planes;
+    size_t bytes;
+};
+inline FwdWs fwd_ws(Dims d, int extra_parts, void *base)
+{
+    const size_t npix = (size_t)d.B * d.H * d.W;
+    const size_t parts = align16((make_space(d.B, d.H, d.W).nparts + extra_parts) * npix * sizeof(float));
+    const size_t bytes = parts + align16((size_t)d.B * sizeof(unsigned int));
+    return {ws_at<float>(base, 0), ws_at<unsigned int>(base, parts), ws_at<void>(base, bytes), bytes};
+}
+// backward (2D, and the 3D op on the frames view): delta [B*H*W] fp32, then [3*B] per-sample counters, each rounded up to
+// 16 bytes; the planes-mode buffers follow at `planes`
+struct BwdWs {
+    float *delta;
+    unsigned int *counters;
+    void *planes;
+    size_t bytes;
+};
+inline BwdWs bwd_ws(Dims d, void *base)
+{
+    const size_t delta = align16((size_t)d.B * d.H * d.W * sizeof(float));
+    const size_t bytes = delta + align16(3 * (size_t)d.B * sizeof(unsigned int));
+    return {ws_at<float>(base, 0), ws_at<unsigned int>(base, delta), ws_at<void>(base, bytes), bytes};
+}
+// planes mode (deterministic, tiled lines): one [nparts*B, H, W, c] fp32 plane buffer per entry of `channels`, each at a
+// 256-byte boundary (TMA needs 16) from `at` rounded up to 256; the extra 256 bytes pay for that rounding
+struct PlanesWs {
+    float *p[3];
+    size_t bytes;
+};
+inline PlanesWs planes_ws(Dims d, std::initializer_list<int> channels, void *at)
+{
+    const size_t per = (size_t)make_space(d.B, d.H, d.W).nparts * d.B * d.H * d.W * sizeof(float);
+    void *base = reinterpret_cast<void *>(align256(reinterpret_cast<uintptr_t>(at)));
+    PlanesWs w = {};
+    size_t off = 0;
+    int i = 0;
+    for (int c : channels) {
+        w.p[i++] = ws_at<float>(base, off);
+        off += align256(per * c);
+    }
+    w.bytes = off + 256;
+    return w;
+}
+// attention-map backward: rho [B*H*W] fp32 rounded up to 256 bytes, then (det, tiled lines) the dQ and dK planes
+struct AttnBwdWs {
+    float *rho;
+    PlanesWs planes;
+    size_t bytes;
+};
+inline AttnBwdWs attn_bwd_ws(Dims d, bool det, void *base)
+{
+    const size_t rho = align256((size_t)d.B * d.H * d.W * sizeof(float));
+    AttnBwdWs w = {ws_at<float>(base, 0), planes_ws(d, {d.Cq, d.Cq}, ws_at<void>(base, rho)), rho};
+    if (det && tc_tiled(d)) w.bytes += w.planes.bytes;
+    return w;
+}
+
 // the shapes the kernels are written for (no device query)
 inline bool shape_fits(Dims d, int dtype)
 {

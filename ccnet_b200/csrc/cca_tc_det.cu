@@ -8,16 +8,10 @@
 namespace cca {
 namespace tc {
 
-template cudaError_t launch_fwd<80, float, true>(const void *, const void *, const void *, void *, float *, const float *,
-                                                 unsigned int *, Dims, cudaStream_t, const char **, int);
-template cudaError_t launch_fwd<112, float, true>(const void *, const void *, const void *, void *, float *, const float *,
-                                                  unsigned int *, Dims, cudaStream_t, const char **, int);
-template cudaError_t launch_bwd<80, float, true>(const void *, const void *, const void *, const void *, const void *, const float *,
-                                                 float *, unsigned int *, void *, void *, void *, Dims, int, cudaStream_t,
-                                                 const char **);
-template cudaError_t launch_bwd<112, float, true>(const void *, const void *, const void *, const void *, const void *, const float *,
-                                                  float *, unsigned int *, void *, void *, void *, Dims, int, cudaStream_t,
-                                                  const char **);
+template cudaError_t launch_fwd<80, float, true>(const FwdArgs &);
+template cudaError_t launch_fwd<112, float, true>(const FwdArgs &);
+template cudaError_t launch_bwd<80, float, true>(const BwdArgs &);
+template cudaError_t launch_bwd<112, float, true>(const BwdArgs &);
 
 namespace {
 struct PlaneSums {
@@ -60,16 +54,7 @@ cudaError_t planes_sum(const float *const *src, float *const *dst, const long *n
     p.count = count; p.nparts = nparts;
     const long want = (total + 255) / 256;
     const int grid = (int)(want < 8L * sm_count() ? (want > 0 ? want : 1) : 8L * sm_count());
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(256); cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = tc_pdl() ? 1 : 0;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, cca_planes_sum_kernel, p);
-    count_launch();
-    return e != cudaSuccess ? e : cudaGetLastError();
+    return launch_kernel(cca_planes_sum_kernel, grid, 256, 0, true, st, p);
 }
 
 }  // namespace tc
@@ -85,44 +70,35 @@ bool tc_tiled(Dims d)
 size_t tc_planes_bytes(int which, Dims d)
 {
     if (!tc_tiled(d)) return 0;
-    const size_t per = (size_t)make_space(d.B, d.H, d.W).nparts * d.B * d.H * d.W * sizeof(float);
-    return (which == CCA_WS_FORWARD ? align256(per * d.C) : 2 * align256(per * d.Cq) + align256(per * d.C)) + 256;
+    return which == CCA_WS_FORWARD ? planes_ws(d, {d.C}, nullptr).bytes : planes_ws(d, {d.Cq, d.Cq, d.C}, nullptr).bytes;
 }
 
 cudaError_t tc_forward_planes(const void *q, const void *k, const void *v, float *out, float *lse, const float *parts,
                               unsigned int *cdone, void *planes, Dims d, cudaStream_t st, const char **why, int extra_parts)
 {
-    const ItemSpace sp = make_space(d.B, d.H, d.W);
-    const int lk = lk_for(max_tile(sp));
-    float *po = reinterpret_cast<float *>((reinterpret_cast<uintptr_t>(planes) + 255) & ~(uintptr_t)255);
-    cudaError_t e = lk == 80 ? launch_fwd<80, float, true>(q, k, v, po, lse, parts, cdone, d, st, why, extra_parts)
-                             : launch_fwd<112, float, true>(q, k, v, po, lse, parts, cdone, d, st, why, extra_parts);
+    float *po = planes_ws(d, {d.C}, planes).p[0];
+    const FwdArgs a{q, k, v, po, lse, parts, cdone, d, st, why, extra_parts};
+    cudaError_t e = with_tile(d, [&](auto lk) { return launch_fwd<lk(), float, true>(a); });
     if (e != cudaSuccess) return e;
     const float *src[1] = {po};
     float *dst[1] = {out};
     const long n[1] = {(long)d.B * d.H * d.W * d.C};
-    return planes_sum(src, dst, n, 1, sp.nparts, st);
+    return planes_sum(src, dst, n, 1, make_space(d.B, d.H, d.W).nparts, st);
 }
 
 cudaError_t tc_backward_planes(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
                                float *delta, unsigned int *counters, float *dq, float *dk, float *dv, void *planes, Dims d,
                                int delta_mode, cudaStream_t st, const char **why)
 {
-    const ItemSpace sp = make_space(d.B, d.H, d.W);
-    const size_t per = (size_t)sp.nparts * d.B * d.H * d.W * sizeof(float);
-    // 256-byte aligned plane buffers inside the workspace (TMA needs 16)
-    uint8_t *base = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(planes) + 255) & ~(uintptr_t)255);
-    float *pq = reinterpret_cast<float *>(base), *pk = reinterpret_cast<float *>(base + align256(per * d.Cq));
-    float *pv = reinterpret_cast<float *>(base + 2 * align256(per * d.Cq));
-    const int lk = lk_for(max_tile(sp));
-    cudaError_t e = lk == 80 ? launch_bwd<80, float, true>(dout, q, k, v, out, lse, delta, counters, pq, pk, pv, d, delta_mode, st, why)
-                             : launch_bwd<112, float, true>(dout, q, k, v, out, lse, delta, counters, pq, pk, pv, d, delta_mode, st, why);
+    const PlanesWs w = planes_ws(d, {d.Cq, d.Cq, d.C}, planes);
+    const BwdArgs a{dout, q, k, v, out, lse, delta, counters, w.p[0], w.p[1], w.p[2], d, delta_mode, st, why};
+    cudaError_t e = with_tile(d, [&](auto lk) { return launch_bwd<lk(), float, true>(a); });
     if (e != cudaSuccess) return e;
     const long npix = (long)d.B * d.H * d.W;
-    const float *src[3] = {pq, pk, pv};
+    const float *src[3] = {w.p[0], w.p[1], w.p[2]};
     float *dst[3] = {dq, dk, dv};
     const long n[3] = {npix * d.Cq, npix * d.Cq, npix * d.C};
-    return planes_sum(src, dst, n, 3, sp.nparts, st);
+    return planes_sum(src, dst, n, 3, make_space(d.B, d.H, d.W).nparts, st);
 }
 
 }  // namespace cca

@@ -8,18 +8,12 @@
 namespace cca {
 namespace tc {
 
-template cudaError_t launch_stats<80, __half>(const void *, const void *, float *, void *, long, unsigned int *, int, Dims,
-                                            cudaStream_t, const char **);
-template cudaError_t launch_stats<112, __half>(const void *, const void *, float *, void *, long, unsigned int *, int, Dims,
-                                             cudaStream_t, const char **);
-template cudaError_t launch_fwd<80, __half>(const void *, const void *, const void *, void *, float *, const float *, unsigned int *,
-                                            Dims, cudaStream_t, const char **, int);
-template cudaError_t launch_fwd<112, __half>(const void *, const void *, const void *, void *, float *, const float *, unsigned int *,
-                                             Dims, cudaStream_t, const char **, int);
-template cudaError_t launch_bwd<80, __half>(const void *, const void *, const void *, const void *, const void *, const float *,
-                                            float *, unsigned int *, void *, void *, void *, Dims, int, cudaStream_t, const char **);
-template cudaError_t launch_bwd<112, __half>(const void *, const void *, const void *, const void *, const void *, const float *,
-                                             float *, unsigned int *, void *, void *, void *, Dims, int, cudaStream_t, const char **);
+template cudaError_t launch_stats<80, __half>(const StatsArgs &);
+template cudaError_t launch_stats<112, __half>(const StatsArgs &);
+template cudaError_t launch_fwd<80, __half>(const FwdArgs &);
+template cudaError_t launch_fwd<112, __half>(const FwdArgs &);
+template cudaError_t launch_bwd<80, __half>(const BwdArgs &);
+template cudaError_t launch_bwd<112, __half>(const BwdArgs &);
 
 }  // namespace tc
 }  // namespace cca

@@ -45,11 +45,21 @@
 namespace cca {
 namespace tc {
 
-// extra_parts: planes of `parts` past the statistics pass's own (the time branch of the 3D op, cca_tc_time.cu) that the final
-// lse combines too; the item space and the planes-mode output buffer stay those of the 2D problem
-template <int LK, typename E, bool PL = false>
-cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, float *lse, const float *parts, unsigned int *cdone,
-                       Dims d, cudaStream_t st, const char **why, int extra_parts = 0);
+// PL: `out` is the [nparts*B, H, W, C] plane buffer (cca_tc_det.cu sums it into the output).  extra_parts: planes of `parts`
+// past the statistics pass's own (the time branch of the 3D op, cca_tc_time.cu) that the final lse combines too; the item
+// space and the planes-mode output buffer stay those of the 2D problem
+struct FwdArgs {
+    const void *q, *k, *v;
+    void *out;
+    float *lse;
+    const float *parts;
+    unsigned int *cdone;
+    Dims d;
+    cudaStream_t st;
+    const char **why;
+    int extra_parts;
+};
+template <int LK, typename E, bool PL = false> cudaError_t launch_fwd(const FwdArgs &a);
 
 struct FwdParams {
     ItemSpace sp;
@@ -344,34 +354,24 @@ cca_tc_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant
     }
 }
 
-// PL: `out` is the [nparts*B, H, W, C] plane buffer (cca_tc_det.cu sums it into the output)
-template <int LK, typename E, bool PL>
-cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, float *lse, const float *parts, unsigned int *cdone,
-                       Dims d, cudaStream_t st, const char **why, int extra_parts)
+template <int LK, typename E, bool PL> cudaError_t launch_fwd(const FwdArgs &a)
 {
     CUtensorMap m[8];
-    const void *base[4] = {q, k, v, out};
-    const int ch[4] = {d.Cq, d.Cq, d.C, d.C};
+    const Dims &d = a.d;
     FwdParams p;
     p.sp = make_space(d.B, d.H, d.W);
-    for (int t = 0; t < 4; ++t)
-        for (int r = 0; r < 2; ++r) {
-            // loads: LK-pixel boxes, pixels past the line are zero-filled; output: boxes of one tile of the direction, so a
-            // store never reaches into the next tile of a line (pixels past the line are not written)
-            const int box = t < 3 ? LK : (r == 0 ? p.sp.col.tl : p.sp.row.tl);
-            const int nb = PL && t == 3 ? p.sp.nparts * d.B : d.B;
-            if (!get_map(&m[2 * t + r], base[t], nb, d.H, d.W, ch[t], box, r == 0, kDtype<E>)) {
-                if (why) *why = "cuTensorMapEncodeTiled failed";
-                return cudaErrorInvalidValue;
-            }
-        }
-    p.sp.nparts += extra_parts;          // (after the maps: the planes-mode output holds the 2D problem's planes only)
+    // loads: LK-pixel boxes, pixels past the line are zero-filled; output: boxes of one tile of the direction, so a store
+    // never reaches into the next tile of a line (pixels past the line are not written)
+    const MapSpec out{a.out, PL ? p.sp.nparts * d.B : d.B, d.C, p.sp.col.tl, p.sp.row.tl};
+    if (cudaError_t e = get_maps(m, {{a.q, d.B, d.Cq, LK, LK}, {a.k, d.B, d.Cq, LK, LK}, {a.v, d.B, d.C, LK, LK}, out}, d, kDtype<E>,
+                                 a.why))
+        return e;
+    p.sp.nparts += a.extra_parts;        // (after the maps: the planes-mode output holds the 2D problem's planes only)
     p.C = d.C; p.Cq = d.Cq;
     p.npix = (long)d.B * d.H * d.W;
-    p.parts = parts; p.lse = lse; p.cdone = cdone;
+    p.parts = a.parts; p.lse = a.lse; p.cdone = a.cdone;
     p.hints = tc_l2_hints();
-    const int sms = sm_count();
-    const int grid = p.sp.total < sms ? p.sp.total : sms;
+    const int grid = item_grid(p.sp);
     // Item order (default; DESIGN.md 4).  Sample after sample, the first consumers of each sample wait for its last producers,
     // up to about one item per CTA and sample; in the lagged order two samples' v and out are in play in the L2 instead of one.
     // The wait weighs less the more items a sample has per CTA.  Measured on an H100 (132 SMs): sample after sample is faster
@@ -379,32 +379,16 @@ cudaError_t launch_fwd(const void *q, const void *k, const void *v, void *out, f
     // of 73 and 81) or 2 samples.
     const int lag = tc_lag();
     p.lag = lag >= 0 ? lag : (d.B >= 4 && 3 * p.sp.per_sample >= 4 * grid ? 0 : 1);
-    auto kern = cca_tc_fwd_kernel<LK, E, PL>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem<LK, E>::kBytes);
-    if (e != cudaSuccess) return e;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = FwdSmem<LK, E>::kBytes; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = tc_pdl() ? 1 : 0;     // may start ahead of the statistics kernel's completion (griddepcontrol.wait inside)
-    e = cudaLaunchKernelEx(&cfg, kern, m[0], m[1], m[2], m[3], m[4], m[5], m[6], m[7], p);
-    count_launch();
-    return e != cudaSuccess ? e : cudaGetLastError();
+    // may start ahead of the statistics kernel's completion (griddepcontrol.wait inside)
+    return launch_kernel(cca_tc_fwd_kernel<LK, E, PL>, grid, kThreads, FwdSmem<LK, E>::kBytes, true, a.st, m[0], m[1], m[2], m[3], m[4],
+                         m[5], m[6], m[7], p);
 }
 
-
-// The f16 instantiations live in their own translation unit (cca_tc_f16.cu).
-extern template cudaError_t launch_fwd<80, __half>(const void *, const void *, const void *, void *, float *, const float *,
-                                                   unsigned int *, Dims, cudaStream_t, const char **, int);
-extern template cudaError_t launch_fwd<112, __half>(const void *, const void *, const void *, void *, float *, const float *,
-                                                    unsigned int *, Dims, cudaStream_t, const char **, int);
-// The planes-mode instantiations (fp32) live in cca_tc_det.cu.
-extern template cudaError_t launch_fwd<80, float, true>(const void *, const void *, const void *, void *, float *, const float *,
-                                                        unsigned int *, Dims, cudaStream_t, const char **, int);
-extern template cudaError_t launch_fwd<112, float, true>(const void *, const void *, const void *, void *, float *, const float *,
-                                                         unsigned int *, Dims, cudaStream_t, const char **, int);
+// The f16 instantiations live in their own translation unit (cca_tc_f16.cu), the planes-mode ones (fp32) in cca_tc_det.cu.
+extern template cudaError_t launch_fwd<80, __half>(const FwdArgs &);
+extern template cudaError_t launch_fwd<112, __half>(const FwdArgs &);
+extern template cudaError_t launch_fwd<80, float, true>(const FwdArgs &);
+extern template cudaError_t launch_fwd<112, float, true>(const FwdArgs &);
 
 }  // namespace tc
 }  // namespace cca

@@ -51,6 +51,18 @@ bool get_map(CUtensorMap *m, const void *base, int B, int H, int W, int C, int L
     return true;
 }
 
+cudaError_t get_maps(CUtensorMap *m, std::initializer_list<MapSpec> tensors, Dims d, int dtype, const char **why)
+{
+    for (const MapSpec &t : tensors) {
+        if (!get_map(m++, t.base, t.B, d.H, d.W, t.C, t.box_col, true, dtype) ||
+            !get_map(m++, t.base, t.B, d.H, d.W, t.C, t.box_row, false, dtype)) {
+            if (why) *why = "cuTensorMapEncodeTiled failed";
+            return cudaErrorInvalidValue;
+        }
+    }
+    return cudaSuccess;
+}
+
 int sm_count()
 {
     int dev = 0;

@@ -157,41 +157,37 @@ cca_tc_stats_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_consta
     }
 }
 
-template <int LK, typename E>
-cudaError_t launch_stats(const void *q, const void *k, float *parts, void *zero_ptr, long zero_bytes, unsigned int *counters,
-                         int n_counters, Dims d, cudaStream_t st, const char **why)
+// parts: [nparts][B*H*W] fp32; n_counters words at counters are cleared (0: none)
+struct StatsArgs {
+    const void *q, *k;
+    float *parts;
+    unsigned int *counters;
+    int n_counters;
+    Dims d;
+    cudaStream_t st;
+    const char **why;
+};
+
+template <int LK, typename E> cudaError_t launch_stats(const StatsArgs &a)
 {
     CUtensorMap m[4];
-    const void *base[2] = {q, k};
-    for (int t = 0; t < 2; ++t)
-        for (int r = 0; r < 2; ++r)
-            if (!get_map(&m[2 * t + r], base[t], d.B, d.H, d.W, d.Cq, LK, r == 0, kDtype<E>)) {
-                if (why) *why = "cuTensorMapEncodeTiled failed";
-                return cudaErrorInvalidValue;
-            }
+    const Dims &d = a.d;
+    if (cudaError_t e = get_maps(m, {{a.q, d.B, d.Cq, LK, LK}, {a.k, d.B, d.Cq, LK, LK}}, d, kDtype<E>, a.why)) return e;
     StatsParams p;
     p.sp = make_space(d.B, d.H, d.W);
     p.Cq = d.Cq;
     p.npix = (long)d.B * d.H * d.W;
-    p.parts = parts;
-    p.zero_ptr = reinterpret_cast<uint8_t *>(zero_ptr); p.zero_bytes = zero_bytes;
-    p.counters = counters; p.n_counters = n_counters;
-    auto kern = cca_tc_stats_kernel<LK, E>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, StatsSmem<LK, E>::kBytes);
-    if (e != cudaSuccess) return e;
-    const int sms = sm_count();
-    const int grid = p.sp.total < sms ? p.sp.total : sms;
-    kern<<<grid, kThreads, StatsSmem<LK, E>::kBytes, st>>>(m[0], m[1], m[2], m[3], p);
-    count_launch();
-    return cudaGetLastError();
+    p.parts = a.parts;
+    p.zero_ptr = nullptr; p.zero_bytes = 0;
+    p.counters = a.counters; p.n_counters = a.n_counters;
+    // the first launch of an op: nothing to overlap with
+    return launch_kernel(cca_tc_stats_kernel<LK, E>, item_grid(p.sp), kThreads, StatsSmem<LK, E>::kBytes, false, a.st, m[0], m[1],
+                         m[2], m[3], p);
 }
 
-
 // The f16 instantiations live in their own translation unit (cca_tc_f16.cu).
-extern template cudaError_t launch_stats<80, __half>(const void *, const void *, float *, void *, long, unsigned int *, int, Dims,
-                                                   cudaStream_t, const char **);
-extern template cudaError_t launch_stats<112, __half>(const void *, const void *, float *, void *, long, unsigned int *, int, Dims,
-                                                    cudaStream_t, const char **);
+extern template cudaError_t launch_stats<80, __half>(const StatsArgs &);
+extern template cudaError_t launch_stats<112, __half>(const StatsArgs &);
 
 }  // namespace tc
 }  // namespace cca

@@ -235,39 +235,23 @@ __global__ void __launch_bounds__(32 * kWarps) cca_time_bwd_kernel(const __grid_
         }
 }
 
-template <int TM, typename E> cudaError_t launch_time_tm(int kind, const TimeParams &p, cudaStream_t st)
-{
-    void (*kern)(TimeParams) = kind == kStats    ? cca_time_stats_kernel<TM, E>
-                               : kind == kValues ? cca_time_values_kernel<TM, E>
-                                                 : cca_time_bwd_kernel<TM, E>;
-    const size_t smem = (size_t)kWarps * warp_floats(kind, p.T, p.Cq) * sizeof(float);
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)((p.lines + kWarps - 1) / kWarps)); cfg.blockDim = dim3(32 * kWarps);
-    cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = tc_pdl() ? 1 : 0;
-    e = cudaLaunchKernelEx(&cfg, kern, p);
-    count_launch();
-    return e != cudaSuccess ? e : cudaGetLastError();
-}
-
-template <typename E> cudaError_t launch_time_e(int kind, const TimeParams &p, cudaStream_t st)
-{
-    if (p.T <= 8) return launch_time_tm<8, E>(kind, p, st);
-    if (p.T <= 16) return launch_time_tm<16, E>(kind, p, st);
-    return launch_time_tm<kTimeMaxT, E>(kind, p, st);
-}
-
 cudaError_t launch_time(int kind, const TimeParams &p, int dtype, cudaStream_t st)
 {
-    if (dtype == CCA_F16) return launch_time_e<__half>(kind, p, st);
-    if (dtype == CCA_BF16) return launch_time_e<__nv_bfloat16>(kind, p, st);
-    return launch_time_e<float>(kind, p, st);
+    const unsigned grid = (unsigned)((p.lines + kWarps - 1) / kWarps);
+    const size_t smem = (size_t)kWarps * warp_floats(kind, p.T, p.Cq) * sizeof(float);
+    return with_elem(dtype, [&](auto e) {
+        using E = decltype(e);
+        auto tier = [&](auto tm) {                    // TM: the frames the register arrays hold
+            constexpr int TM = decltype(tm)::value;
+            void (*kern)(TimeParams) = kind == kStats    ? cca_time_stats_kernel<TM, E>
+                                       : kind == kValues ? cca_time_values_kernel<TM, E>
+                                                         : cca_time_bwd_kernel<TM, E>;
+            return launch_kernel(kern, grid, 32 * kWarps, smem, true, st, p);
+        };
+        if (p.T <= 8) return tier(std::integral_constant<int, 8>{});
+        if (p.T <= 16) return tier(std::integral_constant<int, 16>{});
+        return tier(std::integral_constant<int, kTimeMaxT>{});
+    });
 }
 
 TimeParams time_params(Dims3 d)
@@ -277,14 +261,6 @@ TimeParams time_params(Dims3 d)
     p.hw = (long)d.H * d.W;
     p.T = d.T; p.Cq = d.Cq; p.C = d.C;
     return p;
-}
-
-// partial lse planes of the 3D forward: the frames view's 2D planes, then the time plane
-size_t parts3d_bytes(Dims3 d)
-{
-    const Dims f = d.frames();
-    const size_t npix = (size_t)f.B * f.H * f.W;
-    return ((size_t)(make_space(f.B, f.H, f.W).nparts + 1) * npix * sizeof(float) + 15) & ~(size_t)15;
 }
 
 }  // namespace
@@ -297,12 +273,9 @@ bool tc3d_supported(Dims3 d, int dtype)
     return d.T >= 1 && d.T <= kTimeMaxT && (long)d.B * d.T < (1L << 31) && shape_supported(d.frames(), dtype);
 }
 
-// Workspace of the 3D forward: [nparts + 1][B*T*H*W] fp32 partial lse planes, then [B*T] per-frame counters of the values
-// kernel (planes mode: tc_planes_bytes of the frames view follow).
-size_t tc_forward3d_workspace(Dims3 d)
-{
-    return parts3d_bytes(d) + (((size_t)d.B * d.T * sizeof(unsigned int) + 15) & ~(size_t)15);
-}
+// Workspace of the 3D forward: that of the 2D forward on the frames view with one more partial lse plane, the time plane
+// (planes mode: tc_planes_bytes of the frames view follow).
+size_t tc_forward3d_workspace(Dims3 d) { return fwd_ws(d.frames(), 1, nullptr).bytes; }
 
 // Workspace of the 3D backward: that of the 2D backward on the frames view (delta first)
 size_t tc_backward3d_workspace(Dims3 d) { return tc_backward_workspace(d.frames()); }
@@ -311,17 +284,14 @@ cudaError_t tc_forward3d(const void *q, const void *k, const void *v, void *out,
                          cudaStream_t st, const char **why, bool det)
 {
     const Dims f = d.frames();
-    const long npix = (long)f.B * f.H * f.W;
-    float *parts = reinterpret_cast<float *>(ws);
-    unsigned int *cdone = reinterpret_cast<unsigned int *>(reinterpret_cast<uint8_t *>(ws) + parts3d_bytes(d));
-    cudaError_t e = tc_stats(q, k, parts, nullptr, 0, cdone, f.B, f, dtype, st, why);
+    const FwdWs w = fwd_ws(f, 1, ws);
+    cudaError_t e = tc_stats(q, k, w.parts, w.cdone, f.B, f, dtype, st, why);
     if (e != cudaSuccess) return e;
     TimeParams p = time_params(d);
     p.q = q; p.k = k; p.v = v; p.out = out; p.lse = lse;
-    p.part = parts + (long)make_space(f.B, f.H, f.W).nparts * npix;
+    p.part = w.parts + (long)make_space(f.B, f.H, f.W).nparts * f.B * f.H * f.W;
     if ((e = launch_time(kStats, p, dtype, st)) != cudaSuccess) return e;
-    e = tc_values(q, k, v, out, lse, parts, cdone, reinterpret_cast<uint8_t *>(ws) + tc_forward3d_workspace(d), f, dtype, st, why,
-                  det, 1);
+    e = tc_values(q, k, v, out, lse, w.parts, w.cdone, w.planes, f, dtype, st, why, det, 1);
     if (e != cudaSuccess) return e;
     return launch_time(kValues, p, dtype, st);
 }
@@ -334,7 +304,7 @@ cudaError_t tc_backward3d(const void *dout, const void *q, const void *k, const 
     TimeParams p = time_params(d);
     p.q = q; p.k = k; p.v = v; p.dout = dout; p.lse = lse;
     p.dq = dq; p.dk = dk; p.dv = dv;
-    p.delta = reinterpret_cast<const float *>(ws);      // (tc_backward leaves delta at the start of its workspace)
+    p.delta = bwd_ws(d.frames(), ws).delta;             // (left there by tc_backward)
     return launch_time(kBackward, p, dtype, st);
 }
 

@@ -1,6 +1,7 @@
 """CPU tests: the C-ABI library loads and exports every symbol of include/cca_b200.h, the
 nn.Module mirrors the reference surface, and nothing silently falls back to CPU."""
 import ctypes
+import json
 import os
 import re
 
@@ -35,6 +36,19 @@ def test_version_and_workspace_and_strerror_without_gpu():
     assert lib.cca_b200_tc_supported(capi.CCA_WS_FORWARD, 1, 8, 64, 32, 32, capi.CCA_F32) == 0      # Cq < 16
     assert lib.cca_b200_strerror(0) == b"ok"
     assert b"unsupported" in lib.cca_b200_strerror(-2)
+
+
+def _workspace_cases():
+    with open(os.path.join(ROOT, "tests", "golden", "workspace_bytes.json")) as f:
+        return sorted(json.load(f).items())
+
+
+@pytest.mark.parametrize("query,cases", _workspace_cases(), ids=lambda x: x if isinstance(x, str) else "")
+def test_workspace_bytes_match_the_recorded_sizes(query, cases):
+    # callers allocate by these sizes: every one stays byte-identical (fixture: tests/golden/make_workspace_bytes.py)
+    fn = getattr(capi.load(), query)
+    wrong = [(args, want, fn(*args)) for *args, want in cases if fn(*args) != want]
+    assert not wrong, f"{len(wrong)} of {len(cases)} sizes differ, e.g. {wrong[:5]}"
 
 
 def test_invalid_arguments_are_rejected_before_any_cuda_call():
