@@ -447,6 +447,86 @@ int cca_b200_backward3d(const void *dout, const void *q, const void *k, const vo
 }
 
 // ---------------------------------------------------------------------------------------
+// attention map of the 3D op: tensor-core path (cca_tc_attn3d.cu) or generic kernels (cca_simt_attn3d.cu)
+// ---------------------------------------------------------------------------------------
+namespace {
+int check_attention_dims3d(int B, int Cq, int T, int H, int W, int dtype)
+{
+    int rc = check_dims3d(B, Cq, 1, T, H, W, dtype);
+    if (rc) return rc;
+    const long long npix = (long long)B * T * H * W;
+    if (npix * Cq >= (1ll << 40) || npix * ((long long)H + W + T) >= (1ll << 40)) return fail(CCA_ERR_UNSUPPORTED, "tensor too large%s%s");
+    return CCA_OK;
+}
+}  // namespace
+
+int cca_b200_attention_tc3d_supported(int B, int Cq, int T, int H, int W, int dtype)
+{
+    if (B <= 0 || T <= 0 || check_attention_dims3d(B, Cq, T, H, W, dtype) || other_device()) return 0;
+    return tc3d_attention_supported(Dims3{B, Cq, 0, T, H, W}, dtype) ? 1 : 0;
+}
+
+size_t cca_b200_attention_workspace_bytes3d(int backward, int B, int Cq, int T, int H, int W, int dtype, unsigned flags)
+{
+    if (B <= 0 || Cq <= 0 || T <= 0 || H <= 0 || W <= 0 || (long long)B * T >= (1ll << 31)) return 0;
+    const Dims3 d{B, Cq, 0, T, H, W};
+    const size_t simt = simt_attention3d_workspace(backward, d);
+    const size_t tcb = tc_attention3d_workspace(backward, d, attention_det_planes(d.frames(), dtype, flags));
+    return simt > tcb ? simt : tcb;
+}
+
+int cca_b200_attention_forward3d(const void *q, const void *k, float *attn, void *ws, size_t ws_bytes, int B, int Cq, int T, int H,
+                                 int W, int dtype, unsigned flags, void *stream)
+{
+    int rc = check_attention_dims3d(B, Cq, T, H, W, dtype);
+    if (rc) return rc;
+    if (!q || !k || !attn || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
+    if (reinterpret_cast<uintptr_t>(attn) & 3) return fail(CCA_ERR_INVALID, "attn must be 4-byte aligned%s%s");
+    if (ws_bytes < cca_b200_attention_workspace_bytes3d(0, B, Cq, T, H, W, dtype, flags))
+        return fail(CCA_ERR_WORKSPACE, "attention map workspace too small%s%s");
+    const Dims3 d{B, Cq, 0, T, H, W};
+    // (the forward writes every map element once: deterministic in every mode)
+    const int fam = kernel_family(flags, (flags & CCA_FLAG_NHWC) && tc3d_attention_supported(d, dtype), false, "3D attention map",
+                                  "NCDHW");
+    if (fam < 0) return fam;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (fam == 1) {
+        if (!aligned16({q, k, ws})) return fail(CCA_ERR_INVALID, kAlignMsg);
+        const char *why = "";
+        cudaError_t e = tc_attention_forward3d(q, k, attn, ws, d, dtype, st, &why);
+        return e != cudaSuccess ? cuda_fail(e, why && *why ? why : "tc_attention_forward3d") : CCA_OK;
+    }
+    cudaError_t e = simt_attention_forward3d(q, k, attn, d, dtype, st);
+    return e != cudaSuccess ? cuda_fail(e, "simt_attention_forward3d") : CCA_OK;
+}
+
+int cca_b200_attention_backward3d(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk, void *ws,
+                                  size_t ws_bytes, int B, int Cq, int T, int H, int W, int dtype, unsigned flags, void *stream)
+{
+    int rc = check_attention_dims3d(B, Cq, T, H, W, dtype);
+    if (rc) return rc;
+    if (!dattn || !attn || !q || !k || !dq || !dk || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
+    if ((reinterpret_cast<uintptr_t>(attn) | reinterpret_cast<uintptr_t>(dattn)) & 3)
+        return fail(CCA_ERR_INVALID, "attn and dattn must be 4-byte aligned%s%s");
+    if (ws_bytes < cca_b200_attention_workspace_bytes3d(1, B, Cq, T, H, W, dtype, flags))
+        return fail(CCA_ERR_WORKSPACE, "attention map backward workspace too small%s%s");
+    const Dims3 d{B, Cq, 0, T, H, W};
+    const int fam = kernel_family(flags, (flags & CCA_FLAG_NHWC) && tc3d_attention_supported(d, dtype),
+                                  det_16bit_tiled(flags, d.frames(), dtype), "3D attention map", "NCDHW");
+    if (fam < 0) return fam;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (fam == 1) {
+        if (!aligned16({q, k, dq, dk, ws})) return fail(CCA_ERR_INVALID, kAlignMsg);
+        const char *why = "";
+        cudaError_t e = tc_attention_backward3d(dattn, attn, q, k, dq, dk, ws, d, dtype, st, &why, (flags & CCA_FLAG_DETERMINISTIC) != 0);
+        return e != cudaSuccess ? cuda_fail(e, why && *why ? why : "tc_attention_backward3d") : CCA_OK;
+    }
+    if (reinterpret_cast<uintptr_t>(ws) & 3) return fail(CCA_ERR_INVALID, "workspace must be 4-byte aligned%s%s");
+    cudaError_t e = simt_attention_backward3d(dattn, attn, q, k, dq, dk, ws, d, dtype, st);
+    return e != cudaSuccess ? cuda_fail(e, "simt_attention_backward3d") : CCA_OK;
+}
+
+// ---------------------------------------------------------------------------------------
 // 1x1 Q/K/V projections (functions.py:29,32,35) as tensor-core GEMMs on the channels-last view
 // ---------------------------------------------------------------------------------------
 namespace {

@@ -132,7 +132,7 @@ size_t simt_attention_workspace(int backward, Dims d);
 cudaError_t simt_attention_forward(const void *q, const void *k, float *attn, Dims d, int dtype, cudaStream_t st);
 cudaError_t simt_attention_backward(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk,
                                     void *ws, Dims d, int dtype, cudaStream_t st);
-//   rho[p] = sum_j attn[p,j] dattn[p,j] over the hw2 = H+W entries of each of the npix pixels (one warp per pixel, fixed
+//   rho[p] = sum_j attn[p,j] dattn[p,j] over the hw2 entries (H+W; H+W+T for the 3D map) of each of the npix pixels (one warp per pixel, fixed
 //   order); also clears clear_bytes at each of c0 and c1 (may be 0)
 cudaError_t attn_rho(const float *dattn, const float *attn, float *rho, long npix, int hw2, void *c0, void *c1, long clear_bytes,
                      cudaStream_t st);
@@ -143,6 +143,20 @@ cudaError_t tc_attention_forward(const void *q, const void *k, float *attn, void
                                  const char **why);
 cudaError_t tc_attention_backward(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk, void *ws,
                                   Dims d, int dtype, cudaStream_t st, const char **why, bool det);
+
+// the attention map of the 3D op, attn[B,T,H,W,H+W+T] (fp32: column, row, time keys) and its gradient w.r.t. q, k
+//   generic kernels, NCDHW q, k of any Cq and shape (cca_simt_attn3d.cu); the backward's workspace is rho [B*T*H*W]
+size_t simt_attention3d_workspace(int backward, Dims3 d);
+cudaError_t simt_attention_forward3d(const void *q, const void *k, float *attn, Dims3 d, int dtype, cudaStream_t st);
+cudaError_t simt_attention_backward3d(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk,
+                                      void *ws, Dims3 d, int dtype, cudaStream_t st);
+//   tensor-core path, NDHWC q, k (cca_tc_attn3d.cu): the 2D map kernels on the frames view + time kernels; T <= kTimeMaxT
+bool tc3d_attention_supported(Dims3 d, int dtype);
+size_t tc_attention3d_workspace(int backward, Dims3 d, bool det);
+cudaError_t tc_attention_forward3d(const void *q, const void *k, float *attn, void *ws, Dims3 d, int dtype, cudaStream_t st,
+                                   const char **why);
+cudaError_t tc_attention_backward3d(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk, void *ws,
+                                    Dims3 d, int dtype, cudaStream_t st, const char **why, bool det);
 
 // wgmma GEMMs of the 1x1 Q/K/V projections (cca_gemm.cu), fp32 channels-last tensors as [pixels, channels] matrices
 bool qkv_gemm_supported(int C, int Cq);

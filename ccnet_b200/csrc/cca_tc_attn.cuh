@@ -69,10 +69,14 @@ __device__ __forceinline__ float2 load_pair(const float *row, int c, int lk, boo
     return make_float2(__ldg(row + c), c + 1 < lk ? __ldg(row + c + 1) : 0.f);
 }
 
-template <int LK, typename E>
-__global__ void __launch_bounds__(kThreads, 1)
-cca_tc_attn_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant__ CUtensorMap mqr,
-                       const __grid_constant__ CUtensorMap mkc, const __grid_constant__ CUtensorMap mkr, AttnFwdParams p)
+// Row length of the map: H + W entries in 2D.  The 3D map (cca_tc_attn3d.cu) runs these kernels on the frames view of a
+// clip batch with rows of H + W + T entries, its params type carrying T; the item arithmetic is the same.
+__device__ __forceinline__ long map_row(const AttnFwdParams &p) { return (long)p.sp.H + p.sp.W; }
+
+// (the kernels' bodies, shared by the 2D and 3D map kernels)
+template <int LK, typename E, typename P>
+__device__ __forceinline__ void attn_fwd(const CUtensorMap &mqc, const CUtensorMap &mqr, const CUtensorMap &mkc,
+                                         const CUtensorMap &mkr, const P &p)
 {
     using T = Tiles<LK, E>;
     using S = StatsSmem<LK, E>;          // the same Q + K ring as the statistics pre-pass
@@ -113,7 +117,7 @@ cca_tc_attn_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_con
     } else if (tid >= 128) {
         const int t = tid - 128, wg = t >> 7, wq = (t >> 5) & 3;
         const int rbase = 64 * wg + 16 * wq + (lane >> 2), cq = 2 * (lane & 3);
-        const long hw2 = (long)p.sp.H + p.sp.W;
+        const long hw2 = map_row(p);
         const uint32_t ld_base = smem_u32(smem + S::off_ld);
         pdl_wait();                      // the partial planes come from the statistics kernel
         for (int k = 0; k < nk; ++k) {
@@ -176,6 +180,14 @@ cca_tc_attn_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_con
     }
 }
 
+template <int LK, typename E>
+__global__ void __launch_bounds__(kThreads, 1)
+cca_tc_attn_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant__ CUtensorMap mqr,
+                       const __grid_constant__ CUtensorMap mkc, const __grid_constant__ CUtensorMap mkr, AttnFwdParams p)
+{
+    attn_fwd<LK, E>(mqc, mqr, mkc, mkr, p);
+}
+
 struct AttnBwdParams {
     ItemSpace sp;
     int Cq;
@@ -201,12 +213,12 @@ template <int LK, typename E> struct AttnBwdSmem {
     static_assert(kBytes <= kBudget, "shared memory budget");
 };
 
-template <int LK, typename E, bool PL>
-__global__ void __launch_bounds__(kThreads, 1)
-cca_tc_attn_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant__ CUtensorMap mqr,
-                       const __grid_constant__ CUtensorMap mkc, const __grid_constant__ CUtensorMap mkr,
-                       const __grid_constant__ CUtensorMap mdqc, const __grid_constant__ CUtensorMap mdqr,
-                       const __grid_constant__ CUtensorMap mdkc, const __grid_constant__ CUtensorMap mdkr, AttnBwdParams p)
+__device__ __forceinline__ long map_row(const AttnBwdParams &p) { return (long)p.sp.H + p.sp.W; }
+
+template <int LK, typename E, bool PL, typename P>
+__device__ __forceinline__ void attn_bwd(const CUtensorMap &mqc, const CUtensorMap &mqr, const CUtensorMap &mkc,
+                                         const CUtensorMap &mkr, const CUtensorMap &mdqc, const CUtensorMap &mdqr,
+                                         const CUtensorMap &mdkc, const CUtensorMap &mdkr, const P &p)
 {
     using T = Tiles<LK, E>;
     using S = AttnBwdSmem<LK, E>;
@@ -250,7 +262,7 @@ cca_tc_attn_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_con
         const int t = tid - 128, wg = t >> 7, wq = (t >> 5) & 3;
         const int rbase = 64 * wg + 16 * wq + (lane >> 2);         // accumulator rows rbase, rbase + 8
         const int cq = 2 * (lane & 3);                             // first accumulator column of this thread (+ 8j)
-        const long hw2 = (long)p.sp.H + p.sp.W;
+        const long hw2 = map_row(p);
         const uint32_t ld_base = smem_u32(smem + S::off_ld), pb = smem_u32(smem + S::off_p);
         uint8_t *pgen = smem + S::off_p;
         // this thread's accumulator rows (nc channels from 0) -> `tile`, laid out as the output's swizzled TMA box(es)
@@ -390,6 +402,124 @@ cca_tc_attn_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_con
         }
         if (t == 0) bulk_wait<0>();                                // shared memory must outlive the last bulk reads
     }
+}
+
+template <int LK, typename E, bool PL>
+__global__ void __launch_bounds__(kThreads, 1)
+cca_tc_attn_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant__ CUtensorMap mqr,
+                       const __grid_constant__ CUtensorMap mkc, const __grid_constant__ CUtensorMap mkr,
+                       const __grid_constant__ CUtensorMap mdqc, const __grid_constant__ CUtensorMap mdqr,
+                       const __grid_constant__ CUtensorMap mdkc, const __grid_constant__ CUtensorMap mdkr, AttnBwdParams p)
+{
+    attn_bwd<LK, E, PL>(mqc, mqr, mkc, mkr, mdqc, mdqr, mdkc, mdkr, p);
+}
+
+// The 3D map (cca_tc_attn3d.cu): the kernels above on the [B*T, H, W, Cq] frames view of NDHWC q, k, writing the column and
+// row entries of map rows of H + W + T entries; the forward's lse combine takes one more plane, the time branch's.
+struct AttnFwdParams3 : AttnFwdParams {
+    int T;
+};
+struct AttnBwdParams3 : AttnBwdParams {
+    int T;
+};
+__device__ __forceinline__ long map_row(const AttnFwdParams3 &p) { return (long)p.sp.H + p.sp.W + p.T; }
+__device__ __forceinline__ long map_row(const AttnBwdParams3 &p) { return (long)p.sp.H + p.sp.W + p.T; }
+
+template <int LK, typename E>
+__global__ void __launch_bounds__(kThreads, 1)
+cca_tc_attn3d_fwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant__ CUtensorMap mqr,
+                         const __grid_constant__ CUtensorMap mkc, const __grid_constant__ CUtensorMap mkr, AttnFwdParams3 p)
+{
+    attn_fwd<LK, E>(mqc, mqr, mkc, mkr, p);
+}
+
+template <int LK, typename E, bool PL>
+__global__ void __launch_bounds__(kThreads, 1)
+cca_tc_attn3d_bwd_kernel(const __grid_constant__ CUtensorMap mqc, const __grid_constant__ CUtensorMap mqr,
+                         const __grid_constant__ CUtensorMap mkc, const __grid_constant__ CUtensorMap mkr,
+                         const __grid_constant__ CUtensorMap mdqc, const __grid_constant__ CUtensorMap mdqr,
+                         const __grid_constant__ CUtensorMap mdkc, const __grid_constant__ CUtensorMap mdkr, AttnBwdParams3 p)
+{
+    attn_bwd<LK, E, PL>(mqc, mqr, mkc, mkr, mdqc, mdqr, mdkc, mdkr, p);
+}
+
+// ---- host launchers.  X3 = false: the 2D map on d (T unused); X3: the 3D map of clips of T frames on the frames view d
+// (d.B = B*T), its lse combining the statistics pass's planes and the time plane after them.
+template <int LK, typename E, bool X3>
+cudaError_t launch_attn_fwd(const void *q, const void *k, float *attn, const float *parts, Dims d, int T, cudaStream_t st,
+                            const char **why)
+{
+    CUtensorMap m[4];
+    if (cudaError_t e = get_maps(m, {{q, d.B, d.Cq, LK, LK}, {k, d.B, d.Cq, LK, LK}}, d, kDtype<E>, why)) return e;
+    AttnFwdParams3 p;
+    p.sp = make_space(d.B, d.H, d.W);
+    p.Cq = d.Cq;
+    p.npix = (long)d.B * d.H * d.W;
+    p.parts = parts;
+    p.attn = attn;
+    p.T = T;
+    const int smem = StatsSmem<LK, E>::kBytes;
+    if constexpr (!X3) {
+        return launch_kernel(cca_tc_attn_fwd_kernel<LK, E>, item_grid(p.sp), kThreads, smem, true, st, m[0], m[1], m[2], m[3],
+                             static_cast<const AttnFwdParams &>(p));
+    } else {
+        p.sp.nparts += 1;                // (the items do not depend on it: only the lse combine reads it)
+        return launch_kernel(cca_tc_attn3d_fwd_kernel<LK, E>, item_grid(p.sp), kThreads, smem, true, st, m[0], m[1], m[2], m[3], p);
+    }
+}
+
+// PL: dq, dk are the [nparts*B, H, W, Cq] fp32 plane buffers
+template <int LK, typename E, bool PL, bool X3>
+cudaError_t launch_attn_bwd(const float *dattn, const float *attn, const float *rho, const void *q, const void *k, void *dq, void *dk,
+                            Dims d, int T, cudaStream_t st, const char **why)
+{
+    CUtensorMap m[8];
+    AttnBwdParams3 p;
+    p.sp = make_space(d.B, d.H, d.W);
+    // output boxes: one tile of the direction (a store never reaches the next tile)
+    const int nb = PL ? p.sp.nparts * d.B : d.B;
+    if (cudaError_t e = get_maps(m, {{q, d.B, d.Cq, LK, LK}, {k, d.B, d.Cq, LK, LK}, {dq, nb, d.Cq, p.sp.col.tl, p.sp.row.tl},
+                                     {dk, nb, d.Cq, p.sp.col.tl, p.sp.row.tl}},
+                                 d, kDtype<E>, why))
+        return e;
+    p.Cq = d.Cq;
+    p.attn = attn; p.dattn = dattn; p.rho = rho;
+    p.T = T;
+    const int smem = AttnBwdSmem<LK, E>::kBytes;
+    if constexpr (!X3)
+        return launch_kernel(cca_tc_attn_bwd_kernel<LK, E, PL>, item_grid(p.sp), kThreads, smem, true, st, m[0], m[1], m[2], m[3],
+                             m[4], m[5], m[6], m[7], static_cast<const AttnBwdParams &>(p));
+    else
+        return launch_kernel(cca_tc_attn3d_bwd_kernel<LK, E, PL>, item_grid(p.sp), kThreads, smem, true, st, m[0], m[1], m[2],
+                             m[3], m[4], m[5], m[6], m[7], p);
+}
+
+// Backward of the 2D map (X3 = false) or of the 3D map's column and row entries on the frames view d: the rho pass over rows
+// of H + W (+ T) entries, which also clears dq and dk for the reduce-adds, then the item kernel; in planes mode (det on
+// tiled lines; fp32, cca_capi.cu refuses 16-bit I/O there) the items store into the dQ, dK planes and planes_sum adds them.
+template <bool X3>
+cudaError_t map_backward(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk, void *ws, Dims d,
+                         int T, int dtype, cudaStream_t st, const char **why, bool det)
+{
+    const long npix = (long)d.B * d.H * d.W;
+    const bool planes = det && tc_tiled(d);
+    const AttnBwdWs w = attn_bwd_ws(d, planes, ws);
+    const long clear = planes ? 0 : npix * d.Cq * (dtype == CCA_F32 ? 4 : 2);
+    cudaError_t e = attn_rho(dattn, attn, w.rho, npix, d.H + d.W + (X3 ? T : 0), planes ? nullptr : dq, planes ? nullptr : dk,
+                             clear, st);
+    if (e != cudaSuccess) return e;
+    if (planes) {
+        float *pq = w.planes.p[0], *pk = w.planes.p[1];
+        e = with_tile(d, [&](auto lk) { return launch_attn_bwd<lk(), float, true, X3>(dattn, attn, w.rho, q, k, pq, pk, d, T, st, why); });
+        if (e != cudaSuccess) return e;
+        const float *src[2] = {pq, pk};
+        float *dst[2] = {reinterpret_cast<float *>(dq), reinterpret_cast<float *>(dk)};
+        const long n[2] = {npix * d.Cq, npix * d.Cq};
+        return planes_sum(src, dst, n, 2, make_space(d.B, d.H, d.W).nparts, st);
+    }
+    return with_elem_tile(dtype, d, [&](auto el, auto lk) {
+        return launch_attn_bwd<lk(), decltype(el), false, X3>(dattn, attn, w.rho, q, k, dq, dk, d, T, st, why);
+    });
 }
 
 }  // namespace tc

@@ -18,70 +18,19 @@
 // elements per pixel for 2T(Cq + C) FLOPs, bandwidth-bound on CUDA cores, so it uses no tensor cores.  The shared memory
 // per warp grows with T * Cq; kTimeMaxT = 32 keeps the backward's four warps under 140 KB.
 #include "cca_items.cuh"
-#include "cca_tc_common.cuh"
+#include "cca_tc_time.cuh"
 
 namespace cca {
 namespace tc {
 namespace {
 
-constexpr int kWarps = 4;   // T-lines per CTA
 enum TimeKind { kStats = 0, kValues = 1, kBackward = 2 };
-
-struct TimeParams {
-    const void *q, *k, *v, *dout;
-    void *out, *dq, *dk, *dv;
-    float *part;              // stats: the time plane [B*T*H*W] (log2-sum-exp2 of the T-line logits, self excluded)
-    const float *lse;         // final natural-log lse [B*T*H*W]
-    const float *delta;       // backward: <dout, out> per pixel (the 2D backward's workspace)
-    long lines;               // B*H*W
-    long hw;                  // H*W
-    int T, Cq, C;
-};
 
 // floats of shared memory per warp: Q, K [T][Cq+1]; values: + P [T][T+1]; backward: + P, dS [T][T+1], dO, V chunks [T][33]
 __host__ __device__ inline long warp_floats(int kind, int T, int Cq)
 {
     const long qk = 2L * T * (Cq + 1), pp = (long)T * (T + 1), ch = 32L + 1;
     return kind == kStats ? qk : kind == kValues ? qk + pp : qk + 2 * pp + 2 * T * ch;
-}
-
-// pixel of frame 0 of a T-line (b, hw); frame t is t * hw pixels further
-__device__ __forceinline__ long line_pix0(long line, const TimeParams &p)
-{
-    const long b = line / p.hw;
-    return b * p.T * p.hw + (line - b * p.hw);
-}
-
-template <typename E>
-__device__ __forceinline__ void stage_qk(const TimeParams &p, long pix0, float *qs, float *ks, int lane)
-{
-    const E *q = static_cast<const E *>(p.q), *k = static_cast<const E *>(p.k);
-    const int ld = p.Cq + 1;
-    for (int t = 0; t < p.T; ++t) {
-        const long base = (pix0 + t * p.hw) * p.Cq;
-        for (int c = lane; c < p.Cq; c += 32) {
-            qs[t * ld + c] = to_f(q[base + c]);
-            ks[t * ld + c] = to_f(k[base + c]);
-        }
-    }
-    __syncwarp();
-}
-
-// s[j] = log2e * (q_t . k_j), j < T, of query frame t
-template <int TM>
-__device__ __forceinline__ void row_logits(const TimeParams &p, const float *qs, const float *ks, int t, float (&s)[TM])
-{
-    const int ld = p.Cq + 1;
-#pragma unroll
-    for (int j = 0; j < TM; ++j) s[j] = 0.f;
-    for (int c = 0; c < p.Cq; ++c) {
-        const float a = qs[t * ld + c];
-#pragma unroll
-        for (int j = 0; j < TM; ++j)
-            if (j < p.T) s[j] = fmaf(a, ks[j * ld + c], s[j]);
-    }
-#pragma unroll
-    for (int j = 0; j < TM; ++j) s[j] *= kLog2e;
 }
 
 // lane t < T: P[t][j] = exp2(s_j - lse2_t), 0 at j == t, into pr and row t of ps
@@ -98,8 +47,6 @@ __device__ __forceinline__ void row_probs(const TimeParams &p, const float *qs, 
         if (j < p.T) ps[t * (p.T + 1) + j] = pr[j];
     }
 }
-
-template <typename E> __device__ __forceinline__ void add_to(E *dst, float x) { *dst = from_f<E>(to_f(*dst) + x); }
 
 template <int TM, typename E>
 __global__ void __launch_bounds__(32 * kWarps) cca_time_stats_kernel(const __grid_constant__ TimeParams p)
@@ -241,29 +188,26 @@ cudaError_t launch_time(int kind, const TimeParams &p, int dtype, cudaStream_t s
     const size_t smem = (size_t)kWarps * warp_floats(kind, p.T, p.Cq) * sizeof(float);
     return with_elem(dtype, [&](auto e) {
         using E = decltype(e);
-        auto tier = [&](auto tm) {                    // TM: the frames the register arrays hold
+        auto tier = [&](auto tm) {
             constexpr int TM = decltype(tm)::value;
             void (*kern)(TimeParams) = kind == kStats    ? cca_time_stats_kernel<TM, E>
                                        : kind == kValues ? cca_time_values_kernel<TM, E>
                                                          : cca_time_bwd_kernel<TM, E>;
             return launch_kernel(kern, grid, 32 * kWarps, smem, true, st, p);
         };
-        if (p.T <= 8) return tier(std::integral_constant<int, 8>{});
-        if (p.T <= 16) return tier(std::integral_constant<int, 16>{});
-        return tier(std::integral_constant<int, kTimeMaxT>{});
+        return with_time_tier(p.T, tier);
     });
 }
 
-TimeParams time_params(Dims3 d)
+}  // namespace
+
+cudaError_t tc_time_stats(const void *q, const void *k, float *part, Dims3 d, int dtype, cudaStream_t st)
 {
-    TimeParams p = {};
-    p.lines = (long)d.B * d.H * d.W;
-    p.hw = (long)d.H * d.W;
-    p.T = d.T; p.Cq = d.Cq; p.C = d.C;
-    return p;
+    TimeParams p = time_params(d);
+    p.q = q; p.k = k; p.part = part;
+    return launch_time(kStats, p, dtype, st);
 }
 
-}  // namespace
 }  // namespace tc
 
 using namespace tc;

@@ -88,10 +88,11 @@ def _upcast(dtype, H: int, W: int, deterministic: bool, T: int = 1) -> bool:
     the bf16x3 split), the result rounded to the 16-bit type ONCE:
     - lines longer than one 112-pixel tile: every output element of the native kernels is the sum of up to 2*ceil(L/112) TMA
       reduce-adds, each rounded to the 16-bit type in memory, in no fixed order -- at the 1e-2 budget for bf16.
-    - bf16 with T > 1 (the 3D op): the time pass adds onto out, dq, dk and dv after the 2D passes have rounded them to the
-      I/O type, a third rounding of every output element; in bf16 that puts the emulated floor at up to 0.73 of the 1e-2
-      budget (tests/test_cca3d_host.py), in fp16 at a third of its budget.  At T = 1 the time pass adds nothing and the
-      native kernels give the 2D op's bits.
+    - bf16 with T > 1 (the 3D op and its attention map's backward): the time pass adds onto out, dq, dk and dv after the
+      2D passes have rounded them to the I/O type, a third rounding of every output element; in bf16 that puts the
+      emulated floor at up to 0.73 of the 1e-2 budget (tests/test_cca3d_host.py), in fp16 at a third of its budget (the
+      map's dq, dk: tests/test_attention3d_host.py).  At T = 1 the time pass adds nothing and the native kernels give the
+      2D op's bits.
     CCA_B200_BF16_NATIVE=1 keeps the native bf16 and fp16 kernels (the C ABI always does), except in deterministic mode on
     long lines: only the fp32 kernels have it there."""
     if dtype not in (torch.bfloat16, torch.float16):
@@ -474,3 +475,83 @@ class _CCA3DFunction(torch.autograd.Function):
 def cca3d(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", deterministic=None) -> torch.Tensor:
     """Differentiable criss-cross attention over clips (out only); see ``cca3d_forward``."""
     return _CCA3DFunction.apply(q, k, v, impl, _resolve_deterministic(deterministic))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# attention map of criss-cross attention over clips and its gradient
+# ---------------------------------------------------------------------------------------------------------------------
+def attention3d_tc_eligible(B: int, Cq: int, T: int, H: int, W: int, dtype: torch.dtype) -> bool:
+    """True if the tensor-core (channels_last_3d) kernels of the 3D attention map cover this problem."""
+    return dtype in _DTYPES and capi.load().cca_b200_attention_tc3d_supported(B, Cq, T, H, W, _DTYPES[dtype]) == 1
+
+
+def cca3d_attention_forward(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", deterministic=None) -> torch.Tensor:
+    """The attention map of ``cca3d_forward``, attn[B,T,H,W,H+W+T] float32: attn[b,t,h,w,g] is the weight of column key
+    (t, g, w) for g < H (0 at g == h), of row key (t, h, g - H) for H <= g < H + W and of time key (g - H - W, h, w) after
+    that (0 at g - H - W == t).  It is normalised by the lse of ``cca3d_forward``; at T = 1, attn[..., :H+W] is
+    ``cca_attention_forward`` of every frame and attn[..., H+W] is 0.
+
+    ``impl`` as for ``cca3d_forward`` (the generic kernels take any Cq and shape).  Every map element is written once, so
+    the result is the same in every mode; ``deterministic`` only sets the flag the C ABI is called with."""
+    _check_inputs(q, k, rank=5)
+    det = _resolve_deterministic(deterministic)
+    lib = capi.load()
+    B, Cq, T, H, W = q.shape
+    dt = _DTYPES[q.dtype]
+    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_attention_tc3d_supported(B, Cq, T, H, W, dt) == 1, q)
+    q, k = (t.contiguous(memory_format=fmt) for t in (q, k))
+    with torch.cuda.device(q.device):
+        attn = torch.empty((B, T, H, W, H + W + T), dtype=torch.float32, device=q.device)
+        ws = _workspace(lib.cca_b200_attention_workspace_bytes3d(0, B, Cq, T, H, W, dt, flags), q.device)
+        rc = lib.cca_b200_attention_forward3d(q.data_ptr(), k.data_ptr(), attn.data_ptr(), ws.data_ptr(), ws.numel(),
+                                              B, Cq, T, H, W, dt, flags, _stream_ptr(q.device))
+        capi.check(rc, "cca_b200_attention_forward3d")
+    return attn
+
+
+def cca3d_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministic=None):
+    """Gradients (dq, dk) of ``cca3d_attention_forward`` given dattn = dL/dattn and the forward's map, in the closed form
+    of ``cca_attention_backward`` over the H + W + T entries of a row.  Same ``impl`` / memory-format / ``deterministic``
+    rules as ``cca3d_backward``."""
+    _check_inputs(q, k, rank=5)
+    det = _resolve_deterministic(deterministic)
+    lib = capi.load()
+    B, Cq, T, H, W = q.shape
+    for name, t in (("attn", attn), ("dattn", dattn)):
+        if t.dtype != torch.float32 or tuple(t.shape) != (B, T, H, W, H + W + T) or t.device != q.device:
+            raise RuntimeError(f"ccnet_b200: {name} must be a float32 [B,T,H,W,H+W+T] tensor on the device of q, k")
+    dt = _DTYPES[q.dtype]
+    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_attention_tc3d_supported(B, Cq, T, H, W, dt) == 1, q)
+    if use_tc and _upcast(q.dtype, H, W, det, T):
+        dq, dk = cca3d_attention_backward(dattn, attn, q.float(), k.float(), impl, det)
+        return dq.to(q.dtype), dk.to(q.dtype)
+    q, k = (t.contiguous(memory_format=fmt) for t in (q, k))
+    dattn, attn = dattn.contiguous(), attn.contiguous()
+    with torch.cuda.device(q.device):
+        dq = torch.empty_like(q, memory_format=fmt)
+        dk = torch.empty_like(k, memory_format=fmt)
+        _grouped_call(lib.cca_b200_attention_backward3d, lib.cca_b200_attention_workspace_bytes3d, 1,
+                      (dattn, attn, q, k, dq, dk), (Cq, T, H, W), dt, flags)
+    return dq, dk
+
+
+class _CCA3DAttentionFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, q, k, impl, deterministic):
+        attn = cca3d_attention_forward(q, k, impl, deterministic)
+        ctx.save_for_backward(q, k, attn)
+        ctx.impl = impl
+        ctx.deterministic = deterministic
+        return attn
+
+    @staticmethod
+    def backward(ctx, dattn):
+        q, k, attn = ctx.saved_tensors
+        dq, dk = cca3d_attention_backward(dattn, attn, q, k, ctx.impl, ctx.deterministic)
+        return dq, dk, None, None
+
+
+def cca3d_attention(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", deterministic=None) -> torch.Tensor:
+    """Differentiable attention map attn[B,T,H,W,H+W+T] (float32) of criss-cross attention over clips; the gradient flows
+    to q and k.  ``deterministic``: as for ``cca3d``; the mode is fixed when the forward runs and the backward uses it too."""
+    return _CCA3DAttentionFunction.apply(q, k, impl, _resolve_deterministic(deterministic))

@@ -11,7 +11,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import ops  # noqa: F401  (torch.ops.cca.attention)
+from . import ops  # noqa: F401  (torch.ops.cca.attention, attention3d)
 
 from .functional import (cca, cca3d, cca_backward, cca_forward, qkv_gemm_eligible, qkv_project, qkv_project_dgrad,
                          qkv_project_wgrad, qkv_wgrad_eligible, tc3d_eligible, tc_eligible)
@@ -184,7 +184,18 @@ class CrissCrossAttention3D(nn.Module):
         self.gamma = nn.Parameter(torch.zeros(1))
         self.impl = impl
 
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
+    def forward(self, x: torch.Tensor, return_attention: bool = False):
+        """``return_attention=True`` returns ``(y, attn)``: y exactly as without it, and the attention map
+        attn[B,T,H,W,H+W+T] (float32; column, row and time keys, ``ccnet_b200.functional.cca3d_attention_forward``),
+        differentiable back to x and the query / key convs.  The fused kernels never materialise the map, so it costs two
+        more Cq-channel 1x1x1 convs, a second statistics pass and B*T*H*W*(H+W+T)*4 bytes."""
+        y = self._step(x)
+        if not return_attention:
+            return y
+        q, k = self.query_conv(x), self.key_conv(x)
+        return y, torch.ops.cca.attention3d(q, k, self.impl)
+
+    def _step(self, x: torch.Tensor) -> torch.Tensor:
         if not x.is_cuda:
             raise RuntimeError("ccnet_b200.CrissCrossAttention3D runs on CUDA (H100, sm_90) only")
         B, C, T, H, W = x.shape

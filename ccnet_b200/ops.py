@@ -7,10 +7,12 @@
     torch.ops.cca.attention_backward(dattn, attn, q, k)   -> (dq, dk)
     torch.ops.cca.forward3d(q, k, v)                      -> (out, lse)      clips [B,C,T,H,W], lse [B,T,H,W]
     torch.ops.cca.backward3d(dout, q, k, v, out, lse)     -> (dq, dk, dv)
+    torch.ops.cca.attention3d(q, k)                       -> attn            [B,T,H,W,H+W+T] fp32 (column | row | time)
+    torch.ops.cca.attention3d_backward(dattn, attn, q, k) -> (dq, dk)
 
 CUDA implementations call the C ABI (ccnet_b200.functional -> libcca_b200.so); FakeTensor ("meta") implementations give
 shapes / dtypes / memory formats so that ``torch.compile`` and ``torch.export`` trace through ``networks/ccnet.py`` without a
-graph break; autograd is registered on ``forward``, ``forward_residual``, ``attention`` and ``forward3d``.  Registration happens through ``torch.library``
+graph break; autograd is registered on ``forward``, ``forward_residual``, ``attention``, ``forward3d`` and ``attention3d``.  Registration happens through ``torch.library``
 (the Python face of TORCH_LIBRARY): the kernels themselves stay behind the torch-free C ABI."""
 from __future__ import annotations
 
@@ -174,3 +176,39 @@ def _fwd3d_backward(ctx, dout, dlse):
 
 
 forward3d.register_autograd(_fwd3d_backward, setup_context=_fwd_setup)
+
+
+# ---- the attention map over clips:  attention3d(q, k) -> attn[B,T,H,W,H+W+T] fp32,
+#      attention3d_backward(dattn, attn, q, k) -> (dq, dk)
+@torch.library.custom_op("cca::attention3d", mutates_args=(), device_types="cuda")
+def attention3d(q: Tensor, k: Tensor, impl: str = "auto") -> Tensor:
+    return F_.cca3d_attention_forward(q, k, impl)
+
+
+@attention3d.register_fake
+def _(q, k, impl="auto"):
+    B, _, T, H, W = q.shape
+    return q.new_empty((B, T, H, W, H + W + T), dtype=torch.float32)
+
+
+@torch.library.custom_op("cca::attention3d_backward", mutates_args=(), device_types="cuda")
+def attention3d_backward(dattn: Tensor, attn: Tensor, q: Tensor, k: Tensor, impl: str = "auto") -> Tuple[Tensor, Tensor]:
+    return F_.cca3d_attention_backward(dattn, attn, q, k, impl)
+
+
+@attention3d_backward.register_fake
+def _(dattn, attn, q, k, impl="auto"):
+    B, Cq, T, H, W = q.shape
+    cl = impl != "simt" and F_.attention3d_tc_eligible(B, Cq, T, H, W, q.dtype)
+    fmt = torch.channels_last_3d if cl else torch.contiguous_format
+    mk = lambda t: torch.empty(t.shape, dtype=t.dtype, device=t.device).contiguous(memory_format=fmt)
+    return mk(q), mk(k)
+
+
+def _attn3d_backward(ctx, dattn):
+    q, k, attn = ctx.saved_tensors
+    dq, dk = torch.ops.cca.attention3d_backward(dattn.contiguous(), attn, q, k, ctx.impl)
+    return dq, dk, None
+
+
+attention3d.register_autograd(_attn3d_backward, setup_context=_attn_setup)

@@ -222,6 +222,26 @@ CCA_API int cca_b200_backward3d(const void *dout, const void *q, const void *k, 
                                 int B, int Cq, int C, int T, int H, int W, int dtype, unsigned flags, void *cuda_stream);
 
 /*
+ * The attention map of the 3D op above and its gradient:
+ *   attn[b,t,h,w,g], fp32 contiguous [B,T,H,W,H+W+T]: g < H the weight of column key (t,g,w) (0 at g == h), H <= g < H+W
+ *                   that of row key (t,h,g-H), g >= H+W that of time key (g-H-W,h,w) (0 at g-H-W == t); normalised by the
+ *                   lse of cca_b200_forward3d.  At T = 1, attn[...,:H+W] is the 2D map of every frame and attn[...,H+W] is 0.
+ *   backward: as for cca_b200_attention_backward, over the H+W+T entries of a row.
+ * NDHWC q, k (and dq, dk) with CCA_FLAG_NHWC: the tensor-core path (cca_b200_attention_tc3d_supported: the shapes
+ * cca_b200_attention_tc_supported covers for B*T frames, and 1 <= T <= 32).  NCDHW-contiguous q, k: generic kernels of any
+ * Cq and shape.  Flags, the deterministic mode and alignment as for cca_b200_attention_forward / _backward: attn and dattn
+ * need only the alignment of a float; indices into the map are 64-bit.  Workspace: cca_b200_attention_workspace_bytes3d for
+ * the same flags (one size that covers whichever family runs).
+ */
+CCA_API int cca_b200_attention_tc3d_supported(int B, int Cq, int T, int H, int W, int dtype);
+CCA_API size_t cca_b200_attention_workspace_bytes3d(int backward, int B, int Cq, int T, int H, int W, int dtype, unsigned flags);
+CCA_API int cca_b200_attention_forward3d(const void *q, const void *k, float *attn, void *workspace, size_t workspace_bytes,
+                                         int B, int Cq, int T, int H, int W, int dtype, unsigned flags, void *cuda_stream);
+CCA_API int cca_b200_attention_backward3d(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk,
+                                          void *workspace, size_t workspace_bytes,
+                                          int B, int Cq, int T, int H, int W, int dtype, unsigned flags, void *cuda_stream);
+
+/*
  * Host-buffer variants: same maths, pointers are HOST memory (pinned or pageable).
  * They allocate device memory, copy in, run on an internal stream, copy out, free and
  * synchronise.  These are the calls a non-CUDA host language binds directly.
