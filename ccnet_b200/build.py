@@ -15,9 +15,10 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.environ.get("CCA_B200_LIBDIR") or os.path.join(HERE, "lib")      # (override: a second build flavour)
 LIB = os.path.join(LIBDIR, "libcca_b200.so")
 SOURCES = ["cca_capi.cu", "cca_simt.cu", "cca_simt_attn.cu", "cca_simt_3d.cu", "cca_tc_host.cu", "cca_tc_stats.cu", "cca_tc_fwd.cu", "cca_tc_bwd.cu", "cca_tc_f16.cu",
-           "cca_tc_det.cu", "cca_tc_attn.cu", "cca_tc_time.cu", "cca_tc_attn3d.cu", "cca_simt_attn3d.cu", "cca_gemm.cu"]
+           "cca_tc_det.cu", "cca_tc_attn.cu", "cca_tc_time.cu", "cca_tc_attn3d.cu", "cca_simt_attn3d.cu", "cca_gemm.cu",
+           "cca_tc_causal.cu", "cca_simt_causal.cu"]
 HEADERS = ["cca_common.cuh", "cca_sm90.cuh", "cca_tc_common.cuh", "cca_items.cuh", "cca_tc_stats.cuh", "cca_tc_fwd.cuh",
-           "cca_tc_bwd.cuh", "cca_tc_attn.cuh", "cca_tc_time.cuh", "../../include/cca_b200.h"]
+           "cca_tc_bwd.cuh", "cca_tc_attn.cuh", "cca_tc_time.cuh", "cca_tc_attn3d.cuh", "../../include/cca_b200.h"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo", "--use_fast_math",

@@ -14,6 +14,7 @@ LIB_PATH = os.environ.get("CCA_B200_LIB") or os.path.join(_HERE, "lib", "libcca_
 
 CCA_F32, CCA_BF16, CCA_F16 = 0, 1, 2
 CCA_FLAG_AUTO, CCA_FLAG_FORCE_SIMT, CCA_FLAG_FORCE_TC, CCA_FLAG_NHWC, CCA_FLAG_DETERMINISTIC = 0, 1, 2, 4, 8
+CCA_FLAG_CAUSAL = 16
 CCA_WS_FORWARD, CCA_WS_BACKWARD = 0, 1
 
 # every symbol include/cca_b200.h declares: name -> (restype, argtypes)
@@ -48,6 +49,8 @@ SYMBOLS = {
     "cca_b200_workspace_bytes3d": (_sz, [_i] * 8 + [_u]),
     "cca_b200_forward3d": (_i, [_vp] * 6 + [_sz] + [_i] * 7 + [_u, _vp]),
     "cca_b200_backward3d": (_i, [_vp] * 10 + [_sz] + [_i] * 7 + [_u, _vp]),
+    "cca_b200_workspace_bytes3d_step": (_sz, [_i] * 7 + [_u]),
+    "cca_b200_forward3d_step": (_i, [_vp] * 8 + [_sz] + [_i] * 7 + [_u, _vp]),
     "cca_b200_attention_tc3d_supported": (_i, [_i] * 6),
     "cca_b200_attention_workspace_bytes3d": (_sz, [_i] * 7 + [_u]),
     "cca_b200_attention_forward3d": (_i, [_vp] * 4 + [_sz] + [_i] * 6 + [_u, _vp]),

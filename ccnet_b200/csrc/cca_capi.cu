@@ -409,13 +409,14 @@ int cca_b200_forward3d(const void *q, const void *k, const void *v, void *out, f
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (fam == 0) {
         if (!simt3d_supported(d)) return fail(CCA_ERR_UNSUPPORTED, "H + W + T - 2 above 2048 for the generic 3D kernels%s%s");
-        cudaError_t e = simt_forward3d(q, k, v, out, lse, d, dtype, st);
+        cudaError_t e = (flags & CCA_FLAG_CAUSAL) ? simt_forward3d_causal(q, k, v, out, lse, d, dtype, st)
+                                                  : simt_forward3d(q, k, v, out, lse, d, dtype, st);
         return e != cudaSuccess ? cuda_fail(e, "simt_forward3d") : CCA_OK;
     }
     if (!aligned16({q, k, v, out, ws})) return fail(CCA_ERR_INVALID, kAlignMsg);
     const char *why = "";
     const bool det = (flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d.frames());
-    cudaError_t e = tc_forward3d(q, k, v, out, lse, ws, d, dtype, st, &why, det);
+    cudaError_t e = ((flags & CCA_FLAG_CAUSAL) ? tc_forward3d_causal : tc_forward3d)(q, k, v, out, lse, ws, d, dtype, st, &why, det);
     return e != cudaSuccess ? cuda_fail(e, why && *why ? why : "tc_forward3d") : CCA_OK;
 }
 
@@ -436,14 +437,55 @@ int cca_b200_backward3d(const void *dout, const void *q, const void *k, const vo
     if (fam == 0) {
         if (!simt3d_supported(d)) return fail(CCA_ERR_UNSUPPORTED, "H + W + T - 2 above 2048 for the generic 3D kernels%s%s");
         if (reinterpret_cast<uintptr_t>(ws) & 3) return fail(CCA_ERR_INVALID, "workspace must be 4-byte aligned%s%s");
-        cudaError_t e = simt_backward3d(dout, q, k, v, out, lse, dq, dk, dv, ws, d, dtype, st);
+        cudaError_t e = ((flags & CCA_FLAG_CAUSAL) ? simt_backward3d_causal : simt_backward3d)(dout, q, k, v, out, lse, dq, dk, dv, ws, d,
+                                                                                             dtype, st);
         return e != cudaSuccess ? cuda_fail(e, "simt_backward3d") : CCA_OK;
     }
     if (!aligned16({dout, q, k, v, out, dq, dk, dv, ws})) return fail(CCA_ERR_INVALID, kAlignMsg);
     const char *why = "";
     const bool det = (flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d.frames());
-    cudaError_t e = tc_backward3d(dout, q, k, v, out, lse, dq, dk, dv, ws, d, dtype, st, &why, det);
+    cudaError_t e = ((flags & CCA_FLAG_CAUSAL) ? tc_backward3d_causal : tc_backward3d)(dout, q, k, v, out, lse, dq, dk, dv, ws, d, dtype,
+                                                                                       st, &why, det);
     return e != cudaSuccess ? cuda_fail(e, why && *why ? why : "tc_backward3d") : CCA_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// streaming step of the causal 3D op: tensor-core path (cca_tc_causal.cu) or generic kernel (cca_simt_causal.cu)
+// ---------------------------------------------------------------------------------------
+size_t cca_b200_workspace_bytes3d_step(int B, int Cq, int C, int S, int H, int W, int dtype, unsigned flags)
+{
+    // the forward workspace of a one-frame clip: the frame's lse planes and the time plane
+    if (S < 0) return 0;
+    return cca_b200_workspace_bytes3d(CCA_WS_FORWARD, B, Cq, C, 1, H, W, dtype, flags);
+}
+
+int cca_b200_forward3d_step(const void *q, const void *k, const void *v, const void *k_cache, const void *v_cache, void *out, float *lse,
+                            void *ws, size_t ws_bytes, int B, int Cq, int C, int S, int H, int W, int dtype, unsigned flags,
+                            void *stream)
+{
+    if (S < 0) return fail(CCA_ERR_INVALID, "negative number of cached frames%s%s");
+    int rc = check_dims3d(B, Cq, C, S + 1, H, W, dtype);
+    if (rc) return rc;
+    if (!q || !k || !v || !out || !lse || !ws || (S > 0 && (!k_cache || !v_cache))) return fail(CCA_ERR_INVALID, "null pointer%s%s");
+    if (ws_bytes < cca_b200_workspace_bytes3d_step(B, Cq, C, S, H, W, dtype, flags))
+        return fail(CCA_ERR_WORKSPACE, "step workspace too small%s%s");
+    const Dims3 d3{B, Cq, C, S + 1, H, W};
+    const Dims d{B, Cq, C, H, W};
+    const int fam = kernel_family(flags, (flags & CCA_FLAG_NHWC) && tc3d_supported(d3, dtype), det_16bit_tiled(flags, d, dtype),
+                                  "3D step", "NCHW q, k, v and NCDHW caches");
+    if (fam < 0) return fam;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (fam == 0) {
+        if ((long)H + W + S - 1 > kMaxKeys3d || !simt3d_supported(d3))
+            return fail(CCA_ERR_UNSUPPORTED, "H + W + S - 1 above 2048 for the generic step kernel%s%s");
+        cudaError_t e = simt_forward3d_step(q, k, v, k_cache, v_cache, out, lse, d, S, dtype, st);
+        return e != cudaSuccess ? cuda_fail(e, "simt_forward3d_step") : CCA_OK;
+    }
+    if (!aligned16({q, k, v, out, ws}) || (S > 0 && !aligned16({k_cache, v_cache}))) return fail(CCA_ERR_INVALID, kAlignMsg);
+    const char *why = "";
+    const bool det = (flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d);
+    cudaError_t e = tc_forward3d_step(q, k, v, k_cache, v_cache, out, lse, ws, d, S, dtype, st, &why, det);
+    return e != cudaSuccess ? cuda_fail(e, why && *why ? why : "tc_forward3d_step") : CCA_OK;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -493,10 +535,11 @@ int cca_b200_attention_forward3d(const void *q, const void *k, float *attn, void
     if (fam == 1) {
         if (!aligned16({q, k, ws})) return fail(CCA_ERR_INVALID, kAlignMsg);
         const char *why = "";
-        cudaError_t e = tc_attention_forward3d(q, k, attn, ws, d, dtype, st, &why);
+        cudaError_t e = ((flags & CCA_FLAG_CAUSAL) ? tc_attention_forward3d_causal : tc_attention_forward3d)(q, k, attn, ws, d, dtype, st,
+                                                                                                         &why);
         return e != cudaSuccess ? cuda_fail(e, why && *why ? why : "tc_attention_forward3d") : CCA_OK;
     }
-    cudaError_t e = simt_attention_forward3d(q, k, attn, d, dtype, st);
+    cudaError_t e = ((flags & CCA_FLAG_CAUSAL) ? simt_attention_forward3d_causal : simt_attention_forward3d)(q, k, attn, d, dtype, st);
     return e != cudaSuccess ? cuda_fail(e, "simt_attention_forward3d") : CCA_OK;
 }
 
@@ -518,11 +561,13 @@ int cca_b200_attention_backward3d(const float *dattn, const float *attn, const v
     if (fam == 1) {
         if (!aligned16({q, k, dq, dk, ws})) return fail(CCA_ERR_INVALID, kAlignMsg);
         const char *why = "";
-        cudaError_t e = tc_attention_backward3d(dattn, attn, q, k, dq, dk, ws, d, dtype, st, &why, (flags & CCA_FLAG_DETERMINISTIC) != 0);
+        cudaError_t e = ((flags & CCA_FLAG_CAUSAL) ? tc_attention_backward3d_causal : tc_attention_backward3d)(
+            dattn, attn, q, k, dq, dk, ws, d, dtype, st, &why, (flags & CCA_FLAG_DETERMINISTIC) != 0);
         return e != cudaSuccess ? cuda_fail(e, why && *why ? why : "tc_attention_backward3d") : CCA_OK;
     }
     if (reinterpret_cast<uintptr_t>(ws) & 3) return fail(CCA_ERR_INVALID, "workspace must be 4-byte aligned%s%s");
-    cudaError_t e = simt_attention_backward3d(dattn, attn, q, k, dq, dk, ws, d, dtype, st);
+    cudaError_t e = ((flags & CCA_FLAG_CAUSAL) ? simt_attention_backward3d_causal : simt_attention_backward3d)(dattn, attn, q, k, dq, dk,
+                                                                                                              ws, d, dtype, st);
     return e != cudaSuccess ? cuda_fail(e, "simt_attention_backward3d") : CCA_OK;
 }
 

@@ -125,6 +125,25 @@ cudaError_t simt_backward3d(const void *dout, const void *q, const void *k, cons
                             void *dq, void *dk, void *dv, void *ws, Dims3 d, int dtype, cudaStream_t st);
 cudaError_t tc_backward3d(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
                           void *dq, void *dk, void *dv, void *ws, Dims3 d, int dtype, cudaStream_t st, const char **why, bool det);
+//   causal mode (CCA_FLAG_CAUSAL: the time keys of frame t are the frames s < t; cca_tc_causal.cu): the same passes and
+//   workspaces with the causal time kernels, and the streaming step: frame S of the causal forward from the new frame's q, k, v
+//   [B,H,W,c] and the caches kc [B,S,H,W,Cq], vc [B,S,H,W,C] (S <= kTimeMaxT - 1; workspace: tc_forward3d_workspace of
+//   Dims3{B, Cq, C, 1, H, W})
+cudaError_t tc_forward3d_causal(const void *q, const void *k, const void *v, void *out, float *lse, void *ws, Dims3 d, int dtype,
+                                cudaStream_t st, const char **why, bool det);
+cudaError_t tc_backward3d_causal(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
+                                 void *dq, void *dk, void *dv, void *ws, Dims3 d, int dtype, cudaStream_t st, const char **why,
+                                 bool det);
+cudaError_t tc_forward3d_step(const void *q, const void *k, const void *v, const void *kc, const void *vc, void *out, float *lse,
+                              void *ws, Dims d, int S, int dtype, cudaStream_t st, const char **why, bool det);
+//   generic kernels of causal mode (cca_simt_causal.cu), NCDHW tensors: the forward and backward (same limits and workspace as
+//   simt_forward3d / simt_backward3d) and the step on NCHW q, k, v and NCDHW caches (H + W + S - 1 <= kMaxKeys3d)
+cudaError_t simt_forward3d_causal(const void *q, const void *k, const void *v, void *out, float *lse, Dims3 d, int dtype,
+                                  cudaStream_t st);
+cudaError_t simt_backward3d_causal(const void *dout, const void *q, const void *k, const void *v, const void *out,
+                                   const float *lse, void *dq, void *dk, void *dv, void *ws, Dims3 d, int dtype, cudaStream_t st);
+cudaError_t simt_forward3d_step(const void *q, const void *k, const void *v, const void *kc, const void *vc, void *out, float *lse,
+                                Dims d, int S, int dtype, cudaStream_t st);
 
 // the attention map attn[B,H,W,H+W] (fp32) and its gradient w.r.t. q, k (Dims.C is not used)
 //   generic kernels, NCHW q, k (cca_simt_attn.cu); the backward's workspace is rho [B*H*W]
@@ -157,6 +176,15 @@ cudaError_t tc_attention_forward3d(const void *q, const void *k, float *attn, vo
                                    const char **why);
 cudaError_t tc_attention_backward3d(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk, void *ws,
                                     Dims3 d, int dtype, cudaStream_t st, const char **why, bool det);
+//   causal mode: the same passes with the causal time map kernels (cca_tc_causal.cu) and the causal generic kernels
+//   (cca_simt_causal.cu); the map keeps its layout, time entries s >= t are 0
+cudaError_t tc_attention_forward3d_causal(const void *q, const void *k, float *attn, void *ws, Dims3 d, int dtype, cudaStream_t st,
+                                          const char **why);
+cudaError_t tc_attention_backward3d_causal(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk,
+                                           void *ws, Dims3 d, int dtype, cudaStream_t st, const char **why, bool det);
+cudaError_t simt_attention_forward3d_causal(const void *q, const void *k, float *attn, Dims3 d, int dtype, cudaStream_t st);
+cudaError_t simt_attention_backward3d_causal(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk,
+                                             void *ws, Dims3 d, int dtype, cudaStream_t st);
 
 // wgmma GEMMs of the 1x1 Q/K/V projections (cca_gemm.cu), fp32 channels-last tensors as [pixels, channels] matrices
 bool qkv_gemm_supported(int C, int Cq);

@@ -70,15 +70,16 @@ def _check_saved(q, v, dout, out, lse):
         raise RuntimeError(f"ccnet_b200: lse must be the forward's float32 [B,{s}] tensor on the same device")
 
 
-def _plan(impl: str, det: bool, covered, q, v=None):
+def _plan(impl: str, det: bool, covered, q, v=None, causal: bool = False):
     """(use_tc, flags, memory format) of a call: the tensor-core kernels on channels-last memory where ``covered()``, the
     op's coverage query, says they take the shape and ``impl`` allows them, else the generic kernels on contiguous memory.
-    impl="tc" on a shape the tensor-core kernels do not cover raises."""
+    impl="tc" on a shape the tensor-core kernels do not cover raises.  ``causal`` adds CCA_FLAG_CAUSAL (3D ops)."""
     use_tc = impl in ("auto", "tc") and covered()
     if impl == "tc" and not use_tc:
         shapes = f"q{tuple(q.shape)}" + ("" if v is None else f" v{tuple(v.shape)}")
         raise RuntimeError(f"ccnet_b200: tensor-core kernels do not cover {shapes} {q.dtype}")
-    flags = _IMPL_FLAGS[impl] | (capi.CCA_FLAG_NHWC if use_tc else 0) | (capi.CCA_FLAG_DETERMINISTIC if det else 0)
+    flags = (_IMPL_FLAGS[impl] | (capi.CCA_FLAG_NHWC if use_tc else 0) | (capi.CCA_FLAG_DETERMINISTIC if det else 0)
+             | (capi.CCA_FLAG_CAUSAL if causal else 0))
     fmt = (torch.channels_last_3d if q.dim() == 5 else torch.channels_last) if use_tc else torch.contiguous_format
     return use_tc, flags, fmt
 
@@ -401,7 +402,8 @@ def tc3d_eligible(B: int, Cq: int, C: int, T: int, H: int, W: int, dtype: torch.
     return dtype in _DTYPES and capi.load().cca_b200_tc3d_supported(capi.CCA_WS_FORWARD, B, Cq, C, T, H, W, _DTYPES[dtype]) == 1
 
 
-def cca3d_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", deterministic=None):
+def cca3d_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", deterministic=None,
+                  causal: bool = False):
     """Criss-cross attention over clips: returns (out[B,C,T,H,W], lse[B,T,H,W] fp32).  q, k are [B,Cq,T,H,W], v [B,C,T,H,W].
     Pixel (b,t,h,w) attends to its column (self masked), its row and its time line (self masked), one softmax over the
     H + W + T logits.  At T = 1 this is ``cca_forward`` on every frame.
@@ -409,7 +411,10 @@ def cca3d_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str =
     ``impl``: "auto" (the tensor-core path where ``tc3d_eligible``, else the generic kernels), "tc" (tensor-core path or
     error), "simt" (generic kernels: any Cq and C, H + W + T - 2 <= 2048).  The tensor-core path works on channels_last_3d
     memory (inputs in another format are converted, the output is channels_last_3d), the generic kernels on contiguous
-    NCDHW memory.  ``deterministic`` as for ``cca_forward``."""
+    NCDHW memory.  ``deterministic`` as for ``cca_forward``.
+
+    ``causal``: the time keys of frame t are the frames s < t only (CCA_FLAG_CAUSAL); frame 0 then has no time key and is
+    ``cca_forward`` on its frame.  For streaming inference, ``cca3d_step`` produces one new frame from cached keys and values."""
     _check_inputs(q, k, v, rank=5)
     det = _resolve_deterministic(deterministic)
     lib = capi.load()
@@ -417,9 +422,9 @@ def cca3d_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str =
     C = v.shape[1]
     dt = _DTYPES[q.dtype]
     use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc3d_supported(capi.CCA_WS_FORWARD, B, Cq, C, T, H, W, dt) == 1,
-                               q, v)
+                               q, v, causal)
     if use_tc and _upcast(q.dtype, H, W, det, T):
-        out32, lse = cca3d_forward(q.float(), k.float(), v.float(), impl, det)
+        out32, lse = cca3d_forward(q.float(), k.float(), v.float(), impl, det, causal)
         return out32.to(q.dtype), lse
     q, k, v = (t.contiguous(memory_format=fmt) for t in (q, k, v))
     with torch.cuda.device(q.device):
@@ -430,9 +435,9 @@ def cca3d_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str =
     return out, lse
 
 
-def cca3d_backward(dout, q, k, v, out, lse, impl: str = "auto", deterministic=None):
+def cca3d_backward(dout, q, k, v, out, lse, impl: str = "auto", deterministic=None, causal: bool = False):
     """Gradients (dq, dk, dv) of ``cca3d_forward`` given dout and the saved forward tensors.  Same ``impl`` / memory-format /
-    ``deterministic`` rules as ``cca3d_forward``."""
+    ``deterministic`` / ``causal`` rules as ``cca3d_forward``."""
     _check_inputs(q, k, v, rank=5)
     _check_saved(q, v, dout, out, lse)
     det = _resolve_deterministic(deterministic)
@@ -441,9 +446,9 @@ def cca3d_backward(dout, q, k, v, out, lse, impl: str = "auto", deterministic=No
     C = v.shape[1]
     dt = _DTYPES[q.dtype]
     use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc3d_supported(capi.CCA_WS_BACKWARD, B, Cq, C, T, H, W, dt) == 1,
-                               q, v)
+                               q, v, causal)
     if use_tc and _upcast(q.dtype, H, W, det, T):
-        res = cca3d_backward(dout.float(), q.float(), k.float(), v.float(), out.float(), lse, impl, det)
+        res = cca3d_backward(dout.float(), q.float(), k.float(), v.float(), out.float(), lse, impl, det, causal)
         return tuple(g.to(q.dtype) for g in res)
     dout, q, k, v, out = (t.contiguous(memory_format=fmt) for t in (dout, q, k, v, out))
     lse = lse.contiguous()
@@ -458,23 +463,26 @@ def cca3d_backward(dout, q, k, v, out, lse, impl: str = "auto", deterministic=No
 
 class _CCA3DFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, impl, deterministic):
-        out, lse = cca3d_forward(q, k, v, impl, deterministic)
+    def forward(ctx, q, k, v, impl, deterministic, causal):
+        out, lse = cca3d_forward(q, k, v, impl, deterministic, causal)
         ctx.save_for_backward(q, k, v, out, lse)
         ctx.impl = impl
         ctx.deterministic = deterministic
+        ctx.causal = causal
         return out
 
     @staticmethod
     def backward(ctx, dout):
         q, k, v, out, lse = ctx.saved_tensors
-        dq, dk, dv = cca3d_backward(dout, q, k, v, out, lse, ctx.impl, ctx.deterministic)
-        return dq, dk, dv, None, None
+        dq, dk, dv = cca3d_backward(dout, q, k, v, out, lse, ctx.impl, ctx.deterministic, ctx.causal)
+        return dq, dk, dv, None, None, None
 
 
-def cca3d(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", deterministic=None) -> torch.Tensor:
-    """Differentiable criss-cross attention over clips (out only); see ``cca3d_forward``."""
-    return _CCA3DFunction.apply(q, k, v, impl, _resolve_deterministic(deterministic))
+def cca3d(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", deterministic=None,
+          causal: bool = False) -> torch.Tensor:
+    """Differentiable criss-cross attention over clips (out only); see ``cca3d_forward``.  The ``causal`` mode of the forward
+    is kept for the backward."""
+    return _CCA3DFunction.apply(q, k, v, impl, _resolve_deterministic(deterministic), bool(causal))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -485,20 +493,22 @@ def attention3d_tc_eligible(B: int, Cq: int, T: int, H: int, W: int, dtype: torc
     return dtype in _DTYPES and capi.load().cca_b200_attention_tc3d_supported(B, Cq, T, H, W, _DTYPES[dtype]) == 1
 
 
-def cca3d_attention_forward(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", deterministic=None) -> torch.Tensor:
+def cca3d_attention_forward(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", deterministic=None,
+                            causal: bool = False) -> torch.Tensor:
     """The attention map of ``cca3d_forward``, attn[B,T,H,W,H+W+T] float32: attn[b,t,h,w,g] is the weight of column key
     (t, g, w) for g < H (0 at g == h), of row key (t, h, g - H) for H <= g < H + W and of time key (g - H - W, h, w) after
     that (0 at g - H - W == t).  It is normalised by the lse of ``cca3d_forward``; at T = 1, attn[..., :H+W] is
     ``cca_attention_forward`` of every frame and attn[..., H+W] is 0.
 
     ``impl`` as for ``cca3d_forward`` (the generic kernels take any Cq and shape).  Every map element is written once, so
-    the result is the same in every mode; ``deterministic`` only sets the flag the C ABI is called with."""
+    the result is the same in every mode; ``deterministic`` only sets the flag the C ABI is called with.  ``causal``: the map
+    of ``cca3d_forward(..., causal=True)``, same layout, time entries H + W + s with s >= t exactly 0."""
     _check_inputs(q, k, rank=5)
     det = _resolve_deterministic(deterministic)
     lib = capi.load()
     B, Cq, T, H, W = q.shape
     dt = _DTYPES[q.dtype]
-    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_attention_tc3d_supported(B, Cq, T, H, W, dt) == 1, q)
+    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_attention_tc3d_supported(B, Cq, T, H, W, dt) == 1, q, causal=causal)
     q, k = (t.contiguous(memory_format=fmt) for t in (q, k))
     with torch.cuda.device(q.device):
         attn = torch.empty((B, T, H, W, H + W + T), dtype=torch.float32, device=q.device)
@@ -509,10 +519,10 @@ def cca3d_attention_forward(q: torch.Tensor, k: torch.Tensor, impl: str = "auto"
     return attn
 
 
-def cca3d_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministic=None):
+def cca3d_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministic=None, causal: bool = False):
     """Gradients (dq, dk) of ``cca3d_attention_forward`` given dattn = dL/dattn and the forward's map, in the closed form
-    of ``cca_attention_backward`` over the H + W + T entries of a row.  Same ``impl`` / memory-format / ``deterministic``
-    rules as ``cca3d_backward``."""
+    of ``cca_attention_backward`` over the H + W + T entries of a row.  Same ``impl`` / memory-format / ``deterministic`` /
+    ``causal`` rules as ``cca3d_backward``."""
     _check_inputs(q, k, rank=5)
     det = _resolve_deterministic(deterministic)
     lib = capi.load()
@@ -521,9 +531,9 @@ def cca3d_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministi
         if t.dtype != torch.float32 or tuple(t.shape) != (B, T, H, W, H + W + T) or t.device != q.device:
             raise RuntimeError(f"ccnet_b200: {name} must be a float32 [B,T,H,W,H+W+T] tensor on the device of q, k")
     dt = _DTYPES[q.dtype]
-    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_attention_tc3d_supported(B, Cq, T, H, W, dt) == 1, q)
+    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_attention_tc3d_supported(B, Cq, T, H, W, dt) == 1, q, causal=causal)
     if use_tc and _upcast(q.dtype, H, W, det, T):
-        dq, dk = cca3d_attention_backward(dattn, attn, q.float(), k.float(), impl, det)
+        dq, dk = cca3d_attention_backward(dattn, attn, q.float(), k.float(), impl, det, causal)
         return dq.to(q.dtype), dk.to(q.dtype)
     q, k = (t.contiguous(memory_format=fmt) for t in (q, k))
     dattn, attn = dattn.contiguous(), attn.contiguous()
@@ -537,21 +547,73 @@ def cca3d_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministi
 
 class _CCA3DAttentionFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, impl, deterministic):
-        attn = cca3d_attention_forward(q, k, impl, deterministic)
+    def forward(ctx, q, k, impl, deterministic, causal):
+        attn = cca3d_attention_forward(q, k, impl, deterministic, causal)
         ctx.save_for_backward(q, k, attn)
         ctx.impl = impl
         ctx.deterministic = deterministic
+        ctx.causal = causal
         return attn
 
     @staticmethod
     def backward(ctx, dattn):
         q, k, attn = ctx.saved_tensors
-        dq, dk = cca3d_attention_backward(dattn, attn, q, k, ctx.impl, ctx.deterministic)
-        return dq, dk, None, None
+        dq, dk = cca3d_attention_backward(dattn, attn, q, k, ctx.impl, ctx.deterministic, ctx.causal)
+        return dq, dk, None, None, None
 
 
-def cca3d_attention(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", deterministic=None) -> torch.Tensor:
+def cca3d_attention(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", deterministic=None,
+                    causal: bool = False) -> torch.Tensor:
     """Differentiable attention map attn[B,T,H,W,H+W+T] (float32) of criss-cross attention over clips; the gradient flows
-    to q and k.  ``deterministic``: as for ``cca3d``; the mode is fixed when the forward runs and the backward uses it too."""
-    return _CCA3DAttentionFunction.apply(q, k, impl, _resolve_deterministic(deterministic))
+    to q and k.  ``deterministic`` and ``causal``: as for ``cca3d``; the modes are fixed when the forward runs and the
+    backward uses them too."""
+    return _CCA3DAttentionFunction.apply(q, k, impl, _resolve_deterministic(deterministic), bool(causal))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# streaming step of causal criss-cross attention over clips
+# ---------------------------------------------------------------------------------------------------------------------
+def cca3d_step(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor,
+               impl: str = "auto", deterministic=None):
+    """One new frame of causal criss-cross attention over clips, for streaming inference: returns (out[B,C,H,W],
+    lse[B,H,W] fp32).  q, k [B,Cq,H,W] and v [B,C,H,W] are the new frame's; k_cache [B,Cq,S,H,W] and v_cache [B,C,S,H,W]
+    the keys and values of the S previous frames in time order.  By definition the result is frame S of
+    ``cca3d_forward(..., causal=True)`` on the clip whose frames 0..S-1 have those keys and values and whose frame S has
+    k, v (the past frames' queries do not enter); S = 0 is ``cca_forward`` on the frame.
+
+    ``impl`` / ``deterministic`` as for ``cca3d_forward``: the tensor-core path (channels-last frame, channels_last_3d
+    caches, S <= 31) where it covers a clip of S + 1 frames, else the generic kernel (contiguous tensors, any Cq and C,
+    H + W + S - 1 <= 2048).  There is no backward: train with ``cca3d(..., causal=True)``."""
+    if torch.is_grad_enabled() and any(t.requires_grad for t in (q, k, v, k_cache, v_cache)):
+        raise RuntimeError("ccnet_b200: cca3d_step has no backward (streaming inference); train with "
+                           "cca3d(q, k, v, causal=True) on clips")
+    _check_inputs(q, k, v)
+    B, Cq, H, W = q.shape
+    C = v.shape[1]
+    if (k_cache.dim() != 5 or v_cache.dim() != 5 or tuple(k_cache.shape[:2]) != (B, Cq) or tuple(k_cache.shape[3:]) != (H, W)
+            or tuple(v_cache.shape) != (B, C, k_cache.shape[2], H, W)):
+        raise RuntimeError(f"ccnet_b200: expected k_cache [B,Cq,S,H,W] and v_cache [B,C,S,H,W] for q{tuple(q.shape)} "
+                           f"v{tuple(v.shape)}, got {tuple(k_cache.shape)}, {tuple(v_cache.shape)}")
+    if any(t.dtype != q.dtype or t.device != q.device for t in (k_cache, v_cache)):
+        raise RuntimeError("ccnet_b200: k_cache, v_cache must match q, k, v in dtype and device")
+    S = k_cache.shape[2]
+    det = _resolve_deterministic(deterministic)
+    lib = capi.load()
+    dt = _DTYPES[q.dtype]
+    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc3d_supported(capi.CCA_WS_FORWARD, B, Cq, C, S + 1, H, W, dt) == 1,
+                               q, v)
+    if use_tc and _upcast(q.dtype, H, W, det, S + 1):
+        out32, lse = cca3d_step(q.float(), k.float(), v.float(), k_cache.float(), v_cache.float(), impl, det)
+        return out32.to(q.dtype), lse
+    cfmt = torch.channels_last_3d if use_tc else torch.contiguous_format
+    q, k, v = (t.contiguous(memory_format=fmt) for t in (q, k, v))
+    k_cache, v_cache = (t.contiguous(memory_format=cfmt) for t in (k_cache, v_cache))
+    with torch.cuda.device(q.device):
+        out = torch.empty_like(v, memory_format=fmt)
+        lse = torch.empty((B, H, W), dtype=torch.float32, device=q.device)
+        ws = _workspace(lib.cca_b200_workspace_bytes3d_step(B, Cq, C, S, H, W, dt, flags), q.device)
+        rc = lib.cca_b200_forward3d_step(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_cache.data_ptr() if S else None,
+                                         v_cache.data_ptr() if S else None, out.data_ptr(), lse.data_ptr(), ws.data_ptr(),
+                                         ws.numel(), B, Cq, C, S, H, W, dt, flags, _stream_ptr(q.device))
+        capi.check(rc, "cca_b200_forward3d_step")
+    return out, lse

@@ -13,7 +13,7 @@ import torch.nn.functional as F
 
 from . import ops  # noqa: F401  (torch.ops.cca.attention, attention3d)
 
-from .functional import (cca, cca3d, cca_backward, cca_forward, qkv_gemm_eligible, qkv_project, qkv_project_dgrad,
+from .functional import (cca, cca3d, cca3d_step, cca_backward, cca_forward, qkv_gemm_eligible, qkv_project, qkv_project_dgrad,
                          qkv_project_wgrad, qkv_wgrad_eligible, tc3d_eligible, tc_eligible)
 
 
@@ -174,15 +174,20 @@ class CrissCrossAttention3D(nn.Module):
 
     Where the tensor-core path covers the shape, the projections (per pixel) run as GEMMs on the [B*T, C, H, W] frames view
     of channels_last_3d x (a view, no copy) and q, k, v come out channels_last_3d, the layout of those kernels.  Elsewhere
-    (other channel counts, T > 32, lines over 896, ``impl="simt"``) the convs are stock Conv3d and the generic kernels run."""
+    (other channel counts, T > 32, lines over 896, ``impl="simt"``) the convs are stock Conv3d and the generic kernels run.
 
-    def __init__(self, in_dim: int, impl: str = "auto"):
+    ``causal=True``: frame t attends to the frames before it only (its column and row as before), for models that run on a
+    live stream; the parameters and state-dict keys are those of the bidirectional module.  ``step`` then produces one new
+    frame from a cache of the past frames' keys and values."""
+
+    def __init__(self, in_dim: int, impl: str = "auto", causal: bool = False):
         super().__init__()
         self.query_conv = nn.Conv3d(in_channels=in_dim, out_channels=in_dim // 8, kernel_size=1)
         self.key_conv = nn.Conv3d(in_channels=in_dim, out_channels=in_dim // 8, kernel_size=1)
         self.value_conv = nn.Conv3d(in_channels=in_dim, out_channels=in_dim, kernel_size=1)
         self.gamma = nn.Parameter(torch.zeros(1))
         self.impl = impl
+        self.causal = causal
 
     def forward(self, x: torch.Tensor, return_attention: bool = False):
         """``return_attention=True`` returns ``(y, attn)``: y exactly as without it, and the attention map
@@ -193,7 +198,7 @@ class CrissCrossAttention3D(nn.Module):
         if not return_attention:
             return y
         q, k = self.query_conv(x), self.key_conv(x)
-        return y, torch.ops.cca.attention3d(q, k, self.impl)
+        return y, torch.ops.cca.attention3d(q, k, self.impl, self.causal)
 
     def _step(self, x: torch.Tensor) -> torch.Tensor:
         if not x.is_cuda:
@@ -209,4 +214,51 @@ class CrissCrossAttention3D(nn.Module):
             q, k, v = self.query_conv(x), self.key_conv(x), self.value_conv(x)
         if q.dtype != v.dtype or k.dtype != v.dtype:       # autocast corner: keep one dtype
             q, k = q.to(v.dtype), k.to(v.dtype)
-        return torch.addcmul(x, self.gamma, cca3d(q, k, v, self.impl))
+        return torch.addcmul(x, self.gamma, cca3d(q, k, v, self.impl, causal=self.causal))
+
+    @torch.no_grad()
+    def step(self, x_t: torch.Tensor, state=None, max_frames: int = 31):
+        """One frame of a stream through the causal module: x_t [B, C, H, W] -> (y_t, state).  ``state`` (None for the first
+        frame) holds the keys and values of up to ``max_frames`` previous frames in time order; pass the returned one with the
+        next frame.  q, k, v of the frame are the Conv3d projections applied as 1x1 convs, y_t = gamma * out + x_t.
+
+        Frame by frame, ``step`` gives the frames of ``forward(clip)`` while the clip has at most ``max_frames + 1`` frames;
+        after that the window slides, and y_t is the last frame of the causal forward on the last ``max_frames + 1`` frames.
+        The cost is the 2D op on one frame plus a time pass over the cached frames, instead of the whole window again, plus a
+        copy of the cache: each call writes a new one with the new frame's k, v appended.  Inference only (no gradient)."""
+        if not self.causal:
+            raise RuntimeError("ccnet_b200.CrissCrossAttention3D.step needs a causal module: CrissCrossAttention3D(in_dim, "
+                               "causal=True); a bidirectional frame attends to future frames")
+        if not x_t.is_cuda:
+            raise RuntimeError("ccnet_b200.CrissCrossAttention3D runs on CUDA (H100, sm_90) only")
+        if max_frames < 0:
+            raise ValueError("max_frames must be >= 0")
+        B, C, H, W = x_t.shape
+        S = 0 if state is None else state[0].shape[2]
+        tc = self.impl != "simt" and tc3d_eligible(B, C // 8, C, S + 1, H, W, x_t.dtype)
+        if tc:
+            # channels-last projections: q, k, v come out in the layout of the tensor-core step, and the cache is kept
+            # channels_last_3d, so the step does not convert it again
+            x_t = x_t.contiguous(memory_format=torch.channels_last)
+        q, k, v = (F.conv2d(x_t, conv.weight.squeeze(-1), conv.bias) for conv in (self.query_conv, self.key_conv, self.value_conv))
+        if q.dtype != v.dtype or k.dtype != v.dtype:       # autocast corner: keep one dtype
+            q, k = q.to(v.dtype), k.to(v.dtype)
+        if state is None:
+            k_cache, v_cache = k.unsqueeze(2)[:, :, :0], v.unsqueeze(2)[:, :, :0]
+        else:
+            k_cache, v_cache = state
+        out, _ = cca3d_step(q, k, v, k_cache, v_cache, self.impl)
+        y = torch.addcmul(x_t, self.gamma.to(out.dtype), out)
+        fmt = torch.channels_last_3d if tc else torch.contiguous_format
+        return y, (_append_frame(k_cache, k, max_frames, fmt), _append_frame(v_cache, v, max_frames, fmt))
+
+
+def _append_frame(cache: torch.Tensor, x: torch.Tensor, keep: int, fmt) -> torch.Tensor:
+    """the last `keep` frames of cat(cache [B,c,S,H,W], x [B,c,H,W]) along time, as one new tensor in memory format `fmt`"""
+    n = min(cache.shape[2] + 1, keep)
+    out = torch.empty((*x.shape[:2], n, *x.shape[2:]), dtype=x.dtype, device=x.device, memory_format=fmt)
+    if n > 1:
+        out[:, :, :n - 1].copy_(cache[:, :, cache.shape[2] - (n - 1):])
+    if n > 0:
+        out[:, :, n - 1].copy_(x)
+    return out

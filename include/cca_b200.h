@@ -84,6 +84,12 @@ typedef enum cca_status {
                                  * onto the output in no fixed order, and one more kernel adds the planes
                                  * in a fixed order.  fp32 only there: 16-bit I/O on such lines returns
                                  * CCA_ERR_UNSUPPORTED (call CCA_F32 on upcast tensors).                   */
+#define CCA_FLAG_CAUSAL 16u     /* causal criss-cross attention over clips: honoured by cca_b200_forward3d, _backward3d,
+                                 * _attention_forward3d and _attention_backward3d (the 2D entry points handle flag bits as
+                                 * before).  The time keys of frame t are the frames s < t.  Workspace sizes are those
+                                 * without the flag.  The bit was added without a version change: a library without it
+                                 * ignores the bit and computes the bidirectional op.  A caller detects causal support by
+                                 * the presence of the cca_b200_forward3d_step symbol (dlsym / GetProcAddress).           */
 
 /* which workspace */
 #define CCA_WS_FORWARD 0
@@ -220,6 +226,30 @@ CCA_API int cca_b200_backward3d(const void *dout, const void *q, const void *k, 
                                 const void *out, const float *lse, void *dq, void *dk, void *dv,
                                 void *workspace, size_t workspace_bytes,
                                 int B, int Cq, int C, int T, int H, int W, int dtype, unsigned flags, void *cuda_stream);
+
+/*
+ * Causal mode (CCA_FLAG_CAUSAL) of the 3D op and its map: pixel (b,t,h,w) attends to its column (self masked), its row and
+ * the time keys (b,s,h,w) with s < t only, one softmax over them.  Frame 0 has no time key: its row is the 2D step's.  The
+ * map keeps its layout [B,T,H,W,H+W+T]; entries H+W+s with s >= t are exactly 0.  Same coverage, workspace, deterministic
+ * mode and limits as without the flag.
+ *
+ * Streaming step: frame S of the causal forward, from the new frame and caches of the S previous frames' keys and values
+ * (the queries of past frames do not enter).  q, k [B,Cq,H,W] and v, out [B,C,H,W] of the new frame, k_cache [B,Cq,S,H,W],
+ * v_cache [B,C,S,H,W] in time order, lse [B,H,W] fp32.  out and lse equal frame S of cca_b200_forward3d with CCA_FLAG_CAUSAL
+ * on the clip whose frames 0..S-1 have keys and values k_cache, v_cache and whose frame S has k, v: bit for bit in fp32 on the
+ * tensor-core path on lines of at most 112 pixels and with CCA_FLAG_DETERMINISTIC (longer lines without it: the 2D passes
+ * add their partial results in no fixed order, in the clip forward as in the step).  S = 0 (the caches may then be NULL) is the 2D step on the frame.
+ * CCA_FLAG_NHWC: q, k, v, out channels-last, the caches NDHWC (torch.channels_last_3d); the tensor-core path, covering what
+ * cca_b200_tc3d_supported(CCA_WS_FORWARD, B, Cq, C, S + 1, H, W, dtype) covers (S <= 31).  Without it: NCHW / NCDHW tensors
+ * and the generic kernel, any Cq and C, H + W + S - 1 <= 2048.  Flags, alignment and the deterministic mode as for
+ * cca_b200_forward3d (16-bit I/O with CCA_FLAG_DETERMINISTIC on tiled lines: CCA_ERR_UNSUPPORTED).  Every argument is checked
+ * before any CUDA call (S < 0 and NULL caches with S > 0 are CCA_ERR_INVALID); nothing is written on an error.  No backward:
+ * causal training uses cca_b200_forward3d / _backward3d with CCA_FLAG_CAUSAL.
+ */
+CCA_API size_t cca_b200_workspace_bytes3d_step(int B, int Cq, int C, int S, int H, int W, int dtype, unsigned flags);
+CCA_API int cca_b200_forward3d_step(const void *q, const void *k, const void *v, const void *k_cache, const void *v_cache,
+                                    void *out, float *lse, void *workspace, size_t workspace_bytes,
+                                    int B, int Cq, int C, int S, int H, int W, int dtype, unsigned flags, void *cuda_stream);
 
 /*
  * The attention map of the 3D op above and its gradient:
