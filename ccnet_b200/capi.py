@@ -55,6 +55,11 @@ SYMBOLS = {
     "cca_b200_attention_workspace_bytes3d": (_sz, [_i] * 7 + [_u]),
     "cca_b200_attention_forward3d": (_i, [_vp] * 4 + [_sz] + [_i] * 6 + [_u, _vp]),
     "cca_b200_attention_backward3d": (_i, [_vp] * 7 + [_sz] + [_i] * 6 + [_u, _vp]),
+    "cca_b200_forward3d_window": (_i, [_vp] * 6 + [_sz] + [_i] * 8 + [_u, _vp]),
+    "cca_b200_backward3d_window": (_i, [_vp] * 10 + [_sz] + [_i] * 8 + [_u, _vp]),
+    "cca_b200_attention_forward3d_window": (_i, [_vp] * 4 + [_sz] + [_i] * 7 + [_u, _vp]),
+    "cca_b200_attention_backward3d_window": (_i, [_vp] * 7 + [_sz] + [_i] * 7 + [_u, _vp]),
+    "cca_b200_forward3d_step_ring": (_i, [_vp] * 8 + [_sz] + [_i] * 9 + [_u, _vp]),
     "cca_b200_forward_host": (_i, [_vp] * 5 + [_i] * 6 + [_u]),
     "cca_b200_backward_host": (_i, [_vp] * 9 + [_i] * 6 + [_u]),
 }

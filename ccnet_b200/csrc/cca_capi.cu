@@ -364,11 +364,19 @@ int cca_b200_attention_backward(const float *dattn, const float *attn, const voi
 // criss-cross attention over clips (the 3D op): tensor-core path (cca_tc_time.cu) or generic kernels (cca_simt_3d.cu)
 // ---------------------------------------------------------------------------------------
 namespace {
+constexpr const char *kSimt3dKeysMsg = "H + W - 1 + time keys (T - 1, or the window) above 2048 for the generic 3D kernels%s%s";
 int check_dims3d(int B, int Cq, int C, int T, int H, int W, int dtype)
 {
     if (T <= 0) return fail(CCA_ERR_INVALID, "non-positive dimension%s%s");
     if ((long long)B * T >= (1ll << 31)) return fail(CCA_ERR_UNSUPPORTED, "tensor too large%s%s");
     return check_dims(B * T, Cq, C, H, W, dtype);
+}
+// a time window (window > 0) is a causal-mode parameter
+int check_window(int window, unsigned flags)
+{
+    if (window < 0) return fail(CCA_ERR_INVALID, "negative time window%s%s");
+    if (window > 0 && !(flags & CCA_FLAG_CAUSAL)) return fail(CCA_ERR_INVALID, "a time window needs CCA_FLAG_CAUSAL%s%s");
+    return CCA_OK;
 }
 bool det3d_planes(Dims3 d, int dtype, unsigned flags)
 {
@@ -397,18 +405,24 @@ size_t cca_b200_workspace_bytes3d(int which, int B, int Cq, int C, int T, int H,
 int cca_b200_forward3d(const void *q, const void *k, const void *v, void *out, float *lse, void *ws, size_t ws_bytes,
                        int B, int Cq, int C, int T, int H, int W, int dtype, unsigned flags, void *stream)
 {
+    return cca_b200_forward3d_window(q, k, v, out, lse, ws, ws_bytes, B, Cq, C, T, H, W, 0, dtype, flags, stream);
+}
+
+int cca_b200_forward3d_window(const void *q, const void *k, const void *v, void *out, float *lse, void *ws, size_t ws_bytes,
+                              int B, int Cq, int C, int T, int H, int W, int window, int dtype, unsigned flags, void *stream)
+{
     int rc = check_dims3d(B, Cq, C, T, H, W, dtype);
-    if (rc) return rc;
+    if (rc || (rc = check_window(window, flags))) return rc;
     if (!q || !k || !v || !out || !lse || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
     if (ws_bytes < cca_b200_workspace_bytes3d(CCA_WS_FORWARD, B, Cq, C, T, H, W, dtype, flags))
         return fail(CCA_ERR_WORKSPACE, "forward workspace too small%s%s");
-    const Dims3 d{B, Cq, C, T, H, W};
+    const Dims3 d{B, Cq, C, T, H, W, window};
     const int fam = kernel_family(flags, (flags & CCA_FLAG_NHWC) && tc3d_supported(d, dtype), det_16bit_tiled(flags, d.frames(), dtype),
                                   "3D op", "NCDHW");
     if (fam < 0) return fam;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (fam == 0) {
-        if (!simt3d_supported(d)) return fail(CCA_ERR_UNSUPPORTED, "H + W + T - 2 above 2048 for the generic 3D kernels%s%s");
+        if (!simt3d_supported(d)) return fail(CCA_ERR_UNSUPPORTED, kSimt3dKeysMsg);
         cudaError_t e = (flags & CCA_FLAG_CAUSAL) ? simt_forward3d_causal(q, k, v, out, lse, d, dtype, st)
                                                   : simt_forward3d(q, k, v, out, lse, d, dtype, st);
         return e != cudaSuccess ? cuda_fail(e, "simt_forward3d") : CCA_OK;
@@ -424,18 +438,25 @@ int cca_b200_backward3d(const void *dout, const void *q, const void *k, const vo
                         void *dq, void *dk, void *dv, void *ws, size_t ws_bytes, int B, int Cq, int C, int T, int H, int W,
                         int dtype, unsigned flags, void *stream)
 {
+    return cca_b200_backward3d_window(dout, q, k, v, out, lse, dq, dk, dv, ws, ws_bytes, B, Cq, C, T, H, W, 0, dtype, flags, stream);
+}
+
+int cca_b200_backward3d_window(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
+                               void *dq, void *dk, void *dv, void *ws, size_t ws_bytes, int B, int Cq, int C, int T, int H, int W,
+                               int window, int dtype, unsigned flags, void *stream)
+{
     int rc = check_dims3d(B, Cq, C, T, H, W, dtype);
-    if (rc) return rc;
+    if (rc || (rc = check_window(window, flags))) return rc;
     if (!dout || !q || !k || !v || !out || !lse || !dq || !dk || !dv || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
     if (ws_bytes < cca_b200_workspace_bytes3d(CCA_WS_BACKWARD, B, Cq, C, T, H, W, dtype, flags))
         return fail(CCA_ERR_WORKSPACE, "backward workspace too small%s%s");
-    const Dims3 d{B, Cq, C, T, H, W};
+    const Dims3 d{B, Cq, C, T, H, W, window};
     const int fam = kernel_family(flags, (flags & CCA_FLAG_NHWC) && tc3d_supported(d, dtype), det_16bit_tiled(flags, d.frames(), dtype),
                                   "3D op", "NCDHW");
     if (fam < 0) return fam;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (fam == 0) {
-        if (!simt3d_supported(d)) return fail(CCA_ERR_UNSUPPORTED, "H + W + T - 2 above 2048 for the generic 3D kernels%s%s");
+        if (!simt3d_supported(d)) return fail(CCA_ERR_UNSUPPORTED, kSimt3dKeysMsg);
         if (reinterpret_cast<uintptr_t>(ws) & 3) return fail(CCA_ERR_INVALID, "workspace must be 4-byte aligned%s%s");
         cudaError_t e = ((flags & CCA_FLAG_CAUSAL) ? simt_backward3d_causal : simt_backward3d)(dout, q, k, v, out, lse, dq, dk, dv, ws, d,
                                                                                              dtype, st);
@@ -463,10 +484,21 @@ int cca_b200_forward3d_step(const void *q, const void *k, const void *v, const v
                             void *ws, size_t ws_bytes, int B, int Cq, int C, int S, int H, int W, int dtype, unsigned flags,
                             void *stream)
 {
+    return cca_b200_forward3d_step_ring(q, k, v, k_cache, v_cache, out, lse, ws, ws_bytes, B, Cq, C, S, S, 0, H, W, dtype, flags, stream);
+}
+
+int cca_b200_forward3d_step_ring(const void *q, const void *k, const void *v, const void *k_ring, const void *v_ring, void *out,
+                                 float *lse, void *ws, size_t ws_bytes, int B, int Cq, int C, int N, int S, int head, int H, int W,
+                                 int dtype, unsigned flags, void *stream)
+{
     if (S < 0) return fail(CCA_ERR_INVALID, "negative number of cached frames%s%s");
+    if (S > N) return fail(CCA_ERR_INVALID, "more cached frames than ring slots%s%s");
+    if (N > 0 && (head < 0 || head >= N)) return fail(CCA_ERR_INVALID, "ring head outside [0, N)%s%s");
     int rc = check_dims3d(B, Cq, C, S + 1, H, W, dtype);
     if (rc) return rc;
-    if (!q || !k || !v || !out || !lse || !ws || (S > 0 && (!k_cache || !v_cache))) return fail(CCA_ERR_INVALID, "null pointer%s%s");
+    if ((long long)N * H * W >= (1ll << 31) || (long long)B * N * H * W * (Cq > C ? Cq : C) >= (1ll << 40))
+        return fail(CCA_ERR_UNSUPPORTED, "tensor too large%s%s");           // (the rings)
+    if (!q || !k || !v || !out || !lse || !ws || (S > 0 && (!k_ring || !v_ring))) return fail(CCA_ERR_INVALID, "null pointer%s%s");
     if (ws_bytes < cca_b200_workspace_bytes3d_step(B, Cq, C, S, H, W, dtype, flags))
         return fail(CCA_ERR_WORKSPACE, "step workspace too small%s%s");
     const Dims3 d3{B, Cq, C, S + 1, H, W};
@@ -478,13 +510,13 @@ int cca_b200_forward3d_step(const void *q, const void *k, const void *v, const v
     if (fam == 0) {
         if ((long)H + W + S - 1 > kMaxKeys3d || !simt3d_supported(d3))
             return fail(CCA_ERR_UNSUPPORTED, "H + W + S - 1 above 2048 for the generic step kernel%s%s");
-        cudaError_t e = simt_forward3d_step(q, k, v, k_cache, v_cache, out, lse, d, S, dtype, st);
+        cudaError_t e = simt_forward3d_step(q, k, v, k_ring, v_ring, out, lse, d, N, S, head, dtype, st);
         return e != cudaSuccess ? cuda_fail(e, "simt_forward3d_step") : CCA_OK;
     }
-    if (!aligned16({q, k, v, out, ws}) || (S > 0 && !aligned16({k_cache, v_cache}))) return fail(CCA_ERR_INVALID, kAlignMsg);
+    if (!aligned16({q, k, v, out, ws}) || (S > 0 && !aligned16({k_ring, v_ring}))) return fail(CCA_ERR_INVALID, kAlignMsg);
     const char *why = "";
     const bool det = (flags & CCA_FLAG_DETERMINISTIC) && tc_tiled(d);
-    cudaError_t e = tc_forward3d_step(q, k, v, k_cache, v_cache, out, lse, ws, d, S, dtype, st, &why, det);
+    cudaError_t e = tc_forward3d_step(q, k, v, k_ring, v_ring, out, lse, ws, d, N, S, head, dtype, st, &why, det);
     return e != cudaSuccess ? cuda_fail(e, why && *why ? why : "tc_forward3d_step") : CCA_OK;
 }
 
@@ -520,13 +552,19 @@ size_t cca_b200_attention_workspace_bytes3d(int backward, int B, int Cq, int T, 
 int cca_b200_attention_forward3d(const void *q, const void *k, float *attn, void *ws, size_t ws_bytes, int B, int Cq, int T, int H,
                                  int W, int dtype, unsigned flags, void *stream)
 {
+    return cca_b200_attention_forward3d_window(q, k, attn, ws, ws_bytes, B, Cq, T, H, W, 0, dtype, flags, stream);
+}
+
+int cca_b200_attention_forward3d_window(const void *q, const void *k, float *attn, void *ws, size_t ws_bytes, int B, int Cq, int T,
+                                        int H, int W, int window, int dtype, unsigned flags, void *stream)
+{
     int rc = check_attention_dims3d(B, Cq, T, H, W, dtype);
-    if (rc) return rc;
+    if (rc || (rc = check_window(window, flags))) return rc;
     if (!q || !k || !attn || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
     if (reinterpret_cast<uintptr_t>(attn) & 3) return fail(CCA_ERR_INVALID, "attn must be 4-byte aligned%s%s");
     if (ws_bytes < cca_b200_attention_workspace_bytes3d(0, B, Cq, T, H, W, dtype, flags))
         return fail(CCA_ERR_WORKSPACE, "attention map workspace too small%s%s");
-    const Dims3 d{B, Cq, 0, T, H, W};
+    const Dims3 d{B, Cq, 0, T, H, W, window};
     // (the forward writes every map element once: deterministic in every mode)
     const int fam = kernel_family(flags, (flags & CCA_FLAG_NHWC) && tc3d_attention_supported(d, dtype), false, "3D attention map",
                                   "NCDHW");
@@ -546,14 +584,21 @@ int cca_b200_attention_forward3d(const void *q, const void *k, float *attn, void
 int cca_b200_attention_backward3d(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk, void *ws,
                                   size_t ws_bytes, int B, int Cq, int T, int H, int W, int dtype, unsigned flags, void *stream)
 {
+    return cca_b200_attention_backward3d_window(dattn, attn, q, k, dq, dk, ws, ws_bytes, B, Cq, T, H, W, 0, dtype, flags, stream);
+}
+
+int cca_b200_attention_backward3d_window(const float *dattn, const float *attn, const void *q, const void *k, void *dq, void *dk,
+                                         void *ws, size_t ws_bytes, int B, int Cq, int T, int H, int W, int window, int dtype,
+                                         unsigned flags, void *stream)
+{
     int rc = check_attention_dims3d(B, Cq, T, H, W, dtype);
-    if (rc) return rc;
+    if (rc || (rc = check_window(window, flags))) return rc;
     if (!dattn || !attn || !q || !k || !dq || !dk || !ws) return fail(CCA_ERR_INVALID, "null pointer%s%s");
     if ((reinterpret_cast<uintptr_t>(attn) | reinterpret_cast<uintptr_t>(dattn)) & 3)
         return fail(CCA_ERR_INVALID, "attn and dattn must be 4-byte aligned%s%s");
     if (ws_bytes < cca_b200_attention_workspace_bytes3d(1, B, Cq, T, H, W, dtype, flags))
         return fail(CCA_ERR_WORKSPACE, "attention map backward workspace too small%s%s");
-    const Dims3 d{B, Cq, 0, T, H, W};
+    const Dims3 d{B, Cq, 0, T, H, W, window};
     const int fam = kernel_family(flags, (flags & CCA_FLAG_NHWC) && tc3d_attention_supported(d, dtype),
                                   det_16bit_tiled(flags, d.frames(), dtype), "3D attention map", "NCDHW");
     if (fam < 0) return fam;

@@ -12,10 +12,14 @@ namespace cca {
 struct Dims {
     int B, Cq, C, H, W;
 };
-// a batch of clips [B, C, T, H, W] (the 3D op, cca_tc_time.cu); frames(): the [B*T, C, H, W] view of its frames
+// a batch of clips [B, C, T, H, W] (the 3D op, cca_tc_time.cu); frames(): the [B*T, C, H, W] view of its frames.  window:
+// causal mode's time window (frame t sees the frames t - window .. t - 1; 0: every past frame)
 struct Dims3 {
     int B, Cq, C, T, H, W;
+    int window;
     Dims frames() const { return Dims{B * T, Cq, C, H, W}; }
+    // the most time keys a query frame has: T - 1, or a shorter window
+    __host__ __device__ int time_keys() const { return window > 0 && window < T - 1 ? window : T - 1; }
 };
 
 // A "line" is one image row (row branch) or one image column (column branch) of a sample.
@@ -115,8 +119,8 @@ size_t tc_forward3d_workspace(Dims3 d);
 size_t tc_backward3d_workspace(Dims3 d);
 cudaError_t tc_forward3d(const void *q, const void *k, const void *v, void *out, float *lse, void *ws, Dims3 d, int dtype,
                          cudaStream_t st, const char **why, bool det);
-//   generic kernels, NCDHW tensors of any Cq and C (cca_simt_3d.cu): one warp per pixel, its H + W + T - 2 keys in shared
-//   memory, so H + W + T - 2 <= kMaxKeys3d; the backward's workspace is delta [B*T*H*W]
+//   generic kernels, NCDHW tensors of any Cq and C (cca_simt_3d.cu): one warp per pixel, its H + W - 1 + d.time_keys() keys
+//   (H + W + T - 2 without a window) in shared memory, so that many <= kMaxKeys3d; the backward's workspace is delta [B*T*H*W]
 constexpr int kMaxKeys3d = 2048;
 bool simt3d_supported(Dims3 d);
 size_t simt3d_workspace(int which, Dims3 d);
@@ -125,25 +129,25 @@ cudaError_t simt_backward3d(const void *dout, const void *q, const void *k, cons
                             void *dq, void *dk, void *dv, void *ws, Dims3 d, int dtype, cudaStream_t st);
 cudaError_t tc_backward3d(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
                           void *dq, void *dk, void *dv, void *ws, Dims3 d, int dtype, cudaStream_t st, const char **why, bool det);
-//   causal mode (CCA_FLAG_CAUSAL: the time keys of frame t are the frames s < t; cca_tc_causal.cu): the same passes and
-//   workspaces with the causal time kernels, and the streaming step: frame S of the causal forward from the new frame's q, k, v
-//   [B,H,W,c] and the caches kc [B,S,H,W,Cq], vc [B,S,H,W,C] (S <= kTimeMaxT - 1; workspace: tc_forward3d_workspace of
-//   Dims3{B, Cq, C, 1, H, W})
+//   causal mode (CCA_FLAG_CAUSAL: the time keys of frame t are the frames t - d.window <= s < t, every s < t at window 0;
+//   cca_tc_causal.cu): the same passes and workspaces with the causal time kernels, and the streaming step: frame S of the
+//   causal forward from the new frame's q, k, v [B,H,W,c] and rings kc [B,N,H,W,Cq], vc [B,N,H,W,C] holding the S past
+//   frames, frame j in slot (head + j) % N (S <= kTimeMaxT - 1; workspace: tc_forward3d_workspace of Dims3{B, Cq, C, 1, H, W})
 cudaError_t tc_forward3d_causal(const void *q, const void *k, const void *v, void *out, float *lse, void *ws, Dims3 d, int dtype,
                                 cudaStream_t st, const char **why, bool det);
 cudaError_t tc_backward3d_causal(const void *dout, const void *q, const void *k, const void *v, const void *out, const float *lse,
                                  void *dq, void *dk, void *dv, void *ws, Dims3 d, int dtype, cudaStream_t st, const char **why,
                                  bool det);
 cudaError_t tc_forward3d_step(const void *q, const void *k, const void *v, const void *kc, const void *vc, void *out, float *lse,
-                              void *ws, Dims d, int S, int dtype, cudaStream_t st, const char **why, bool det);
+                              void *ws, Dims d, int N, int S, int head, int dtype, cudaStream_t st, const char **why, bool det);
 //   generic kernels of causal mode (cca_simt_causal.cu), NCDHW tensors: the forward and backward (same limits and workspace as
-//   simt_forward3d / simt_backward3d) and the step on NCHW q, k, v and NCDHW caches (H + W + S - 1 <= kMaxKeys3d)
+//   simt_forward3d / simt_backward3d) and the step on NCHW q, k, v and NCDHW rings (H + W + S - 1 <= kMaxKeys3d)
 cudaError_t simt_forward3d_causal(const void *q, const void *k, const void *v, void *out, float *lse, Dims3 d, int dtype,
                                   cudaStream_t st);
 cudaError_t simt_backward3d_causal(const void *dout, const void *q, const void *k, const void *v, const void *out,
                                    const float *lse, void *dq, void *dk, void *dv, void *ws, Dims3 d, int dtype, cudaStream_t st);
 cudaError_t simt_forward3d_step(const void *q, const void *k, const void *v, const void *kc, const void *vc, void *out, float *lse,
-                                Dims d, int S, int dtype, cudaStream_t st);
+                                Dims d, int N, int S, int head, int dtype, cudaStream_t st);
 
 // the attention map attn[B,H,W,H+W] (fp32) and its gradient w.r.t. q, k (Dims.C is not used)
 //   generic kernels, NCHW q, k (cca_simt_attn.cu); the backward's workspace is rho [B*H*W]

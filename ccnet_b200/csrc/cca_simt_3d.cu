@@ -197,7 +197,7 @@ cudaError_t bwd3(const void *dout, const void *q, const void *k, const void *v, 
 
 bool simt3d_supported(Dims3 d)
 {
-    const long le = (long)d.H + d.W + d.T - 2;
+    const long le = (long)d.H + d.W - 1 + d.time_keys();      // (H + W + T - 2 without a window)
     return le >= 1 && le <= kMaxKeys3d && (long)d.T * d.H * d.W < (1L << 31);
 }
 

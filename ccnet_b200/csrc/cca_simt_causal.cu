@@ -1,12 +1,13 @@
 // Generic CUDA-core kernels of causal criss-cross attention over clips (CCA_FLAG_CAUSAL), NCDHW tensors of any Cq and C: the
-// key set of pixel (b,t,h,w) is its column (self masked), its row and the time keys (b,s,h,w) with s < t, so
-// Le = H + W - 1 + t varies per pixel.  The kernels follow the bidirectional ones of cca_simt_3d.cu and cca_simt_attn3d.cu
+// key set of pixel (b,t,h,w) is its column (self masked), its row and the time keys (b,s,h,w) with lo(t) <= s < t, where
+// lo(t) = max(0, t - window) (0 without a window), so Le = H + W - 1 + t - lo(t) varies per pixel.  The kernels follow the bidirectional ones of cca_simt_3d.cu and cca_simt_attn3d.cu
 // (same warp layout, sums in the same order), which keep their own code.  The key set is no longer symmetric: the backward
 // and the map backward gather dk and dv of a key pixel of frame t from the time queries u > t (the transposed time set) and,
 // as before, from the column and row queries.  Nothing is added atomically: the results are deterministic.
 //
 // The streaming step (simt_forward3d_step): one warp per pixel of the new frame over its column (self masked), its row and
-// the S cached time keys, in that order, with the arithmetic of the causal forward's last frame.
+// the S past frames of the rings (frame j in slot (head + j) % N), in that order, with the arithmetic of the causal forward's
+// last frame.
 #include "cca_common.cuh"
 
 namespace cca {
@@ -29,36 +30,41 @@ __device__ __forceinline__ Pix pix_of(long p, const Dims3 &d, long vol, long hw)
     x.h = (int)(r / d.W); x.w = (int)(r - (long)x.h * d.W);
     return x;
 }
-// volume offset of entry i of pixel x's walk: column (g != h), row, then the time entries -- with `causal` the frames s < t
-// (the forward's key set, Le = H + W - 1 + t), else every other frame s != t (the backward's walk)
-__device__ __forceinline__ int key_off(int i, const Pix &x, const Dims3 &d, bool causal)
+// first time key of frame t: max(0, t - window)
+__device__ __forceinline__ int time_lo(int t, const Dims3 &d) { return t - min(t, d.time_keys()); }
+// the longest walk of the backward: column and row, and up to d.time_keys() frames on each side of t
+__host__ __device__ inline int bwd_walk(const Dims3 &d) { return d.H + d.W - 1 + min(d.T - 1, 2 * d.time_keys()); }
+
+// volume offset of entry i of pixel x's walk: column (g != h), row, then the time entries from frame lo on -- with `causal`
+// the frames lo <= s < t (the forward's key set), else the frames s != t from lo on (the backward's walk)
+__device__ __forceinline__ int key_off(int i, const Pix &x, const Dims3 &d, int lo, bool causal)
 {
     if (i < d.H - 1) return (x.t * d.H + (i < x.h ? i : i + 1)) * d.W + x.w;
     i -= d.H - 1;
     if (i < d.W) return (x.t * d.H + x.h) * d.W + i;
-    i -= d.W;
+    i += lo - d.W;
     return ((causal || i < x.t ? i : i + 1) * d.H + x.h) * d.W + x.w;
 }
 
-// out = sum_j P_j v_j, lse = log sum_j exp(q . k_j) over the H + W - 1 + t keys of frame t (shared memory laid out for the
-// longest set, t = T - 1)
+// out = sum_j P_j v_j, lse = log sum_j exp(q . k_j) over the H + W - 1 + t - lo(t) keys of frame t (shared memory laid out
+// for the longest set, H + W - 1 + d.time_keys())
 template <typename E>
 __global__ void __launch_bounds__(kThreads3) cca_simt3d_causal_fwd_kernel(const E *__restrict__ q, const E *__restrict__ k,
                                                                            const E *__restrict__ v, E *__restrict__ out,
                                                                            float *__restrict__ lse, Dims3 d)
 {
     extern __shared__ float sm3[];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, Lmax = d.H + d.W + d.T - 2;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, Lmax = d.H + d.W - 1 + d.time_keys();
     float *row = sm3 + (long)warp * 2 * Lmax;
     int *offs = reinterpret_cast<int *>(row + Lmax);
     const long hw = (long)d.H * d.W, vol = hw * d.T, npix = vol * d.B;
     for (long p = (long)blockIdx.x * kWarps3 + warp; p < npix; p += (long)gridDim.x * kWarps3) {
         const Pix x = pix_of(p, d, vol, hw);
-        const int Le = d.H + d.W - 1 + x.t;
+        const int lo = time_lo(x.t, d), Le = d.H + d.W - 1 + x.t - lo;
         const E *qp = q + x.b * d.Cq * vol + x.off, *kb = k + x.b * d.Cq * vol;
         float m = -INFINITY;
         for (int i = lane; i < Le; i += 32) {
-            const int o = key_off(i, x, d, true);
+            const int o = key_off(i, x, d, lo, true);
             float e = 0.f;
             for (int c = 0; c < d.Cq; ++c) e = fmaf(ldg_f(qp + c * vol), ldg_f(kb + c * vol + o), e);
             row[i] = e; offs[i] = o;
@@ -107,9 +113,11 @@ __global__ void __launch_bounds__(kThreads3) cca_simt3d_delta_kernel(const E *__
 
 // Pixel p as a query: dq_p = sum_n dS_pn k_n.  As a key: dk_p = sum_n dS_np q_n, dv_p = sum_n P_np dout_n over the queries n
 // that see p.  dS_uj = P_uj (dout_u . v_j - delta_u), P_uj = exp(q_u . k_j - lse_u).  The column and row parts are symmetric,
-// as in the bidirectional kernel, but the time queries of p (frame t) are the frames u > t while its time keys are the
-// frames s < t: the walk covers every other frame of the line once, entry s < t weighing as a key of p (sq) and entry u > t
-// as a query (pk, sk), the other weights 0 -- the transposed set, gathered, not scattered.
+// as in the bidirectional kernel, but the time queries of p (frame t) are the frames t < u <= t + window while its time keys
+// are the frames t - window <= s < t: the walk covers those frames of the line once, in ascending order, entry s < t weighing
+// as a key of p (sq) and entry u > t as a query (pk, sk), the other weights 0 -- the transposed set, gathered, not
+// scattered.  The walk has up to H + W - 1 + 2 window entries: the time entries' offsets are recomputed instead of staged,
+// so that shared memory holds 3 floats per entry and an int per column and row entry.
 template <typename E>
 __global__ void __launch_bounds__(kThreads3) cca_simt3d_causal_bwd_kernel(const E *__restrict__ dout, const E *__restrict__ q,
                                                                            const E *__restrict__ k, const E *__restrict__ v,
@@ -118,19 +126,20 @@ __global__ void __launch_bounds__(kThreads3) cca_simt3d_causal_bwd_kernel(const 
                                                                            E *__restrict__ dk, E *__restrict__ dv, Dims3 d)
 {
     extern __shared__ float sm3[];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, Le = d.H + d.W + d.T - 2;
-    float *sq = sm3 + (long)warp * 4 * Le, *pk = sq + Le, *sk = pk + Le;
-    int *offs = reinterpret_cast<int *>(sk + Le);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n2 = d.H + d.W - 1, Lmax = bwd_walk(d);
+    float *sq = sm3 + (long)warp * (3 * Lmax + n2), *pk = sq + Lmax, *sk = pk + Lmax;
+    int *offs = reinterpret_cast<int *>(sk + Lmax);
     const long hw = (long)d.H * d.W, vol = hw * d.T, npix = vol * d.B;
     for (long p = (long)blockIdx.x * kWarps3 + warp; p < npix; p += (long)gridDim.x * kWarps3) {
         const Pix x = pix_of(p, d, vol, hw);
+        const int lo = time_lo(x.t, d), nk = x.t - lo, Le = n2 + nk + min(d.T - 1 - x.t, d.time_keys());
         const long sq0 = x.b * d.Cq * vol, sv0 = x.b * d.C * vol, s0 = x.b * vol;
         const E *qb = q + sq0, *kb = k + sq0, *vb = v + sv0, *gb = dout + sv0;
         const float lse_p = lse[p], delta_p = delta[p];
         for (int i = lane; i < Le; i += 32) {
-            const int o = key_off(i, x, d, false);
-            const bool key = i < d.H + d.W - 1 + x.t;                     // o is a key of p
-            const bool query = i < d.H + d.W - 1 || !key;                 // p is a key of o
+            const int o = key_off(i, x, d, lo, false);
+            const bool key = i < n2 + nk;                                 // o is a key of p
+            const bool query = i < n2 || !key;                            // p is a key of o
             float e1 = 0.f, e2 = 0.f, g1 = 0.f, g2 = 0.f;
             for (int c = 0; c < d.Cq; ++c) {
                 e1 = fmaf(ldg_f(qb + c * vol + x.off), ldg_f(kb + c * vol + o), e1);
@@ -144,15 +153,22 @@ __global__ void __launch_bounds__(kThreads3) cca_simt3d_causal_bwd_kernel(const 
             sq[i] = key ? p1 * (g1 - delta_p) : 0.f;
             pk[i] = query ? p2 : 0.f;
             sk[i] = query ? p2 * (g2 - delta[s0 + o]) : 0.f;
-            offs[i] = o;
+            if (i < n2) offs[i] = o;
         }
         __syncwarp();
+        // the time entries from n2 on: frames lo, lo + 1, ... skipping t, at offset s * hw + (the pixel's offset in its frame)
+        const int t0 = (int)(x.off - x.t * hw), tskip = n2 + nk;
         for (int c = lane; c < d.Cq; c += 32) {
             const E *kc = kb + c * vol, *qc = qb + c * vol;
             float a = 0.f, b = 0.f;
-            for (int i = 0; i < Le; ++i) {
+            for (int i = 0; i < n2; ++i) {
                 a = fmaf(sq[i], ldg_f(kc + offs[i]), a);
                 b = fmaf(sk[i], ldg_f(qc + offs[i]), b);
+            }
+            for (int i = n2, o = lo * (int)hw + t0; i < Le; ++i, o += (int)hw) {
+                if (i == tskip) o += (int)hw;
+                a = fmaf(sq[i], ldg_f(kc + o), a);
+                b = fmaf(sk[i], ldg_f(qc + o), b);
             }
             dq[sq0 + c * vol + x.off] = from_f<E>(a);
             dk[sq0 + c * vol + x.off] = from_f<E>(b);
@@ -160,7 +176,11 @@ __global__ void __launch_bounds__(kThreads3) cca_simt3d_causal_bwd_kernel(const 
         for (int c = lane; c < d.C; c += 32) {
             const E *gc = gb + c * vol;
             float a = 0.f;
-            for (int i = 0; i < Le; ++i) a = fmaf(pk[i], ldg_f(gc + offs[i]), a);
+            for (int i = 0; i < n2; ++i) a = fmaf(pk[i], ldg_f(gc + offs[i]), a);
+            for (int i = n2, o = lo * (int)hw + t0; i < Le; ++i, o += (int)hw) {
+                if (i == tskip) o += (int)hw;
+                a = fmaf(pk[i], ldg_f(gc + o), a);
+            }
             dv[sv0 + c * vol + x.off] = from_f<E>(a);
         }
         __syncwarp();
@@ -171,14 +191,14 @@ __global__ void __launch_bounds__(kThreads3) cca_simt3d_causal_bwd_kernel(const 
 constexpr int kMapThreads = 256;
 constexpr int kMapWarps = kMapThreads / 32;
 
-// volume offset of key g of pixel x, -1 for the masked entries (the column's self entry; time entries g >= t)
-__device__ __forceinline__ long key_of(int g, const Pix &x, const Dims3 &d, long hw)
+// volume offset of key g of pixel x, -1 for the masked entries (the column's self entry; time entries outside [lo, t))
+__device__ __forceinline__ long key_of(int g, const Pix &x, const Dims3 &d, long hw, int lo)
 {
     if (g < d.H) return g == x.h ? -1 : x.t * hw + (long)g * d.W + x.w;
     g -= d.H;
     if (g < d.W) return x.t * hw + (long)x.h * d.W + g;
     g -= d.W;
-    return g >= x.t ? -1 : g * hw + (long)x.h * d.W + x.w;
+    return g >= x.t || g < lo ? -1 : g * hw + (long)x.h * d.W + x.w;
 }
 
 // logits into the row, then max, log-sum-exp2 and the normalised row in place (each lane rereads only what it wrote)
@@ -190,11 +210,12 @@ __global__ void __launch_bounds__(kMapThreads) cca_attn3d_causal_map_kernel(cons
     const int lane = threadIdx.x & 31;
     for (long p = (long)blockIdx.x * kMapWarps + (threadIdx.x >> 5); p < npix; p += (long)gridDim.x * kMapWarps) {
         const Pix x = pix_of(p, d, vol, hw);
+        const int lo = time_lo(x.t, d);
         const E *qp = q + x.b * d.Cq * vol + x.off, *kb = k + x.b * d.Cq * vol;
         float *row = attn + p * rl;
         float m = -INFINITY;
         for (int g = lane; g < rl; g += 32) {
-            const long o = key_of(g, x, d, hw);
+            const long o = key_of(g, x, d, hw, lo);
             float e = -INFINITY;
             if (o >= 0) {
                 e = 0.f;
@@ -211,7 +232,8 @@ __global__ void __launch_bounds__(kMapThreads) cca_attn3d_causal_map_kernel(cons
     }
 }
 
-// dq[b,c,t,h,w] = sum_g dS[p,g] k[b,c,key g]; lanes own channels, the keys are walked in order
+// dq[b,c,t,h,w] = sum_g dS[p,g] k[b,c,key g]; lanes own channels, the keys are walked in order (the time entries from lo(t)
+// to t - 1 only: the others are masked)
 template <typename E>
 __global__ void __launch_bounds__(kMapThreads) cca_attn3d_causal_dq_kernel(const float *__restrict__ dattn, const float *__restrict__ attn,
                                                                           const float *__restrict__ rho, const E *__restrict__ k,
@@ -221,14 +243,15 @@ __global__ void __launch_bounds__(kMapThreads) cca_attn3d_causal_dq_kernel(const
     const int lane = threadIdx.x & 31;
     for (long p = (long)blockIdx.x * kMapWarps + (threadIdx.x >> 5); p < npix; p += (long)gridDim.x * kMapWarps) {
         const Pix x = pix_of(p, d, vol, hw);
+        const int lo = time_lo(x.t, d), n2 = d.H + d.W, gend = n2 + x.t;
         const float *a = attn + p * rl, *da = dattn + p * rl;
         const float r = rho[p];
         for (int c0 = 0; c0 < d.Cq; c0 += 32) {
             const int c = c0 + lane;
             const E *kc = k + (x.b * d.Cq + (c < d.Cq ? c : 0)) * vol;
             float acc = 0.f;
-            for (int g = 0; g < rl; ++g) {
-                const long o = key_of(g, x, d, hw);
+            for (int g = 0; g < gend; g = g == n2 - 1 ? n2 + lo : g + 1) {
+                const long o = key_of(g, x, d, hw, lo);
                 if (o < 0) continue;                                   // the masked entries do not depend on q, k
                 acc = fmaf(__ldg(a + g) * (__ldg(da + g) - r), ldg_f(kc + o), acc);
             }
@@ -238,7 +261,8 @@ __global__ void __launch_bounds__(kMapThreads) cca_attn3d_causal_dq_kernel(const
 }
 
 // dk of key pixel (t,y,x) = sum over the queries whose row holds it -- column queries (t,i,x), i != y (entry y), row queries
-// (t,y,j) (entry H + x), time queries (s,y,x), s > t (the transposed time set) (entry H + W + t) -- of dS * q, in that order
+// (t,y,j) (entry H + x), time queries (s,y,x), t < s <= t + window (the transposed time set) (entry H + W + t) -- of dS * q,
+// in that order
 template <typename E>
 __global__ void __launch_bounds__(kMapThreads) cca_attn3d_causal_dk_kernel(const float *__restrict__ dattn, const float *__restrict__ attn,
                                                                           const float *__restrict__ rho, const E *__restrict__ q,
@@ -253,7 +277,8 @@ __global__ void __launch_bounds__(kMapThreads) cca_attn3d_causal_dk_kernel(const
             const int c = c0 + lane;
             const E *qc = q + (x.b * d.Cq + (c < d.Cq ? c : 0)) * vol;
             float acc = 0.f;
-            for (int i = 0; i < rl; ++i) {
+            const int n2 = d.H + d.W, iend = n2 + min(d.T - 1, x.t + d.time_keys()) + 1;
+            for (int i = 0; i < iend; i = i == n2 - 1 ? n2 + x.t + 1 : i + 1) {
                 long qo, g;                                            // query pixel (volume offset), its entry of this key
                 if (i < d.H) {
                     if (i == x.h) continue;
@@ -274,32 +299,37 @@ __global__ void __launch_bounds__(kMapThreads) cca_attn3d_causal_dk_kernel(const
 }
 
 // ---- the streaming step
-// q, k, v [B,c,H,W] of the new frame, kc [B,Cq,S,H,W], vc [B,C,S,H,W]: out [B,C,H,W], lse [B,H,W]
+// q, k, v [B,c,H,W] of the new frame, rings kc [B,Cq,N,H,W], vc [B,C,N,H,W] with past frame j < S in slot (head + j) % N:
+// out [B,C,H,W], lse [B,H,W]
 template <typename E>
 __global__ void __launch_bounds__(kThreads3) cca_simt3d_step_kernel(const E *__restrict__ q, const E *__restrict__ k,
                                                                      const E *__restrict__ v, const E *__restrict__ kc,
                                                                      const E *__restrict__ vc, E *__restrict__ out,
-                                                                     float *__restrict__ lse, Dims d, int S)
+                                                                     float *__restrict__ lse, Dims d, int N, int S, int head)
 {
     extern __shared__ float sm3[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n2 = d.H + d.W - 1, Le = n2 + S;
     float *row = sm3 + (long)warp * 2 * Le;
     int *offs = reinterpret_cast<int *>(row + Le);
-    const long hw = (long)d.H * d.W, cvol = hw * S, npix = hw * d.B;
+    const long hw = (long)d.H * d.W, cvol = hw * N, npix = hw * d.B;
     for (long p = (long)blockIdx.x * kWarps3 + warp; p < npix; p += (long)gridDim.x * kWarps3) {
         const long b = p / hw, off = p - b * hw;
         const int h = (int)(off / d.W), w = (int)(off - (long)h * d.W);
         const E *qp = q + b * d.Cq * hw + off, *kb = k + b * d.Cq * hw, *kcb = kc + b * d.Cq * cvol;
         float m = -INFINITY;
-        for (int i = lane; i < Le; i += 32) {
-            // column keys (g != h) and row keys of the frame, then cached frame i - n2 at (h, w)
-            const bool frame = i < n2;
-            const int o = i < d.H - 1 ? (i < h ? i : i + 1) * d.W + w : frame ? h * d.W + (i - d.H + 1) : (int)((i - n2) * hw + off);
-            const E *kk = frame ? kb : kcb;
-            const long cs = frame ? hw : cvol;
+        for (int i = lane; i < n2; i += 32) {          // column keys (g != h) and row keys of the frame
+            const int o = i < d.H - 1 ? (i < h ? i : i + 1) * d.W + w : h * d.W + (i - d.H + 1);
             float e = 0.f;
-            for (int c = 0; c < d.Cq; ++c) e = fmaf(ldg_f(qp + c * hw), ldg_f(kk + c * cs + o), e);
+            for (int c = 0; c < d.Cq; ++c) e = fmaf(ldg_f(qp + c * hw), ldg_f(kb + c * hw + o), e);
             row[i] = e; offs[i] = o;
+            m = fmaxf(m, e);
+        }
+        for (int j = lane; j < S; j += 32) {           // past frame j at (h, w), in its ring slot
+            const long ot = (j + head) * hw + off;
+            const int o = (int)(ot < cvol ? ot : ot - cvol);
+            float e = 0.f;
+            for (int c = 0; c < d.Cq; ++c) e = fmaf(ldg_f(qp + c * hw), ldg_f(kcb + c * cvol + o), e);
+            row[n2 + j] = e; offs[n2 + j] = o;
             m = fmaxf(m, e);
         }
         m = warp_max(m);
@@ -344,7 +374,7 @@ cudaError_t simt_forward3d_causal(const void *q, const void *k, const void *v, v
                                   cudaStream_t st)
 {
     const long npix = (long)d.B * d.T * d.H * d.W;
-    const size_t smem = (size_t)kWarps3 * 2 * (d.H + d.W + d.T - 2) * sizeof(float);
+    const size_t smem = (size_t)kWarps3 * 2 * (d.H + d.W - 1 + d.time_keys()) * sizeof(float);
     return with_elem(dtype, [&](auto e) {
         using E = decltype(e);
         return launch(cca_simt3d_causal_fwd_kernel<E>, npix, kWarps3, smem, st, (const E *)q, (const E *)k, (const E *)v, (E *)out,
@@ -356,7 +386,7 @@ cudaError_t simt_backward3d_causal(const void *dout, const void *q, const void *
                                    const float *lse, void *dq, void *dk, void *dv, void *ws, Dims3 d, int dtype, cudaStream_t st)
 {
     const long npix = (long)d.B * d.T * d.H * d.W;
-    const size_t smem = (size_t)kWarps3 * 4 * (d.H + d.W + d.T - 2) * sizeof(float);
+    const size_t smem = (size_t)kWarps3 * (3 * bwd_walk(d) + d.H + d.W - 1) * sizeof(float);
     float *delta = reinterpret_cast<float *>(ws);
     return with_elem(dtype, [&](auto e) {
         using E = decltype(e);
@@ -393,14 +423,14 @@ cudaError_t simt_attention_backward3d_causal(const float *dattn, const float *at
 }
 
 cudaError_t simt_forward3d_step(const void *q, const void *k, const void *v, const void *kc, const void *vc, void *out, float *lse,
-                                Dims d, int S, int dtype, cudaStream_t st)
+                                Dims d, int N, int S, int head, int dtype, cudaStream_t st)
 {
     const long npix = (long)d.B * d.H * d.W;
     const size_t smem = (size_t)kWarps3 * 2 * (d.H + d.W - 1 + S) * sizeof(float);
     return with_elem(dtype, [&](auto e) {
         using E = decltype(e);
         return launch(cca_simt3d_step_kernel<E>, npix, kWarps3, smem, st, (const E *)q, (const E *)k, (const E *)v, (const E *)kc,
-                      (const E *)vc, (E *)out, lse, d, S);
+                      (const E *)vc, (E *)out, lse, d, N, S, head);
     });
 }
 

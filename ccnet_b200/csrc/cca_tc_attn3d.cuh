@@ -53,7 +53,7 @@ template <int TM, typename E, bool Causal> __device__ __forceinline__ void time_
         float *row = p.attn + pix * p.row + p.off;
 #pragma unroll
         for (int j = 0; j < TM; ++j)
-            if (j < p.t.T) row[j] = (Causal ? j >= lane : j == lane) ? 0.f : exp2f(s[j] + nl2);   // (not a key of lane: 0)
+            if (j < p.t.T) row[j] = (Causal ? !time_key<true>(j, lane, p.t) : j == lane) ? 0.f : exp2f(s[j] + nl2);   // (not a key: 0)
     }
 }
 
@@ -73,7 +73,8 @@ template <int TM, typename E, bool Causal> __device__ __forceinline__ void time_
         const long pix = pix0 + lane * hw;
         const float rho = __ldcg(p.rho + pix);
         const float *a = p.map + pix * p.row + p.off, *d = p.dattn + pix * p.row + p.off;
-        for (int j = 0; j < T; ++j) ds[lane * lt + j] = (Causal ? j >= lane : j == lane) ? 0.f : __ldg(a + j) * (__ldg(d + j) - rho);
+        for (int j = 0; j < T; ++j)
+            ds[lane * lt + j] = (Causal ? !time_key<true>(j, lane, p.t) : j == lane) ? 0.f : __ldg(a + j) * (__ldg(d + j) - rho);
     }
     __syncwarp();
     // dq[t] += sum_s dS[t][s] k[s],  dk[s] += sum_t dS[t][s] q[t]   (lane = channel)

@@ -1,12 +1,13 @@
 // Causal criss-cross attention over clips on the tensor-core path (CCA_FLAG_CAUSAL): pixel (b, t, h, w) attends to its column
-// (self masked), its row and the time keys (b, s, h, w) with s < t only, one softmax over them.  Only the time kernels change:
-// they are the bodies of cca_tc_time.cuh and cca_tc_attn3d.cuh instantiated with Causal = true (logits of key frames j < t
-// where the bidirectional kernels take j != t), run in the same passes.  Frame 0 has no time key: its time plane is -inf, so
+// (self masked), its row and the time keys (b, s, h, w) with t - window <= s < t only, one softmax over them.  Only the time
+// kernels change: they are the bodies of cca_tc_time.cuh and cca_tc_attn3d.cuh instantiated with Causal = true (logits of key
+// frames t - window <= j < t where the bidirectional kernels take j != t; the window is a run-time field, T when unbounded,
+// so a window needs no kernels of its own), run in the same passes.  Frame 0 has no time key: its time plane is -inf, so
 // its row is the 2D op's row, as at T = 1.  The time backward owns a whole T-line in one warp, so dk and dv of key frame s
 // collect dS[t][s] from the query frames t > s only (P and dS are 0 elsewhere), with no other change.
 //
-// The streaming step (tc_forward3d_step): frame S of the causal clip forward, computed from the new frame's q, k, v and caches
-// of the S previous frames' k and v, without the past queries.  It composes the forward's passes on the new frame:
+// The streaming step (tc_forward3d_step): frame S of the causal clip forward, computed from the new frame's q, k, v and rings
+// of capacity N holding the S previous frames' k and v (frame j in slot (head + j) % N), without the past queries.  It composes the forward's passes on the new frame:
 //   2D statistics on the frame's NHWC view (B frames) -> time step statistics (query: the new frame; keys: the S cached frames
 //   at the same (h, w); no self entry) into one more lse plane -> 2D values with that plane (extra_parts = 1) -> time step
 //   values (out += P_T V_cache with the final lse)
@@ -81,14 +82,22 @@ cudaError_t launch_time_map(bool backward, const TimeMapParams &p, int dtype, cu
 // ---- the streaming step
 struct StepParams {
     const void *q;            // the new frame's q [B*H*W, Cq]
-    const void *kc, *vc;      // the caches [B, S, H, W, Cq], [B, S, H, W, C]
+    const void *kc, *vc;      // the rings [B, N, H, W, Cq], [B, N, H, W, C]: past frame j < S in slot (head + j) % N
     void *out;                // the new frame's out [B*H*W, C]
     float *part;              // stats: the time plane [B*H*W]
     const float *lse;         // values: the final natural-log lse [B*H*W]
     long lines;               // B*H*W: one warp per pixel of the new frame
     long hw;                  // H*W
     int S, Cq, C;
+    int N, head;
 };
+
+// slot of past frame j in the rings
+__device__ __forceinline__ long step_slot(const StepParams &p, int j)
+{
+    const int s = p.head + j;
+    return s < p.N ? s : s - p.N;
+}
 
 // floats of shared memory per warp: q [Cq+1], the cached keys K [S][Cq+1], one float per lane
 __host__ __device__ inline long step_floats(int S, int Cq) { return (long)(S + 1) * (Cq + 1) + 32; }
@@ -99,11 +108,13 @@ __host__ __device__ inline long step_floats(int S, int Cq) { return (long)(S + 1
 template <typename E> __device__ __forceinline__ float step_logit(const StepParams &p, long line, float *qs, float *ks, int lane)
 {
     const long b = line / p.hw, x = line - b * p.hw;
-    const E *q = static_cast<const E *>(p.q) + line * p.Cq, *k = static_cast<const E *>(p.kc) + (b * p.S * p.hw + x) * p.Cq;
+    const E *q = static_cast<const E *>(p.q) + line * p.Cq, *k = static_cast<const E *>(p.kc) + (b * p.N * p.hw + x) * p.Cq;
     const int ld = p.Cq + 1;
     for (int c = lane; c < p.Cq; c += 32) qs[c] = to_f(q[c]);
-    for (int j = 0; j < p.S; ++j)
-        for (int c = lane; c < p.Cq; c += 32) ks[j * ld + c] = to_f(k[j * p.hw * p.Cq + c]);
+    for (int j = 0; j < p.S; ++j) {
+        const E *kj = k + step_slot(p, j) * p.hw * p.Cq;
+        for (int c = lane; c < p.Cq; c += 32) ks[j * ld + c] = to_f(kj[c]);
+    }
     __syncwarp();
     float s = 0.f;
     if (lane < p.S)
@@ -150,11 +161,11 @@ __global__ void __launch_bounds__(32 * kWarps) cca_time_step_values_kernel(const
     if (lane < p.S) ps[lane] = exp2f(fmaf(s, kLog2e, nl2));
     __syncwarp();
     const long b = line / p.hw, x = line - b * p.hw, fs = p.hw * p.C;
-    const E *v = static_cast<const E *>(p.vc) + (b * p.S * p.hw + x) * p.C;
+    const E *v = static_cast<const E *>(p.vc) + (b * p.N * p.hw + x) * p.C;
     E *out = static_cast<E *>(p.out) + line * p.C;
     for (int c = lane; c < p.C; c += 32) {
         float a = 0.f;
-        for (int j = 0; j < p.S; ++j) a = fmaf(ps[j], to_f(v[j * fs + c]), a);
+        for (int j = 0; j < p.S; ++j) a = fmaf(ps[j], to_f(v[step_slot(p, j) * fs + c]), a);
         add_to(out + c, a);
     }
 }
@@ -209,7 +220,7 @@ cudaError_t tc_attention_backward3d_causal(const float *dattn, const float *attn
 
 // the step's workspace is the forward workspace of one frame (fwd_ws with the time plane; planes mode: tc_planes_bytes follow)
 cudaError_t tc_forward3d_step(const void *q, const void *k, const void *v, const void *kc, const void *vc, void *out, float *lse,
-                              void *ws, Dims d, int S, int dtype, cudaStream_t st, const char **why, bool det)
+                              void *ws, Dims d, int N, int S, int head, int dtype, cudaStream_t st, const char **why, bool det)
 {
     const FwdWs w = fwd_ws(d, 1, ws);
     cudaError_t e = tc_stats(q, k, w.parts, w.cdone, d.B, d, dtype, st, why);
@@ -220,6 +231,7 @@ cudaError_t tc_forward3d_step(const void *q, const void *k, const void *v, const
     p.hw = (long)d.H * d.W;
     p.part = w.parts + (long)make_space(d.B, d.H, d.W).nparts * p.lines;
     p.S = S; p.Cq = d.Cq; p.C = d.C;
+    p.N = N; p.head = head;
     if ((e = launch_step(true, p, dtype, st)) != cudaSuccess) return e;
     e = tc_values(q, k, v, out, lse, w.parts, w.cdone, w.planes, d, dtype, st, why, det, 1);
     if (e != cudaSuccess) return e;

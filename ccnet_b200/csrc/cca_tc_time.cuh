@@ -19,6 +19,8 @@ struct TimeParams {
     long lines;               // B*H*W
     long hw;                  // H*W
     int T, Cq, C;
+    int window;               // causal kernels: query frame t sees key frames t - window <= j < t (T: every j < t).  In the
+                              // tail padding, so that the bidirectional kernels' parameter layout (and TimeMapParams) is unchanged
 };
 
 // pixel of frame 0 of a T-line (b, hw); frame t is t * hw pixels further
@@ -76,13 +78,17 @@ inline TimeParams time_params(Dims3 d)
     p.lines = (long)d.B * d.H * d.W;
     p.hw = (long)d.H * d.W;
     p.T = d.T; p.Cq = d.Cq; p.C = d.C;
+    p.window = d.window > 0 ? d.window : d.T;
     return p;
 }
 
-// Key frame j of query frame t on a line of T frames: every other frame, or with Causal (CCA_FLAG_CAUSAL) the frames before t.
-// The kernel bodies below take Causal as a template parameter; the kernels of cca_tc_time.cu instantiate them with false, those
-// of cca_tc_causal.cu with true.
-template <bool Causal> __device__ __forceinline__ bool time_key(int j, int t, int T) { return Causal ? j < t : j < T && j != t; }
+// Key frame j of query frame t on a line of T frames: every other frame, or with Causal (CCA_FLAG_CAUSAL) the frames before t
+// inside the window.  The kernel bodies below take Causal as a template parameter; the kernels of cca_tc_time.cu instantiate
+// them with false, those of cca_tc_causal.cu with true.
+template <bool Causal> __device__ __forceinline__ bool time_key(int j, int t, const TimeParams &p)
+{
+    return Causal ? j < t && j >= t - p.window : j < p.T && j != t;
+}
 
 enum TimeKind { kStats = 0, kValues = 1, kBackward = 2 };
 
@@ -103,7 +109,7 @@ __device__ __forceinline__ void row_probs(const TimeParams &p, const float *qs, 
     const float nl2 = -__ldcg(p.lse + pix0 + t * p.hw) * kLog2e;
 #pragma unroll
     for (int j = 0; j < TM; ++j) {
-        pr[j] = time_key<Causal>(j, t, p.T) ? exp2f(s[j] + nl2) : 0.f;
+        pr[j] = time_key<Causal>(j, t, p) ? exp2f(s[j] + nl2) : 0.f;
         if (j < p.T) ps[t * (p.T + 1) + j] = pr[j];
     }
 }
@@ -127,12 +133,12 @@ template <int TM, typename E, bool Causal> __device__ __forceinline__ void time_
             float m = -INFINITY;
 #pragma unroll
             for (int j = 0; j < TM; ++j)
-                if (time_key<Causal>(j, lane, p.T)) m = fmaxf(m, s[j]);
+                if (time_key<Causal>(j, lane, p)) m = fmaxf(m, s[j]);
             if (m > -INFINITY) {
                 float sum = 0.f;
 #pragma unroll
                 for (int j = 0; j < TM; ++j)
-                    if (time_key<Causal>(j, lane, p.T)) sum += exp2f(s[j] - m);
+                    if (time_key<Causal>(j, lane, p)) sum += exp2f(s[j] - m);
                 l2 = m + log2f(sum);
             }
         }

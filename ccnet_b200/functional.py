@@ -84,6 +84,27 @@ def _plan(impl: str, det: bool, covered, q, v=None, causal: bool = False):
     return use_tc, flags, fmt
 
 
+def _time_window(causal: bool, window) -> int:
+    """The C ABI's window argument of a 3D call: 0 for ``window=None`` (every past frame), else W >= 1, causal mode only."""
+    if window is None:
+        return 0
+    if not causal:
+        raise ValueError("ccnet_b200: a time window needs causal=True (windows of the bidirectional op are not supported)")
+    if isinstance(window, bool) or int(window) != window or window < 1:
+        raise ValueError(f"ccnet_b200: window must be an integer >= 1 or None, got {window!r}")
+    return int(window)
+
+
+def _ws3d(which, B, Cq, C, T, H, W, window, dt, flags) -> int:
+    """cca_b200_workspace_bytes3d for the dimensions of a *_window call (the window does not change it)"""
+    return capi.load().cca_b200_workspace_bytes3d(which, B, Cq, C, T, H, W, dt, flags)
+
+
+def _attn_ws3d(backward, B, Cq, T, H, W, window, dt, flags) -> int:
+    """cca_b200_attention_workspace_bytes3d for the dimensions of a *_window call"""
+    return capi.load().cca_b200_attention_workspace_bytes3d(backward, B, Cq, T, H, W, dt, flags)
+
+
 def _upcast(dtype, H: int, W: int, deterministic: bool, T: int = 1) -> bool:
     """16-bit calls of the tensor-core path that run on the fp32 kernels on upcast tensors (bf16 and fp16 values are exact in
     the bf16x3 split), the result rounded to the 16-bit type ONCE:
@@ -403,7 +424,7 @@ def tc3d_eligible(B: int, Cq: int, C: int, T: int, H: int, W: int, dtype: torch.
 
 
 def cca3d_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", deterministic=None,
-                  causal: bool = False):
+                  causal: bool = False, window=None):
     """Criss-cross attention over clips: returns (out[B,C,T,H,W], lse[B,T,H,W] fp32).  q, k are [B,Cq,T,H,W], v [B,C,T,H,W].
     Pixel (b,t,h,w) attends to its column (self masked), its row and its time line (self masked), one softmax over the
     H + W + T logits.  At T = 1 this is ``cca_forward`` on every frame.
@@ -414,8 +435,14 @@ def cca3d_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str =
     NCDHW memory.  ``deterministic`` as for ``cca_forward``.
 
     ``causal``: the time keys of frame t are the frames s < t only (CCA_FLAG_CAUSAL); frame 0 then has no time key and is
-    ``cca_forward`` on its frame.  For streaming inference, ``cca3d_step`` produces one new frame from cached keys and values."""
+    ``cca_forward`` on its frame.  For streaming inference, ``cca3d_step`` produces one new frame from cached keys and values.
+
+    ``window`` (causal mode only; None: every past frame): W >= 1 limits the time keys of frame t to the frames
+    t - W <= s < t.  With W >= T - 1 the result is bit for bit that of ``window=None``.  The generic kernels then take
+    H + W_img - 1 + min(W, T - 1) <= 2048, so a windowed clip may have any length; ``cca3d_step`` on a ring of the last W
+    frames streams the same op."""
     _check_inputs(q, k, v, rank=5)
+    win = _time_window(causal, window)
     det = _resolve_deterministic(deterministic)
     lib = capi.load()
     B, Cq, T, H, W = q.shape
@@ -424,22 +451,23 @@ def cca3d_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str =
     use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc3d_supported(capi.CCA_WS_FORWARD, B, Cq, C, T, H, W, dt) == 1,
                                q, v, causal)
     if use_tc and _upcast(q.dtype, H, W, det, T):
-        out32, lse = cca3d_forward(q.float(), k.float(), v.float(), impl, det, causal)
+        out32, lse = cca3d_forward(q.float(), k.float(), v.float(), impl, det, causal, window)
         return out32.to(q.dtype), lse
     q, k, v = (t.contiguous(memory_format=fmt) for t in (q, k, v))
     with torch.cuda.device(q.device):
         out = torch.empty_like(v, memory_format=fmt)
         lse = torch.empty((B, T, H, W), dtype=torch.float32, device=q.device)
-        _grouped_call(lib.cca_b200_forward3d, lib.cca_b200_workspace_bytes3d, capi.CCA_WS_FORWARD, (q, k, v, out, lse),
-                      (Cq, C, T, H, W), dt, flags)
+        _grouped_call(lib.cca_b200_forward3d_window, _ws3d, capi.CCA_WS_FORWARD, (q, k, v, out, lse), (Cq, C, T, H, W, win), dt,
+                      flags)
     return out, lse
 
 
-def cca3d_backward(dout, q, k, v, out, lse, impl: str = "auto", deterministic=None, causal: bool = False):
+def cca3d_backward(dout, q, k, v, out, lse, impl: str = "auto", deterministic=None, causal: bool = False, window=None):
     """Gradients (dq, dk, dv) of ``cca3d_forward`` given dout and the saved forward tensors.  Same ``impl`` / memory-format /
-    ``deterministic`` / ``causal`` rules as ``cca3d_forward``."""
+    ``deterministic`` / ``causal`` / ``window`` rules as ``cca3d_forward``."""
     _check_inputs(q, k, v, rank=5)
     _check_saved(q, v, dout, out, lse)
+    win = _time_window(causal, window)
     det = _resolve_deterministic(deterministic)
     lib = capi.load()
     B, Cq, T, H, W = q.shape
@@ -448,7 +476,7 @@ def cca3d_backward(dout, q, k, v, out, lse, impl: str = "auto", deterministic=No
     use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc3d_supported(capi.CCA_WS_BACKWARD, B, Cq, C, T, H, W, dt) == 1,
                                q, v, causal)
     if use_tc and _upcast(q.dtype, H, W, det, T):
-        res = cca3d_backward(dout.float(), q.float(), k.float(), v.float(), out.float(), lse, impl, det, causal)
+        res = cca3d_backward(dout.float(), q.float(), k.float(), v.float(), out.float(), lse, impl, det, causal, window)
         return tuple(g.to(q.dtype) for g in res)
     dout, q, k, v, out = (t.contiguous(memory_format=fmt) for t in (dout, q, k, v, out))
     lse = lse.contiguous()
@@ -456,33 +484,35 @@ def cca3d_backward(dout, q, k, v, out, lse, impl: str = "auto", deterministic=No
         dq = torch.empty_like(q, memory_format=fmt)
         dk = torch.empty_like(k, memory_format=fmt)
         dv = torch.empty_like(v, memory_format=fmt)
-        _grouped_call(lib.cca_b200_backward3d, lib.cca_b200_workspace_bytes3d, capi.CCA_WS_BACKWARD,
-                      (dout, q, k, v, out, lse, dq, dk, dv), (Cq, C, T, H, W), dt, flags)
+        _grouped_call(lib.cca_b200_backward3d_window, _ws3d, capi.CCA_WS_BACKWARD, (dout, q, k, v, out, lse, dq, dk, dv),
+                      (Cq, C, T, H, W, win), dt, flags)
     return dq, dk, dv
 
 
 class _CCA3DFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, impl, deterministic, causal):
-        out, lse = cca3d_forward(q, k, v, impl, deterministic, causal)
+    def forward(ctx, q, k, v, impl, deterministic, causal, window):
+        out, lse = cca3d_forward(q, k, v, impl, deterministic, causal, window)
         ctx.save_for_backward(q, k, v, out, lse)
         ctx.impl = impl
         ctx.deterministic = deterministic
         ctx.causal = causal
+        ctx.window = window
         return out
 
     @staticmethod
     def backward(ctx, dout):
         q, k, v, out, lse = ctx.saved_tensors
-        dq, dk, dv = cca3d_backward(dout, q, k, v, out, lse, ctx.impl, ctx.deterministic, ctx.causal)
-        return dq, dk, dv, None, None, None
+        dq, dk, dv = cca3d_backward(dout, q, k, v, out, lse, ctx.impl, ctx.deterministic, ctx.causal, ctx.window)
+        return dq, dk, dv, None, None, None, None
 
 
 def cca3d(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", deterministic=None,
-          causal: bool = False) -> torch.Tensor:
-    """Differentiable criss-cross attention over clips (out only); see ``cca3d_forward``.  The ``causal`` mode of the forward
-    is kept for the backward."""
-    return _CCA3DFunction.apply(q, k, v, impl, _resolve_deterministic(deterministic), bool(causal))
+          causal: bool = False, window=None) -> torch.Tensor:
+    """Differentiable criss-cross attention over clips (out only); see ``cca3d_forward``.  The ``causal`` mode and
+    ``window`` of the forward are kept for the backward."""
+    _time_window(causal, window)
+    return _CCA3DFunction.apply(q, k, v, impl, _resolve_deterministic(deterministic), bool(causal), window)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -494,7 +524,7 @@ def attention3d_tc_eligible(B: int, Cq: int, T: int, H: int, W: int, dtype: torc
 
 
 def cca3d_attention_forward(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", deterministic=None,
-                            causal: bool = False) -> torch.Tensor:
+                            causal: bool = False, window=None) -> torch.Tensor:
     """The attention map of ``cca3d_forward``, attn[B,T,H,W,H+W+T] float32: attn[b,t,h,w,g] is the weight of column key
     (t, g, w) for g < H (0 at g == h), of row key (t, h, g - H) for H <= g < H + W and of time key (g - H - W, h, w) after
     that (0 at g - H - W == t).  It is normalised by the lse of ``cca3d_forward``; at T = 1, attn[..., :H+W] is
@@ -502,8 +532,10 @@ def cca3d_attention_forward(q: torch.Tensor, k: torch.Tensor, impl: str = "auto"
 
     ``impl`` as for ``cca3d_forward`` (the generic kernels take any Cq and shape).  Every map element is written once, so
     the result is the same in every mode; ``deterministic`` only sets the flag the C ABI is called with.  ``causal``: the map
-    of ``cca3d_forward(..., causal=True)``, same layout, time entries H + W + s with s >= t exactly 0."""
+    of ``cca3d_forward(..., causal=True)``, same layout, time entries H + W + s with s >= t exactly 0.  ``window``: that of
+    ``cca3d_forward(..., causal=True, window=W)``; time entries outside [t - W, t) are exactly 0."""
     _check_inputs(q, k, rank=5)
+    win = _time_window(causal, window)
     det = _resolve_deterministic(deterministic)
     lib = capi.load()
     B, Cq, T, H, W = q.shape
@@ -513,17 +545,18 @@ def cca3d_attention_forward(q: torch.Tensor, k: torch.Tensor, impl: str = "auto"
     with torch.cuda.device(q.device):
         attn = torch.empty((B, T, H, W, H + W + T), dtype=torch.float32, device=q.device)
         ws = _workspace(lib.cca_b200_attention_workspace_bytes3d(0, B, Cq, T, H, W, dt, flags), q.device)
-        rc = lib.cca_b200_attention_forward3d(q.data_ptr(), k.data_ptr(), attn.data_ptr(), ws.data_ptr(), ws.numel(),
-                                              B, Cq, T, H, W, dt, flags, _stream_ptr(q.device))
-        capi.check(rc, "cca_b200_attention_forward3d")
+        rc = lib.cca_b200_attention_forward3d_window(q.data_ptr(), k.data_ptr(), attn.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                     B, Cq, T, H, W, win, dt, flags, _stream_ptr(q.device))
+        capi.check(rc, "cca_b200_attention_forward3d_window")
     return attn
 
 
-def cca3d_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministic=None, causal: bool = False):
+def cca3d_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministic=None, causal: bool = False, window=None):
     """Gradients (dq, dk) of ``cca3d_attention_forward`` given dattn = dL/dattn and the forward's map, in the closed form
     of ``cca_attention_backward`` over the H + W + T entries of a row.  Same ``impl`` / memory-format / ``deterministic`` /
-    ``causal`` rules as ``cca3d_backward``."""
+    ``causal`` / ``window`` rules as ``cca3d_backward``."""
     _check_inputs(q, k, rank=5)
+    win = _time_window(causal, window)
     det = _resolve_deterministic(deterministic)
     lib = capi.load()
     B, Cq, T, H, W = q.shape
@@ -533,48 +566,50 @@ def cca3d_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministi
     dt = _DTYPES[q.dtype]
     use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_attention_tc3d_supported(B, Cq, T, H, W, dt) == 1, q, causal=causal)
     if use_tc and _upcast(q.dtype, H, W, det, T):
-        dq, dk = cca3d_attention_backward(dattn, attn, q.float(), k.float(), impl, det, causal)
+        dq, dk = cca3d_attention_backward(dattn, attn, q.float(), k.float(), impl, det, causal, window)
         return dq.to(q.dtype), dk.to(q.dtype)
     q, k = (t.contiguous(memory_format=fmt) for t in (q, k))
     dattn, attn = dattn.contiguous(), attn.contiguous()
     with torch.cuda.device(q.device):
         dq = torch.empty_like(q, memory_format=fmt)
         dk = torch.empty_like(k, memory_format=fmt)
-        _grouped_call(lib.cca_b200_attention_backward3d, lib.cca_b200_attention_workspace_bytes3d, 1,
-                      (dattn, attn, q, k, dq, dk), (Cq, T, H, W), dt, flags)
+        _grouped_call(lib.cca_b200_attention_backward3d_window, _attn_ws3d, 1, (dattn, attn, q, k, dq, dk), (Cq, T, H, W, win), dt,
+                      flags)
     return dq, dk
 
 
 class _CCA3DAttentionFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, impl, deterministic, causal):
-        attn = cca3d_attention_forward(q, k, impl, deterministic, causal)
+    def forward(ctx, q, k, impl, deterministic, causal, window):
+        attn = cca3d_attention_forward(q, k, impl, deterministic, causal, window)
         ctx.save_for_backward(q, k, attn)
         ctx.impl = impl
         ctx.deterministic = deterministic
         ctx.causal = causal
+        ctx.window = window
         return attn
 
     @staticmethod
     def backward(ctx, dattn):
         q, k, attn = ctx.saved_tensors
-        dq, dk = cca3d_attention_backward(dattn, attn, q, k, ctx.impl, ctx.deterministic, ctx.causal)
-        return dq, dk, None, None, None
+        dq, dk = cca3d_attention_backward(dattn, attn, q, k, ctx.impl, ctx.deterministic, ctx.causal, ctx.window)
+        return dq, dk, None, None, None, None
 
 
 def cca3d_attention(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", deterministic=None,
-                    causal: bool = False) -> torch.Tensor:
+                    causal: bool = False, window=None) -> torch.Tensor:
     """Differentiable attention map attn[B,T,H,W,H+W+T] (float32) of criss-cross attention over clips; the gradient flows
-    to q and k.  ``deterministic`` and ``causal``: as for ``cca3d``; the modes are fixed when the forward runs and the
-    backward uses them too."""
-    return _CCA3DAttentionFunction.apply(q, k, impl, _resolve_deterministic(deterministic), bool(causal))
+    to q and k.  ``deterministic``, ``causal`` and ``window``: as for ``cca3d``; they are fixed when the forward runs and
+    the backward uses them too."""
+    _time_window(causal, window)
+    return _CCA3DAttentionFunction.apply(q, k, impl, _resolve_deterministic(deterministic), bool(causal), window)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # streaming step of causal criss-cross attention over clips
 # ---------------------------------------------------------------------------------------------------------------------
 def cca3d_step(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor,
-               impl: str = "auto", deterministic=None):
+               impl: str = "auto", deterministic=None, frames=None, head: int = 0):
     """One new frame of causal criss-cross attention over clips, for streaming inference: returns (out[B,C,H,W],
     lse[B,H,W] fp32).  q, k [B,Cq,H,W] and v [B,C,H,W] are the new frame's; k_cache [B,Cq,S,H,W] and v_cache [B,C,S,H,W]
     the keys and values of the S previous frames in time order.  By definition the result is frame S of
@@ -583,7 +618,12 @@ def cca3d_step(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_cache: torch
 
     ``impl`` / ``deterministic`` as for ``cca3d_forward``: the tensor-core path (channels-last frame, channels_last_3d
     caches, S <= 31) where it covers a clip of S + 1 frames, else the generic kernel (contiguous tensors, any Cq and C,
-    H + W + S - 1 <= 2048).  There is no backward: train with ``cca3d(..., causal=True)``."""
+    H + W + S - 1 <= 2048).  There is no backward: train with ``cca3d(..., causal=True)``.
+
+    The caches are a ring of N = k_cache.shape[2] slots: ``frames`` (S, None: N) of them hold past frames, frame j (time
+    order) in slot (head + j) % N.  The defaults are the caches in time order.  A stream over a window of W frames keeps a
+    ring of W slots and overwrites the oldest frame's slot after each step (``CrissCrossAttention3D(..., window=W).step``):
+    frame t, stepped with the last min(t, W) frames, is frame t of ``cca3d_forward(..., causal=True, window=W)``."""
     if torch.is_grad_enabled() and any(t.requires_grad for t in (q, k, v, k_cache, v_cache)):
         raise RuntimeError("ccnet_b200: cca3d_step has no backward (streaming inference); train with "
                            "cca3d(q, k, v, causal=True) on clips")
@@ -596,14 +636,17 @@ def cca3d_step(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_cache: torch
                            f"v{tuple(v.shape)}, got {tuple(k_cache.shape)}, {tuple(v_cache.shape)}")
     if any(t.dtype != q.dtype or t.device != q.device for t in (k_cache, v_cache)):
         raise RuntimeError("ccnet_b200: k_cache, v_cache must match q, k, v in dtype and device")
-    S = k_cache.shape[2]
+    N = k_cache.shape[2]
+    S = N if frames is None else int(frames)
+    if not 0 <= S <= N or (N > 0 and not 0 <= head < N):
+        raise ValueError(f"ccnet_b200: frames must be in [0, {N}] and head in [0, {N}), got frames={frames}, head={head}")
     det = _resolve_deterministic(deterministic)
     lib = capi.load()
     dt = _DTYPES[q.dtype]
     use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc3d_supported(capi.CCA_WS_FORWARD, B, Cq, C, S + 1, H, W, dt) == 1,
                                q, v)
     if use_tc and _upcast(q.dtype, H, W, det, S + 1):
-        out32, lse = cca3d_step(q.float(), k.float(), v.float(), k_cache.float(), v_cache.float(), impl, det)
+        out32, lse = cca3d_step(q.float(), k.float(), v.float(), k_cache.float(), v_cache.float(), impl, det, S, head)
         return out32.to(q.dtype), lse
     cfmt = torch.channels_last_3d if use_tc else torch.contiguous_format
     q, k, v = (t.contiguous(memory_format=fmt) for t in (q, k, v))
@@ -612,8 +655,8 @@ def cca3d_step(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_cache: torch
         out = torch.empty_like(v, memory_format=fmt)
         lse = torch.empty((B, H, W), dtype=torch.float32, device=q.device)
         ws = _workspace(lib.cca_b200_workspace_bytes3d_step(B, Cq, C, S, H, W, dt, flags), q.device)
-        rc = lib.cca_b200_forward3d_step(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_cache.data_ptr() if S else None,
-                                         v_cache.data_ptr() if S else None, out.data_ptr(), lse.data_ptr(), ws.data_ptr(),
-                                         ws.numel(), B, Cq, C, S, H, W, dt, flags, _stream_ptr(q.device))
-        capi.check(rc, "cca_b200_forward3d_step")
+        rc = lib.cca_b200_forward3d_step_ring(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_cache.data_ptr() if S else None,
+                                              v_cache.data_ptr() if S else None, out.data_ptr(), lse.data_ptr(), ws.data_ptr(),
+                                              ws.numel(), B, Cq, C, N, S, head, H, W, dt, flags, _stream_ptr(q.device))
+        capi.check(rc, "cca_b200_forward3d_step_ring")
     return out, lse

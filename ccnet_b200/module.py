@@ -7,6 +7,8 @@ convs (north_star); everything between them and the residual is the CUDA extensi
 """
 from __future__ import annotations
 
+from typing import NamedTuple
+
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -167,6 +169,17 @@ class RCCA(nn.Module):
         return (out, maps) if return_attention else out
 
 
+class RingState(NamedTuple):
+    """The stream state of a windowed ``CrissCrossAttention3D.step``: rings of W slots k [B, Cq, W, H, W_img] and
+    v [B, C, W, H, W_img] holding the keys and values of the last ``frames`` frames, frame j (oldest first) in slot
+    (head + j) % W.  Each step reads the rings and then writes the new frame's k and v into the next free slot or, once the
+    rings are full, the oldest frame's slot: the tensors are updated in place and returned in a new ``RingState``."""
+    k: torch.Tensor
+    v: torch.Tensor
+    frames: int
+    head: int
+
+
 class CrissCrossAttention3D(nn.Module):
     """Criss-cross attention over clips x[B, C, T, H, W]: every position attends to the positions that share two of its
     three coordinates (its column, row and time line; T + H + W - 2 keys), y = gamma * cca3d(q(x), k(x), v(x)) + x.
@@ -178,16 +191,26 @@ class CrissCrossAttention3D(nn.Module):
 
     ``causal=True``: frame t attends to the frames before it only (its column and row as before), for models that run on a
     live stream; the parameters and state-dict keys are those of the bidirectional module.  ``step`` then produces one new
-    frame from a cache of the past frames' keys and values."""
+    frame from a cache of the past frames' keys and values.
 
-    def __init__(self, in_dim: int, impl: str = "auto", causal: bool = False):
+    ``window=W`` (causal only): frame t attends to the frames t - W .. t - 1 only, in ``forward`` as in ``step``, so a model
+    trains on clips of any length with the key sets it streams with; ``step`` then keeps a ring of W frames (``RingState``)."""
+
+    def __init__(self, in_dim: int, impl: str = "auto", causal: bool = False, window=None):
         super().__init__()
+        if window is not None:
+            if not causal:
+                raise ValueError("CrissCrossAttention3D: a time window needs causal=True")
+            if isinstance(window, bool) or int(window) != window or window < 1:
+                raise ValueError(f"CrissCrossAttention3D: window must be an integer >= 1 or None, got {window!r}")
+            window = int(window)
         self.query_conv = nn.Conv3d(in_channels=in_dim, out_channels=in_dim // 8, kernel_size=1)
         self.key_conv = nn.Conv3d(in_channels=in_dim, out_channels=in_dim // 8, kernel_size=1)
         self.value_conv = nn.Conv3d(in_channels=in_dim, out_channels=in_dim, kernel_size=1)
         self.gamma = nn.Parameter(torch.zeros(1))
         self.impl = impl
         self.causal = causal
+        self.window = window
 
     def forward(self, x: torch.Tensor, return_attention: bool = False):
         """``return_attention=True`` returns ``(y, attn)``: y exactly as without it, and the attention map
@@ -198,7 +221,7 @@ class CrissCrossAttention3D(nn.Module):
         if not return_attention:
             return y
         q, k = self.query_conv(x), self.key_conv(x)
-        return y, torch.ops.cca.attention3d(q, k, self.impl, self.causal)
+        return y, torch.ops.cca.attention3d(q, k, self.impl, self.causal, self.window or 0)
 
     def _step(self, x: torch.Tensor) -> torch.Tensor:
         if not x.is_cuda:
@@ -214,10 +237,10 @@ class CrissCrossAttention3D(nn.Module):
             q, k, v = self.query_conv(x), self.key_conv(x), self.value_conv(x)
         if q.dtype != v.dtype or k.dtype != v.dtype:       # autocast corner: keep one dtype
             q, k = q.to(v.dtype), k.to(v.dtype)
-        return torch.addcmul(x, self.gamma, cca3d(q, k, v, self.impl, causal=self.causal))
+        return torch.addcmul(x, self.gamma, cca3d(q, k, v, self.impl, causal=self.causal, window=self.window))
 
     @torch.no_grad()
-    def step(self, x_t: torch.Tensor, state=None, max_frames: int = 31):
+    def step(self, x_t: torch.Tensor, state=None, max_frames=None):
         """One frame of a stream through the causal module: x_t [B, C, H, W] -> (y_t, state).  ``state`` (None for the first
         frame) holds the keys and values of up to ``max_frames`` previous frames in time order; pass the returned one with the
         next frame.  q, k, v of the frame are the Conv3d projections applied as 1x1 convs, y_t = gamma * out + x_t.
@@ -225,12 +248,22 @@ class CrissCrossAttention3D(nn.Module):
         Frame by frame, ``step`` gives the frames of ``forward(clip)`` while the clip has at most ``max_frames + 1`` frames;
         after that the window slides, and y_t is the last frame of the causal forward on the last ``max_frames + 1`` frames.
         The cost is the 2D op on one frame plus a time pass over the cached frames, instead of the whole window again, plus a
-        copy of the cache: each call writes a new one with the new frame's k, v appended.  Inference only (no gradient)."""
+        copy of the cache: each call writes a new one with the new frame's k, v appended.  Inference only (no gradient).
+        ``max_frames`` defaults to 31.
+
+        On a module with ``window=W`` the state is a ``RingState`` of W slots, allocated by the first call and then updated
+        in place, with no cache copy; frame by frame, ``step`` gives the frames of ``forward(clip)`` for clips of any
+        length.  ``max_frames`` must then be left unset or equal W."""
         if not self.causal:
             raise RuntimeError("ccnet_b200.CrissCrossAttention3D.step needs a causal module: CrissCrossAttention3D(in_dim, "
                                "causal=True); a bidirectional frame attends to future frames")
+        if self.window is not None and max_frames is not None and max_frames != self.window:
+            raise ValueError(f"max_frames of a windowed module is its window ({self.window}), got {max_frames}")
         if not x_t.is_cuda:
             raise RuntimeError("ccnet_b200.CrissCrossAttention3D runs on CUDA (H100, sm_90) only")
+        if self.window is not None:
+            return self._ring_step(x_t, state)
+        max_frames = 31 if max_frames is None else max_frames
         if max_frames < 0:
             raise ValueError("max_frames must be >= 0")
         B, C, H, W = x_t.shape
@@ -251,6 +284,28 @@ class CrissCrossAttention3D(nn.Module):
         y = torch.addcmul(x_t, self.gamma.to(out.dtype), out)
         fmt = torch.channels_last_3d if tc else torch.contiguous_format
         return y, (_append_frame(k_cache, k, max_frames, fmt), _append_frame(v_cache, v, max_frames, fmt))
+
+    def _ring_step(self, x_t: torch.Tensor, state):
+        B, C, H, W = x_t.shape
+        N = self.window
+        # the family and layout of the full ring (S = N), for every step of the stream: the rings are never converted
+        tc = self.impl != "simt" and tc3d_eligible(B, C // 8, C, N + 1, H, W, x_t.dtype)
+        if tc:
+            x_t = x_t.contiguous(memory_format=torch.channels_last)
+        q, k, v = (F.conv2d(x_t, conv.weight.squeeze(-1), conv.bias) for conv in (self.query_conv, self.key_conv, self.value_conv))
+        if q.dtype != v.dtype or k.dtype != v.dtype:       # autocast corner: keep one dtype
+            q, k = q.to(v.dtype), k.to(v.dtype)
+        if state is None:
+            fmt = torch.channels_last_3d if tc else torch.contiguous_format
+            ring = lambda t: torch.empty((B, t.shape[1], N, H, W), dtype=t.dtype, device=t.device, memory_format=fmt)
+            state = RingState(ring(k), ring(v), 0, 0)
+        kr, vr, S, head = state
+        out, _ = cca3d_step(q, k, v, kr, vr, "tc" if tc or self.impl == "tc" else "simt", frames=S, head=head)
+        y = torch.addcmul(x_t, self.gamma.to(out.dtype), out)
+        slot = (head + S) % N                              # the next free slot, or the oldest frame's once the ring is full
+        kr[:, :, slot].copy_(k)
+        vr[:, :, slot].copy_(v)
+        return y, RingState(kr, vr, S + 1, head) if S < N else RingState(kr, vr, N, (head + 1) % N)
 
 
 def _append_frame(cache: torch.Tensor, x: torch.Tensor, keep: int, fmt) -> torch.Tensor:

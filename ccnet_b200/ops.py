@@ -11,7 +11,9 @@
     torch.ops.cca.attention3d_backward(dattn, attn, q, k) -> (dq, dk)
     torch.ops.cca.forward3d_step(q, k, v, k_cache, v_cache) -> (out, lse)  one new frame of the causal 3D op (inference)
 
-The 3D ops take a trailing ``causal: bool = False`` (CCA_FLAG_CAUSAL: the time keys of frame t are the frames before it).
+The 3D ops take a trailing ``causal: bool = False`` (CCA_FLAG_CAUSAL: the time keys of frame t are the frames before it) and
+``window: int = 0`` (with causal: the frames t - window .. t - 1 only; 0 is every past frame).  ``forward3d_step`` takes
+``frames: int = -1, head: int = 0``: the caches are a ring whose slot (head + j) % N holds past frame j (-1: all N slots).
 
 CUDA implementations call the C ABI (ccnet_b200.functional -> libcca_b200.so); FakeTensor ("meta") implementations give
 shapes / dtypes / memory formats so that ``torch.compile`` and ``torch.export`` trace through ``networks/ccnet.py`` without a
@@ -149,12 +151,13 @@ attention.register_autograd(_attn_backward, setup_context=_attn_setup)
 # ---- criss-cross attention over clips:  forward3d(q, k, v) -> (out, lse[B,T,H,W]),  backward3d(...) -> (dq, dk, dv)
 #      (channels_last_3d results on the tensor-core path, contiguous ones on the generic kernels)
 @torch.library.custom_op("cca::forward3d", mutates_args=(), device_types="cuda")
-def forward3d(q: Tensor, k: Tensor, v: Tensor, causal: bool = False) -> Tuple[Tensor, Tensor]:
-    return F_.cca3d_forward(q, k, v, causal=causal)
+def forward3d(q: Tensor, k: Tensor, v: Tensor, causal: bool = False, window: int = 0) -> Tuple[Tensor, Tensor]:
+    return F_.cca3d_forward(q, k, v, causal=causal, window=window or None)
 
 
 @forward3d.register_fake
-def _(q, k, v, causal=False):
+def _(q, k, v, causal=False, window=0):
+    F_._time_window(causal, window or None)
     B, Cq, T, H, W = q.shape
     fmt = torch.channels_last_3d if F_.tc3d_eligible(B, Cq, v.shape[1], T, H, W, q.dtype) else torch.contiguous_format
     return torch.empty(v.shape, dtype=v.dtype, device=v.device).contiguous(memory_format=fmt), \
@@ -163,28 +166,29 @@ def _(q, k, v, causal=False):
 
 @torch.library.custom_op("cca::backward3d", mutates_args=(), device_types="cuda")
 def backward3d(dout: Tensor, q: Tensor, k: Tensor, v: Tensor, out: Tensor, lse: Tensor,
-               causal: bool = False) -> Tuple[Tensor, Tensor, Tensor]:
-    return F_.cca3d_backward(dout, q, k, v, out, lse, causal=causal)
+               causal: bool = False, window: int = 0) -> Tuple[Tensor, Tensor, Tensor]:
+    return F_.cca3d_backward(dout, q, k, v, out, lse, causal=causal, window=window or None)
 
 
 @backward3d.register_fake
-def _(dout, q, k, v, out, lse, causal=False):
+def _(dout, q, k, v, out, lse, causal=False, window=0):
     fmt = torch.channels_last_3d if out.is_contiguous(memory_format=torch.channels_last_3d) and out.dim() == 5 else torch.contiguous_format
     mk = lambda t: torch.empty(t.shape, dtype=t.dtype, device=t.device).contiguous(memory_format=fmt)
     return mk(q), mk(k), mk(v)
 
 
 def _fwd3d_setup(ctx, inputs, output):
-    q, k, v, causal = inputs
+    q, k, v, causal, window = inputs
     out, lse = output
     ctx.save_for_backward(q, k, v, out, lse)
     ctx.causal = causal
+    ctx.window = window
 
 
 def _fwd3d_backward(ctx, dout, dlse):
     q, k, v, out, lse = ctx.saved_tensors
-    dq, dk, dv = torch.ops.cca.backward3d(dout.contiguous(), q, k, v, out, lse, ctx.causal)
-    return dq, dk, dv, None
+    dq, dk, dv = torch.ops.cca.backward3d(dout.contiguous(), q, k, v, out, lse, ctx.causal, ctx.window)
+    return dq, dk, dv, None, None
 
 
 forward3d.register_autograd(_fwd3d_backward, setup_context=_fwd3d_setup)
@@ -193,24 +197,25 @@ forward3d.register_autograd(_fwd3d_backward, setup_context=_fwd3d_setup)
 # ---- the attention map over clips:  attention3d(q, k) -> attn[B,T,H,W,H+W+T] fp32,
 #      attention3d_backward(dattn, attn, q, k) -> (dq, dk)
 @torch.library.custom_op("cca::attention3d", mutates_args=(), device_types="cuda")
-def attention3d(q: Tensor, k: Tensor, impl: str = "auto", causal: bool = False) -> Tensor:
-    return F_.cca3d_attention_forward(q, k, impl, causal=causal)
+def attention3d(q: Tensor, k: Tensor, impl: str = "auto", causal: bool = False, window: int = 0) -> Tensor:
+    return F_.cca3d_attention_forward(q, k, impl, causal=causal, window=window or None)
 
 
 @attention3d.register_fake
-def _(q, k, impl="auto", causal=False):
+def _(q, k, impl="auto", causal=False, window=0):
+    F_._time_window(causal, window or None)
     B, _, T, H, W = q.shape
     return q.new_empty((B, T, H, W, H + W + T), dtype=torch.float32)
 
 
 @torch.library.custom_op("cca::attention3d_backward", mutates_args=(), device_types="cuda")
 def attention3d_backward(dattn: Tensor, attn: Tensor, q: Tensor, k: Tensor, impl: str = "auto",
-                         causal: bool = False) -> Tuple[Tensor, Tensor]:
-    return F_.cca3d_attention_backward(dattn, attn, q, k, impl, causal=causal)
+                         causal: bool = False, window: int = 0) -> Tuple[Tensor, Tensor]:
+    return F_.cca3d_attention_backward(dattn, attn, q, k, impl, causal=causal, window=window or None)
 
 
 @attention3d_backward.register_fake
-def _(dattn, attn, q, k, impl="auto", causal=False):
+def _(dattn, attn, q, k, impl="auto", causal=False, window=0):
     B, Cq, T, H, W = q.shape
     cl = impl != "simt" and F_.attention3d_tc_eligible(B, Cq, T, H, W, q.dtype)
     fmt = torch.channels_last_3d if cl else torch.contiguous_format
@@ -219,32 +224,36 @@ def _(dattn, attn, q, k, impl="auto", causal=False):
 
 
 def _attn3d_setup(ctx, inputs, output):
-    q, k, impl, causal = inputs
+    q, k, impl, causal, window = inputs
     ctx.save_for_backward(q, k, output)
     ctx.impl = impl
     ctx.causal = causal
+    ctx.window = window
 
 
 def _attn3d_backward(ctx, dattn):
     q, k, attn = ctx.saved_tensors
-    dq, dk = torch.ops.cca.attention3d_backward(dattn.contiguous(), attn, q, k, ctx.impl, ctx.causal)
-    return dq, dk, None, None
+    dq, dk = torch.ops.cca.attention3d_backward(dattn.contiguous(), attn, q, k, ctx.impl, ctx.causal, ctx.window)
+    return dq, dk, None, None, None
 
 
 attention3d.register_autograd(_attn3d_backward, setup_context=_attn3d_setup)
 
 
 # ---- the streaming step of the causal 3D op:  forward3d_step(q, k, v, k_cache, v_cache) -> (out[B,C,H,W], lse[B,H,W])
-#      (channels-last out on the tensor-core path, contiguous on the generic kernel; no autograd: inference only)
+#      (channels-last out on the tensor-core path, contiguous on the generic kernel; no autograd: inference only).  The caches
+#      are a ring: frames (-1: all N slots) past frames, frame j in slot (head + j) % N
 @torch.library.custom_op("cca::forward3d_step", mutates_args=(), device_types="cuda")
-def forward3d_step(q: Tensor, k: Tensor, v: Tensor, k_cache: Tensor, v_cache: Tensor) -> Tuple[Tensor, Tensor]:
-    return F_.cca3d_step(q, k, v, k_cache, v_cache)
+def forward3d_step(q: Tensor, k: Tensor, v: Tensor, k_cache: Tensor, v_cache: Tensor, frames: int = -1,
+                   head: int = 0) -> Tuple[Tensor, Tensor]:
+    return F_.cca3d_step(q, k, v, k_cache, v_cache, frames=None if frames < 0 else frames, head=head)
 
 
 @forward3d_step.register_fake
-def _(q, k, v, k_cache, v_cache):
+def _(q, k, v, k_cache, v_cache, frames=-1, head=0):
     B, Cq, H, W = q.shape
-    cl = F_.tc3d_eligible(B, Cq, v.shape[1], k_cache.shape[2] + 1, H, W, q.dtype)
+    S = k_cache.shape[2] if frames < 0 else frames
+    cl = F_.tc3d_eligible(B, Cq, v.shape[1], S + 1, H, W, q.dtype)
     fmt = torch.channels_last if cl else torch.contiguous_format
     return torch.empty(v.shape, dtype=v.dtype, device=v.device).contiguous(memory_format=fmt), \
         torch.empty((B, H, W), dtype=torch.float32, device=q.device)

@@ -233,6 +233,8 @@ CCA_API int cca_b200_backward3d(const void *dout, const void *q, const void *k, 
  * map keeps its layout [B,T,H,W,H+W+T]; entries H+W+s with s >= t are exactly 0.  Same coverage, workspace, deterministic
  * mode and limits as without the flag.
  *
+ * Time windows of causal mode and the ring-buffer step: the *_window and *_step_ring entry points below.
+ *
  * Streaming step: frame S of the causal forward, from the new frame and caches of the S previous frames' keys and values
  * (the queries of past frames do not enter).  q, k [B,Cq,H,W] and v, out [B,C,H,W] of the new frame, k_cache [B,Cq,S,H,W],
  * v_cache [B,C,S,H,W] in time order, lse [B,H,W] fp32.  out and lse equal frame S of cca_b200_forward3d with CCA_FLAG_CAUSAL
@@ -250,6 +252,43 @@ CCA_API size_t cca_b200_workspace_bytes3d_step(int B, int Cq, int C, int S, int 
 CCA_API int cca_b200_forward3d_step(const void *q, const void *k, const void *v, const void *k_cache, const void *v_cache,
                                     void *out, float *lse, void *workspace, size_t workspace_bytes,
                                     int B, int Cq, int C, int S, int H, int W, int dtype, unsigned flags, void *cuda_stream);
+
+/*
+ * Time windows of causal mode: the *_window entry points are the ones above with an `int window` before dtype.  window = W
+ * >= 1 (with CCA_FLAG_CAUSAL only) limits the time keys of frame t to the frames t - W <= s < t; window = 0 is every past
+ * frame (the entry points without the suffix are these with window 0).  The map keeps its layout; a time entry outside
+ * [t - W, t) is exactly 0.  With W >= T - 1 the results are bit for bit those of window 0.  The tensor-core coverage is
+ * unchanged (1 <= T <= 32); the generic kernels take H + W_img - 1 + min(W, T - 1) <= 2048 (the time keys of a pixel), so a
+ * windowed clip may be as long as memory allows.  Workspace: cca_b200_workspace_bytes3d / _attention_workspace_bytes3d.
+ * window < 0, or window > 0 without CCA_FLAG_CAUSAL, is CCA_ERR_INVALID, returned before any CUDA call.
+ *
+ * Ring-buffer step: cca_b200_forward3d_step on rings of N slots, k_ring [B,Cq,N,H,W], v_ring [B,C,N,H,W] (NDHWC with
+ * CCA_FLAG_NHWC), holding S <= N past frames, frame j (time order) in slot (head + j) % N.  cca_b200_forward3d_step is this
+ * call with N = S, head = 0.  A stream over a window of W frames keeps N = W slots and writes each new frame's k and v into
+ * the slot of the oldest one: frame t of the stream, stepped with the min(t, W) frames before it, is frame t of the windowed
+ * clip forward (bit for bit where cca_b200_forward3d_step is).  S > N, head outside [0, N) when N > 0 and NULL rings with
+ * S > 0 are CCA_ERR_INVALID.  Callers detect these entry points by the presence of their symbols.
+ */
+CCA_API int cca_b200_forward3d_window(const void *q, const void *k, const void *v, void *out, float *lse,
+                                      void *workspace, size_t workspace_bytes,
+                                      int B, int Cq, int C, int T, int H, int W, int window, int dtype, unsigned flags,
+                                      void *cuda_stream);
+CCA_API int cca_b200_backward3d_window(const void *dout, const void *q, const void *k, const void *v,
+                                       const void *out, const float *lse, void *dq, void *dk, void *dv,
+                                       void *workspace, size_t workspace_bytes,
+                                       int B, int Cq, int C, int T, int H, int W, int window, int dtype, unsigned flags,
+                                       void *cuda_stream);
+CCA_API int cca_b200_attention_forward3d_window(const void *q, const void *k, float *attn, void *workspace, size_t workspace_bytes,
+                                                int B, int Cq, int T, int H, int W, int window, int dtype, unsigned flags,
+                                                void *cuda_stream);
+CCA_API int cca_b200_attention_backward3d_window(const float *dattn, const float *attn, const void *q, const void *k, void *dq,
+                                                 void *dk, void *workspace, size_t workspace_bytes,
+                                                 int B, int Cq, int T, int H, int W, int window, int dtype, unsigned flags,
+                                                 void *cuda_stream);
+CCA_API int cca_b200_forward3d_step_ring(const void *q, const void *k, const void *v, const void *k_ring, const void *v_ring,
+                                         void *out, float *lse, void *workspace, size_t workspace_bytes,
+                                         int B, int Cq, int C, int N, int S, int head, int H, int W, int dtype, unsigned flags,
+                                         void *cuda_stream);
 
 /*
  * The attention map of the 3D op above and its gradient:
