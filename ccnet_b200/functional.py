@@ -73,7 +73,8 @@ def _check_saved(q, v, dout, out, lse):
 def _plan(impl: str, det: bool, covered, q, v=None, causal: bool = False):
     """(use_tc, flags, memory format) of a call: the tensor-core kernels on channels-last memory where ``covered()``, the
     op's coverage query, says they take the shape and ``impl`` allows them, else the generic kernels on contiguous memory.
-    impl="tc" on a shape the tensor-core kernels do not cover raises.  ``causal`` adds CCA_FLAG_CAUSAL (3D ops)."""
+    impl="tc" on a shape the tensor-core kernels do not cover raises.  ``causal`` adds CCA_FLAG_CAUSAL (3D ops).  The real
+    calls and the fake implementations of ``ccnet_b200.ops`` both take their memory format from here."""
     use_tc = impl in ("auto", "tc") and covered()
     if impl == "tc" and not use_tc:
         shapes = f"q{tuple(q.shape)}" + ("" if v is None else f" v{tuple(v.shape)}")
@@ -82,6 +83,31 @@ def _plan(impl: str, det: bool, covered, q, v=None, causal: bool = False):
              | (capi.CCA_FLAG_CAUSAL if causal else 0))
     fmt = (torch.channels_last_3d if q.dim() == 5 else torch.channels_last) if use_tc else torch.contiguous_format
     return use_tc, flags, fmt
+
+
+# The coverage queries of the ops for ``_plan``, evaluated only when ``impl`` allows the tensor-core kernels.
+def _covered(which, q, v):
+    """the 2D op (``which``: CCA_WS_FORWARD or CCA_WS_BACKWARD) on q [B,Cq,H,W], v [B,C,H,W]"""
+    B, Cq, H, W = q.shape
+    return lambda: (q.dtype in _DTYPES
+                    and capi.load().cca_b200_tc_supported(which, B, Cq, v.shape[1], H, W, _DTYPES[q.dtype]) == 1)
+
+
+def _attention_covered(q):
+    """the 2D map on q [B,Cq,H,W]"""
+    return lambda: attention_tc_eligible(*q.shape, q.dtype)
+
+
+def _covered3d(which, q, v, T: int):
+    """the 3D op on a clip of T frames: q [B,Cq,T,H,W], or the new frame [B,Cq,H,W] of a step with T = S + 1"""
+    B, Cq, H, W = q.shape[0], q.shape[1], q.shape[-2], q.shape[-1]
+    return lambda: (q.dtype in _DTYPES
+                    and capi.load().cca_b200_tc3d_supported(which, B, Cq, v.shape[1], T, H, W, _DTYPES[q.dtype]) == 1)
+
+
+def _attention_covered3d(q):
+    """the 3D map on q [B,Cq,T,H,W]"""
+    return lambda: attention3d_tc_eligible(*q.shape, q.dtype)
 
 
 def _time_window(causal: bool, window) -> int:
@@ -178,7 +204,7 @@ def cca_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "
     B, Cq, H, W = q.shape
     C = v.shape[1]
     dt = _DTYPES[q.dtype]
-    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc_supported(capi.CCA_WS_FORWARD, B, Cq, C, H, W, dt) == 1, q, v)
+    use_tc, flags, fmt = _plan(impl, det, _covered(capi.CCA_WS_FORWARD, q, v), q, v)
     if use_tc and _upcast(q.dtype, H, W, det):
         out32, lse = cca_forward(q.float(), k.float(), v.float(), impl, det)
         return out32.to(q.dtype), lse
@@ -206,7 +232,7 @@ def cca_backward(dout, q, k, v, out, lse, impl: str = "auto", want_delta: bool =
     B, Cq, H, W = q.shape
     C = v.shape[1]
     dt = _DTYPES[q.dtype]
-    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc_supported(capi.CCA_WS_BACKWARD, B, Cq, C, H, W, dt) == 1, q, v)
+    use_tc, flags, fmt = _plan(impl, det, _covered(capi.CCA_WS_BACKWARD, q, v), q, v)
     if use_tc and _upcast(q.dtype, H, W, det):
         res = cca_backward(dout.float(), q.float(), k.float(), v.float(), out.float(), lse, impl, want_delta, det)
         return tuple(g.to(q.dtype) for g in res[:3]) + tuple(res[3:])
@@ -315,26 +341,11 @@ def qkv_project_wgrad(x, dq, dk, dv, scale=None, deterministic=None):
     return dwq, db[:Cq], dwk, db[Cq:2 * Cq], dwv, db[2 * Cq:]
 
 
-class _CCAFunction(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, q, k, v, impl, deterministic):
-        out, lse = cca_forward(q, k, v, impl, deterministic)
-        ctx.save_for_backward(q, k, v, out, lse)
-        ctx.impl = impl
-        ctx.deterministic = deterministic
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        q, k, v, out, lse = ctx.saved_tensors
-        dq, dk, dv = cca_backward(dout, q, k, v, out, lse, ctx.impl, deterministic=ctx.deterministic)
-        return dq, dk, dv, None, None
-
-
 def cca(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", deterministic=None) -> torch.Tensor:
     """Differentiable criss-cross attention step (out only).  ``deterministic``: as for ``cca_forward``; the mode is fixed
     when the forward runs and the backward uses it too."""
-    return _CCAFunction.apply(q, k, v, impl, _resolve_deterministic(deterministic))
+    _check_inputs(q, k, v)
+    return torch.ops.cca.forward(q, k, v, impl, _resolve_deterministic(deterministic))[0]
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -356,7 +367,7 @@ def cca_attention_forward(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", 
     lib = capi.load()
     B, Cq, H, W = q.shape
     dt = _DTYPES[q.dtype]
-    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_attention_tc_supported(B, Cq, H, W, dt) == 1, q)
+    use_tc, flags, fmt = _plan(impl, det, _attention_covered(q), q)
     q, k = (t.contiguous(memory_format=fmt) for t in (q, k))
     with torch.cuda.device(q.device):
         attn = torch.empty((B, H, W, H + W), dtype=torch.float32, device=q.device)
@@ -379,7 +390,7 @@ def cca_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministic=
         if t.dtype != torch.float32 or tuple(t.shape) != (B, H, W, H + W) or t.device != q.device:
             raise RuntimeError(f"ccnet_b200: {name} must be a float32 [B,H,W,H+W] tensor on the device of q, k")
     dt = _DTYPES[q.dtype]
-    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_attention_tc_supported(B, Cq, H, W, dt) == 1, q)
+    use_tc, flags, fmt = _plan(impl, det, _attention_covered(q), q)
     if use_tc and _upcast(q.dtype, H, W, det):
         dq, dk = cca_attention_backward(dattn, attn, q.float(), k.float(), impl, det)
         return dq.to(q.dtype), dk.to(q.dtype)
@@ -393,26 +404,11 @@ def cca_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministic=
     return dq, dk
 
 
-class _CCAAttentionFunction(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, q, k, impl, deterministic):
-        attn = cca_attention_forward(q, k, impl, deterministic)
-        ctx.save_for_backward(q, k, attn)
-        ctx.impl = impl
-        ctx.deterministic = deterministic
-        return attn
-
-    @staticmethod
-    def backward(ctx, dattn):
-        q, k, attn = ctx.saved_tensors
-        dq, dk = cca_attention_backward(dattn, attn, q, k, ctx.impl, ctx.deterministic)
-        return dq, dk, None, None
-
-
 def cca_attention(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", deterministic=None) -> torch.Tensor:
     """Differentiable attention map attn[B,H,W,H+W] (float32) of one criss-cross step; the gradient flows to q and k.
     ``deterministic``: as for ``cca``; the mode is fixed when the forward runs and the backward uses it too."""
-    return _CCAAttentionFunction.apply(q, k, impl, _resolve_deterministic(deterministic))
+    _check_inputs(q, k)
+    return torch.ops.cca.attention(q, k, impl, _resolve_deterministic(deterministic))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -448,8 +444,7 @@ def cca3d_forward(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str =
     B, Cq, T, H, W = q.shape
     C = v.shape[1]
     dt = _DTYPES[q.dtype]
-    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc3d_supported(capi.CCA_WS_FORWARD, B, Cq, C, T, H, W, dt) == 1,
-                               q, v, causal)
+    use_tc, flags, fmt = _plan(impl, det, _covered3d(capi.CCA_WS_FORWARD, q, v, T), q, v, causal)
     if use_tc and _upcast(q.dtype, H, W, det, T):
         out32, lse = cca3d_forward(q.float(), k.float(), v.float(), impl, det, causal, window)
         return out32.to(q.dtype), lse
@@ -473,8 +468,7 @@ def cca3d_backward(dout, q, k, v, out, lse, impl: str = "auto", deterministic=No
     B, Cq, T, H, W = q.shape
     C = v.shape[1]
     dt = _DTYPES[q.dtype]
-    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc3d_supported(capi.CCA_WS_BACKWARD, B, Cq, C, T, H, W, dt) == 1,
-                               q, v, causal)
+    use_tc, flags, fmt = _plan(impl, det, _covered3d(capi.CCA_WS_BACKWARD, q, v, T), q, v, causal)
     if use_tc and _upcast(q.dtype, H, W, det, T):
         res = cca3d_backward(dout.float(), q.float(), k.float(), v.float(), out.float(), lse, impl, det, causal, window)
         return tuple(g.to(q.dtype) for g in res)
@@ -489,30 +483,13 @@ def cca3d_backward(dout, q, k, v, out, lse, impl: str = "auto", deterministic=No
     return dq, dk, dv
 
 
-class _CCA3DFunction(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, q, k, v, impl, deterministic, causal, window):
-        out, lse = cca3d_forward(q, k, v, impl, deterministic, causal, window)
-        ctx.save_for_backward(q, k, v, out, lse)
-        ctx.impl = impl
-        ctx.deterministic = deterministic
-        ctx.causal = causal
-        ctx.window = window
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        q, k, v, out, lse = ctx.saved_tensors
-        dq, dk, dv = cca3d_backward(dout, q, k, v, out, lse, ctx.impl, ctx.deterministic, ctx.causal, ctx.window)
-        return dq, dk, dv, None, None, None, None
-
-
 def cca3d(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, impl: str = "auto", deterministic=None,
           causal: bool = False, window=None) -> torch.Tensor:
     """Differentiable criss-cross attention over clips (out only); see ``cca3d_forward``.  The ``causal`` mode and
     ``window`` of the forward are kept for the backward."""
-    _time_window(causal, window)
-    return _CCA3DFunction.apply(q, k, v, impl, _resolve_deterministic(deterministic), bool(causal), window)
+    _check_inputs(q, k, v, rank=5)
+    win = _time_window(causal, window)
+    return torch.ops.cca.forward3d(q, k, v, bool(causal), win, impl, _resolve_deterministic(deterministic))[0]
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -540,7 +517,7 @@ def cca3d_attention_forward(q: torch.Tensor, k: torch.Tensor, impl: str = "auto"
     lib = capi.load()
     B, Cq, T, H, W = q.shape
     dt = _DTYPES[q.dtype]
-    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_attention_tc3d_supported(B, Cq, T, H, W, dt) == 1, q, causal=causal)
+    use_tc, flags, fmt = _plan(impl, det, _attention_covered3d(q), q, causal=causal)
     q, k = (t.contiguous(memory_format=fmt) for t in (q, k))
     with torch.cuda.device(q.device):
         attn = torch.empty((B, T, H, W, H + W + T), dtype=torch.float32, device=q.device)
@@ -564,7 +541,7 @@ def cca3d_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministi
         if t.dtype != torch.float32 or tuple(t.shape) != (B, T, H, W, H + W + T) or t.device != q.device:
             raise RuntimeError(f"ccnet_b200: {name} must be a float32 [B,T,H,W,H+W+T] tensor on the device of q, k")
     dt = _DTYPES[q.dtype]
-    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_attention_tc3d_supported(B, Cq, T, H, W, dt) == 1, q, causal=causal)
+    use_tc, flags, fmt = _plan(impl, det, _attention_covered3d(q), q, causal=causal)
     if use_tc and _upcast(q.dtype, H, W, det, T):
         dq, dk = cca3d_attention_backward(dattn, attn, q.float(), k.float(), impl, det, causal, window)
         return dq.to(q.dtype), dk.to(q.dtype)
@@ -578,31 +555,14 @@ def cca3d_attention_backward(dattn, attn, q, k, impl: str = "auto", deterministi
     return dq, dk
 
 
-class _CCA3DAttentionFunction(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, q, k, impl, deterministic, causal, window):
-        attn = cca3d_attention_forward(q, k, impl, deterministic, causal, window)
-        ctx.save_for_backward(q, k, attn)
-        ctx.impl = impl
-        ctx.deterministic = deterministic
-        ctx.causal = causal
-        ctx.window = window
-        return attn
-
-    @staticmethod
-    def backward(ctx, dattn):
-        q, k, attn = ctx.saved_tensors
-        dq, dk = cca3d_attention_backward(dattn, attn, q, k, ctx.impl, ctx.deterministic, ctx.causal, ctx.window)
-        return dq, dk, None, None, None, None
-
-
 def cca3d_attention(q: torch.Tensor, k: torch.Tensor, impl: str = "auto", deterministic=None,
                     causal: bool = False, window=None) -> torch.Tensor:
     """Differentiable attention map attn[B,T,H,W,H+W+T] (float32) of criss-cross attention over clips; the gradient flows
     to q and k.  ``deterministic``, ``causal`` and ``window``: as for ``cca3d``; they are fixed when the forward runs and
     the backward uses them too."""
-    _time_window(causal, window)
-    return _CCA3DAttentionFunction.apply(q, k, impl, _resolve_deterministic(deterministic), bool(causal), window)
+    _check_inputs(q, k, rank=5)
+    win = _time_window(causal, window)
+    return torch.ops.cca.attention3d(q, k, impl, bool(causal), win, _resolve_deterministic(deterministic))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -643,8 +603,7 @@ def cca3d_step(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_cache: torch
     det = _resolve_deterministic(deterministic)
     lib = capi.load()
     dt = _DTYPES[q.dtype]
-    use_tc, flags, fmt = _plan(impl, det, lambda: lib.cca_b200_tc3d_supported(capi.CCA_WS_FORWARD, B, Cq, C, S + 1, H, W, dt) == 1,
-                               q, v)
+    use_tc, flags, fmt = _plan(impl, det, _covered3d(capi.CCA_WS_FORWARD, q, v, S + 1), q, v)
     if use_tc and _upcast(q.dtype, H, W, det, S + 1):
         out32, lse = cca3d_step(q.float(), k.float(), v.float(), k_cache.float(), v_cache.float(), impl, det, S, head)
         return out32.to(q.dtype), lse

@@ -13,10 +13,11 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import ops  # noqa: F401  (torch.ops.cca.attention, attention3d)
+from . import ops  # noqa: F401  (torch.ops.cca, which cca* call)
 
-from .functional import (cca, cca3d, cca3d_step, cca_backward, cca_forward, qkv_gemm_eligible, qkv_project, qkv_project_dgrad,
-                         qkv_project_wgrad, qkv_wgrad_eligible, tc3d_eligible, tc_eligible)
+from .functional import (_time_window, cca, cca3d, cca3d_attention, cca3d_step, cca_attention, cca_backward, cca_forward,
+                         qkv_gemm_eligible, qkv_project, qkv_project_dgrad, qkv_project_wgrad, qkv_wgrad_eligible,
+                         tc3d_eligible, tc_eligible)
 
 
 class _QKVProject(torch.autograd.Function):
@@ -119,7 +120,7 @@ class CrissCrossAttention(nn.Module):
         if not return_attention:
             return y
         q, k = self.query_conv(x), self.key_conv(x)      # functions.py:29,32
-        return y, torch.ops.cca.attention(q, k, self.impl)
+        return y, cca_attention(q, k, self.impl)
 
     def _step(self, x: torch.Tensor) -> torch.Tensor:
         if not x.is_cuda:
@@ -198,12 +199,7 @@ class CrissCrossAttention3D(nn.Module):
 
     def __init__(self, in_dim: int, impl: str = "auto", causal: bool = False, window=None):
         super().__init__()
-        if window is not None:
-            if not causal:
-                raise ValueError("CrissCrossAttention3D: a time window needs causal=True")
-            if isinstance(window, bool) or int(window) != window or window < 1:
-                raise ValueError(f"CrissCrossAttention3D: window must be an integer >= 1 or None, got {window!r}")
-            window = int(window)
+        window = _time_window(causal, window) or None
         self.query_conv = nn.Conv3d(in_channels=in_dim, out_channels=in_dim // 8, kernel_size=1)
         self.key_conv = nn.Conv3d(in_channels=in_dim, out_channels=in_dim // 8, kernel_size=1)
         self.value_conv = nn.Conv3d(in_channels=in_dim, out_channels=in_dim, kernel_size=1)
@@ -221,7 +217,7 @@ class CrissCrossAttention3D(nn.Module):
         if not return_attention:
             return y
         q, k = self.query_conv(x), self.key_conv(x)
-        return y, torch.ops.cca.attention3d(q, k, self.impl, self.causal, self.window or 0)
+        return y, cca3d_attention(q, k, self.impl, causal=self.causal, window=self.window)
 
     def _step(self, x: torch.Tensor) -> torch.Tensor:
         if not x.is_cuda:

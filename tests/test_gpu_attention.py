@@ -289,8 +289,8 @@ def test_tensor_core_module_map_and_gradients_match_the_oracle_module():
 
 def test_torch_ops_opcheck_and_compile_without_graph_break():
     """opcheck on both ops, with the autograd registration of cca::attention.  torch.compile(fullgraph=True) covers what
-    return_attention adds to a step -- the convs and the map op; the module's y path goes through autograd.Functions that
-    dynamo does not trace (INTEGRATION.md section 3), so the module as a whole is not compiled fullgraph here."""
+    return_attention adds to a step -- the convs and the map op; the module picks its y path with a ctypes coverage query
+    that dynamo does not trace (INTEGRATION.md section 3), so the module as a whole is not compiled fullgraph here."""
     dev = _dev()
     q, k, da = (t.to(dev) for t in _inputs((2, 16, 9, 11), torch.float32, seed=8))
     torch.library.opcheck(torch.ops.cca.attention.default, (q, k), test_utils=("test_schema", "test_faketensor"))

@@ -160,3 +160,44 @@ def test_torch_ops_are_registered_with_fake_implementations():
         y, lse2, o2 = torch.ops.cca.forward_residual(q, q, v, v, torch.empty(1, device="cuda"))
         assert y.shape == v.shape and lse2.shape == lse.shape and o2.shape == v.shape
     torch.library.opcheck  # noqa: B018  (present in this torch; the GPU suite runs it on real tensors)
+
+
+def test_differentiable_ops_end_in_their_mode_arguments():
+    """the eight differentiable-op schemas end in the call's mode, impl and deterministic appended after the arguments they
+    had, so positional calls keep their meaning; under FakeTensorMode those calls still work, and impl lands where the
+    fakes read it: impl="tc" on a shape the tensor-core kernels do not cover raises, as the real call does"""
+    from torch._subclasses.fake_tensor import FakeTensorMode
+    mode2d = [("impl", "auto"), ("deterministic", None)]
+    tails = {"forward": mode2d, "backward": mode2d, "attention": mode2d, "attention_backward": mode2d,
+             "forward3d": [("causal", False), ("window", 0)] + mode2d,
+             "backward3d": [("causal", False), ("window", 0)] + mode2d,
+             "attention3d": [("impl", "auto"), ("causal", False), ("window", 0), ("deterministic", None)],
+             "attention3d_backward": [("impl", "auto"), ("causal", False), ("window", 0), ("deterministic", None)]}
+    for name, tail in tails.items():
+        args = getattr(torch.ops.cca, name).default._schema.arguments
+        assert [(a.name, a.default_value) for a in args[-len(tail):]] == tail, name
+        assert str(args[-1].type) == "Optional[bool]" and not any(a.kwarg_only for a in args), name
+    with FakeTensorMode():
+        q = torch.empty(2, 16, 5, 20, 30, device="cuda")
+        v = torch.empty(2, 64, 5, 20, 30, device="cuda")
+        out, lse = torch.ops.cca.forward3d(q, q, v, True, 3)
+        grads = torch.ops.cca.backward3d(out, q, q, v, out, lse, True, 3)
+        attn = torch.ops.cca.attention3d(q, q, "auto", True, 3)
+        dq, dk = torch.ops.cca.attention3d_backward(attn, attn, q, q, "auto", True, 3)
+        o, l = torch.ops.cca.forward3d_step(q[:, :, 0], q[:, :, 0], v[:, :, 0], q, v, 4, 1)
+        assert [t.shape for t in (out, lse, *grads, attn, dq, dk, o, l)] == [
+            v.shape, (2, 5, 20, 30), q.shape, q.shape, v.shape, (2, 5, 20, 30, 55), q.shape, q.shape, v[:, :, 0].shape,
+            (2, 20, 30)]
+        with pytest.raises(ValueError):
+            torch.ops.cca.forward3d(q, q, v, False, 3)
+        # Cq = 8, C = 24: a shape the tensor-core kernels do not cover on any machine
+        q, v = torch.empty(2, 8, 5, 20, 30, device="cuda"), torch.empty(2, 24, 5, 20, 30, device="cuda")
+        out, lse = torch.ops.cca.forward3d(q, q, v, True, 3)
+        attn = torch.ops.cca.attention3d(q, q, "auto", True, 3)
+        o, l = torch.ops.cca.forward(q[:, :, 0], q[:, :, 0], v[:, :, 0])
+        for call in (lambda: torch.ops.cca.forward3d(q, q, v, True, 3, "tc", True),
+                     lambda: torch.ops.cca.backward3d(out, q, q, v, out, lse, True, 3, "tc"),
+                     lambda: torch.ops.cca.attention3d_backward(attn, attn, q, q, "tc", True, 3, False),
+                     lambda: torch.ops.cca.backward(o, q[:, :, 0], q[:, :, 0], v[:, :, 0], o, l, "tc")):
+            with pytest.raises(RuntimeError, match="do not cover"):
+                call()
